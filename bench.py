@@ -62,6 +62,8 @@ def parse_args():
   p.add_argument('--cpu-sample', type=int, default=24000)
   p.add_argument('--no-cpu-baseline', action='store_true')
   p.add_argument('--no-extras', action='store_true', help='skip the fp64-only / K_* / update side measurements')
+  p.add_argument('--dump-outputs', default='', metavar='DIR',
+                 help='after the timed steps, write what the last timed step returned as DIR/<name>.npy (rank 0)')
   return p.parse_args()
 
 
@@ -219,7 +221,7 @@ def workload_config(args, world):
             'parallelism': 'candidate-sharded x%d (posterior replicated)' % world,
             'step': 'build_posterior + score + arg-max',
             'l2': 'explicit L2 flush (512 MB write) before every timed step; per-step working set '
-                  '(W 210 MB + K_* chunk 267 MB) also exceeds the 126 MB L2'}
+                  '(W 210 MB + K_* chunk 267 MB) also exceeds the 50 MB L2'}
   gm = args.global_cands or CONFIGS[args.config][1]
   desc = CONFIGS[args.config][2] % ((gm, n) if args.config == 'c5' else (n, gm))
   return {'workload': desc, 'n_train': n, 'global_candidates': gm,
@@ -310,13 +312,13 @@ def measure_dgemm_peak(torch, dev):
 
 
 def measure_issue_peaks(local):
-  """ tcgen05 kind::i8 and fp64 DMMA issue rates measured in THIS process on THIS GPU (dfb_measure_peak,
+  """ int8 wgmma and fp64 DMMA issue rates measured in THIS process on THIS GPU (dfb_measure_peak,
       csrc/ubench.cu): the roofline denominators MEASURED_PEAKS.json does not carry. """
   import ctypes as C
   from dragonfly_b200 import _lib
   lib = _lib.load()
   out = {}
-  for name, what in [('tcgen05_i8_tops', _lib.DFB_PEAK_TCGEN05_I8), ('dmma_f64_tflops', _lib.DFB_PEAK_DMMA_F64)]:
+  for name, what in [('i8_tops', _lib.DFB_PEAK_I8), ('dmma_f64_tflops', _lib.DFB_PEAK_DMMA_F64)]:
     v = C.c_double(0.0)
     st = lib.dfb_measure_peak(int(local), int(what), C.byref(v))
     out[name] = float(v.value) if st == 0 else None
@@ -331,7 +333,7 @@ def kstar_build_line(prof, n_train, peaks):
   if ms <= 0:
     return None
   gbs = cands * n_train * 8.0 / (ms * 1e-3) * 1e-9
-  hbm = float(peaks.get('hbm_gbs', 6564.2))
+  hbm = float(peaks.get('hbm_gbs', 3350.0))      # else the H100 SXM data-sheet HBM3 bandwidth
   return {'kernel': 'kstar_seg_kernel<Matern, p=2, d=6, ROWS64> (+ cand_prep, mu_reduce) writing fp64 K_* rows', 'achieved_gbs': gbs,
           'achieved_gbs_incl_padding': gbs * npad / n_train,
           'hbm_peak_gbs': hbm, 'frac_of_hbm': gbs / hbm, 'candidates_per_s': cands / (ms * 1e-3),
@@ -399,10 +401,33 @@ class Workload(object):
       best, idx, _ = gp._fused_score(self.acq, self.cands_dev)      # returns after the device is done (16-byte read-back)
       self.local_ms.append(1e3 * (time.perf_counter() - t0))        # this rank's own work, before the collective
       if self.world > 1:
-        dfb_dist.all_reduce_argmax(best, idx + self.rank * self.M, self.dev)
+        best, idx = dfb_dist.all_reduce_argmax(best, idx + self.rank * self.M, self.dev)
+      self.last_out = (gp, {'best_score': best, 'best_index': idx})
+      self.last_local_index = idx - self.rank * self.M
     else:
-      self.operator(gp, 'device')
+      self.last_out = (gp, {'result': self.operator(gp, 'device')})
     return gp
+
+  def dump_outputs(self, out_dir):
+    """ What the last timed step returned (float64 .npy files), plus the posterior's log marginal likelihood, which
+        that step computed on the way.  The inputs are seeded, so two builds can be compared file for file. """
+    gp, res = self.last_out
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'log_marginal_likelihood': gp.compute_log_marginal_likelihood()}
+    for name, val in res.items():
+      if isinstance(val, tuple):              # operators return (point, ...) / (points, indices, ...)
+        for i, v in enumerate(val):
+          arrays['%s_%d' % (name, i)] = v
+      else:
+        arrays[name] = val
+    if 'best_index' in res and 0 <= self.last_local_index < self.M:
+      arrays['best_point'] = self.cands_dev[self.last_local_index]
+    for name, val in arrays.items():
+      if hasattr(val, 'detach'):
+        val = val.detach().cpu().numpy()
+      a = np.asarray(val, dtype=np.float64)
+      assert a.nbytes <= 16 << 20, (name, a.shape)
+      np.save(os.path.join(out_dir, name + '.npy'), a)
 
   def step_e2e(self):
     """ The reference-facing operator with the reference's own host-side candidate draw (NumPy global stream): every
@@ -506,6 +531,9 @@ def run_ours(args):
   launches[0] = 0
   wl.local_ms = []
   t_dev = timed(wl.step_device, args.steps)
+  if args.dump_outputs and rank == 0:
+    wl.dump_outputs(args.dump_outputs)
+  wl.last_out = None
   local_ms = float(np.mean(wl.local_ms)) if wl.local_ms else 0.0
   n_launch = launches[0]
   barrier()
@@ -517,7 +545,7 @@ def run_ours(args):
   if headline:
     wl.step_e2e_device_rng()
     barrier()
-    t_e2e_dev = timed(wl.step_e2e_device_rng, max(2, args.steps // 2))
+    t_e2e_dev = timed(wl.step_e2e_device_rng, args.steps)
     barrier()
   clocks = sampler.stop() if rank == 0 else None
   ms_dev, ms_e2e = float(np.sum(t_dev)), float(np.sum(t_e2e))
@@ -654,38 +682,25 @@ def run_ours(args):
       gemm_ms, gemm_launches, gemm_cands = prof['gemm']
       flops_per_cand = float(N) * float(N + 1)       # triangular W: sum_i 2(i+1) = N(N+1) flops
       fp64_equiv = gemm_cands * flops_per_cand / (gemm_ms * 1e-3) * 1e-12 if gemm_ms > 0 else 0.0
-      traffic = None
-      tpath = os.path.join(ROOT, 'profiles', 'gemm_traffic.json')
-      if os.path.exists(tpath):
-        try:
-          tj = json.load(open(tpath))
-          traffic = tj.get({2: 'dram_bytes_per_launch_i8c2', 1: 'dram_bytes_per_launch_i8x2'}.get(i8_impl, 'dram_bytes_per_launch_i8')
-                           if used_i8 else 'dram_bytes_per_launch')
-        except Exception:  # pylint: disable=broad-except
-          traffic = None
       share = {kname: prof[kname][0] / max(sum(p[0] for p in prof.values()), 1e-9) for kname in prof}
       if used_i8:
-        # dominant kernel: the tcgen05 int8 contraction.  Algorithmic work: one int8 digit product per kept (s, t)
+        # dominant kernel: the int8 wgmma contraction.  Algorithmic work: one int8 digit product per kept (s, t)
         # pair for every fp64 multiply-add of the triangular contraction -- 15 with five radix-256 digits, 21 with
         # six radix-128 digits.
         n_products = 15.0 if i8_r256 else 21.0
         ops_per_cand = n_products * flops_per_cand
         achieved = gemm_cands * ops_per_cand / (gemm_ms * 1e-3) * 1e-12
-        peak = issue.get('tcgen05_i8_tops') or 4577.2
+        peak = issue.get('i8_tops')
         digits = ('five radix-256 digits, 15 exact int8 products' if i8_r256
                   else 'six radix-128 digits, 21 exact int8 products')
-        kname = {2: 'score_i8c2_kernel (persistent 2-CTA clusters; tcgen05.mma.cta_group::2 kind::i8 M256 N128 K32 / '
-                    'UTCIMMA.2CTA, TMEM accumulators, TMA ring)',
-                 1: 'score_i8x2_kernel (persistent, one CTA per SM; tcgen05.mma kind::i8 M128 N128 K32)',
-                 0: 'score_i8_kernel (tcgen05.mma kind::i8 M128 N64 K32)'}[i8_impl]
+        kname = 'score_i8_kernel (wgmma.m64n32k32.s32.s8.s8, register accumulators, TMA + mbarrier ring)'
         line['roofline'] = {
           'bound': 'tensor', 'achieved': achieved, 'peak': peak, 'unit': 'TOP/s (int8)',
-          'frac': achieved / peak, 'traffic': traffic, 'kernel': kname + ': V = L^-1 K_*^T as %s, fused |v|^2' % digits,
+          'frac': achieved / peak if peak else None, 'kernel': kname + ': V = L^-1 K_*^T as %s, fused |v|^2' % digits,
           'int8_products_per_fp64_fma': n_products, 'ops_per_candidate': ops_per_cand,
           'launch_ms_avg': gemm_ms / max(gemm_launches, 1), 'launches_timed': int(gemm_launches),
-          'peak_source': 'tcgen05.mma kind::i8 issue rate (M128 N256 K32 from shared memory) measured live in this run '
-                         'by dfb_measure_peak on this GPU; r01 ubench on this pool: 4577 TOP/s; MEASURED_PEAKS.json bf16 '
-                         'burst = %s TF/s for comparison' % peaks.get('bf16_tflops', 'n/a'),
+          'peak_source': 'int8 wgmma issue rate (m64n256k32 from shared memory) measured live in this run by '
+                         'dfb_measure_peak on this GPU',
           'frac_at_sampled_clock': (achieved / (peak * clocks['sm_mhz'] / clocks['sm_max_mhz'])
                                     if clocks and clocks.get('sm_mhz') else None),
           'fp64_equivalent_tflops': fp64_equiv,
@@ -693,7 +708,7 @@ def run_ours(args):
           'cublas_dgemm_tflops_live': dgemm_peak, 'dmma_issue_peak_tflops_live': issue.get('dmma_f64_tflops'),
           'share_of_scoring': share,
           'i8_sigma2_error_bound': i8_bound, 'argmax_shortlist_rescored_fp64': shortlist}
-        line['dtype'] = ('f64 (sigma^2 contraction screened by an int8 digit expansion of the fp64 operands on tcgen05: '
+        line['dtype'] = ('f64 (sigma^2 contraction screened by an int8 digit expansion of the fp64 operands on wgmma: '
                          'a-priori |d sigma^2| <= %.1e, measured in this run %s over %d candidates; arg-max re-scored in '
                          'fp64 DMMA)' % (i8_bound, ('%.1e' % dsig) if dsig is not None else 'n/a',
                                          extras.get('int8_screen_check', {}).get('candidates', 0)))
@@ -701,7 +716,7 @@ def run_ours(args):
       else:
         line['roofline'] = {
           'bound': 'tensor', 'achieved': fp64_equiv, 'peak': dgemm_peak, 'unit': 'TFLOP/s',
-          'frac': fp64_equiv / dgemm_peak if dgemm_peak > 0 else None, 'traffic': traffic,
+          'frac': fp64_equiv / dgemm_peak if dgemm_peak > 0 else None,
           'kernel': 'score_tma_kernel (fp64 DMMA, TMA + mbarrier ring: V = L^-1 K_*^T fused with |v|^2)',
           'flops_per_candidate': flops_per_cand, 'launch_ms_avg': gemm_ms / max(gemm_launches, 1),
           'launches_timed': int(gemm_launches),

@@ -1,7 +1,7 @@
 """
 ctypes binding of libdfb200.so (include/dfb200.h) -- the only way the Python host reaches the GPU.
 
-There is deliberately NO fallback: if the shared library is missing, or no B200-class CUDA device is
+There is deliberately NO fallback: if the shared library is missing, or no H100 (sm_90) device is
 visible when a handle is created, this module raises.  PyTorch is used only to own device buffers
 (workspace, candidate matrices) and to expose the current CUDA stream.
 """
@@ -22,7 +22,7 @@ DFB_BUILD_FULL, DFB_BUILD_LML_ONLY, DFB_BUILD_NO_ALPHA = 0, 1, 2
 DFB_EXTEND_SAVE = 16
 DFB_MOO_MAX_OBJ = 8
 DFB_RNG_NORMAL, DFB_RNG_UNIFORM = 0, 1
-DFB_PEAK_TCGEN05_I8, DFB_PEAK_DMMA_F64 = 0, 1
+DFB_PEAK_I8, DFB_PEAK_DMMA_F64 = 0, 1
 DFB_MOO_LIN_UCB, DFB_MOO_TCH_UCB, DFB_MOO_LIN_VAL, DFB_MOO_TCH_VAL = 0, 1, 2, 3
 
 
@@ -113,7 +113,7 @@ def load():
     return _lib
   if not os.path.exists(LIB_PATH):
     raise ImportError('dragonfly_b200: %s is missing. Build it with `python -c "import '
-                      '__graft_entry__ as g; g.build()"` (nvcc, sm_100a). There is no CPU '
+                      '__graft_entry__ as g; g.build()"` (nvcc, sm_90a). There is no CPU '
                       'fallback.' % (LIB_PATH))
   lib = C.CDLL(LIB_PATH)
   for name, (restype, argtypes) in PROTOTYPES.items():

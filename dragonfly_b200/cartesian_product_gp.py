@@ -69,7 +69,7 @@ class CPGP(GP):
       domain_lists_of_dists = [None] * kernel.num_kernels
     if any(d is not None for d in domain_lists_of_dists):
       raise NotImplementedError('factors evaluated from precomputed distance lists (kernel.evaluate_from_dists: the '
-                                'neural-network domains) are outside the B200 hot-path scope.')
+                                'neural-network domains) are outside the GPU hot-path scope.')
     self.domain_lists_of_dists = domain_lists_of_dists
     if handle_non_psd_kernels in ('project_first', 'try_before_project'):
       if not kernel.is_guaranteed_psd():
@@ -80,7 +80,7 @@ class CPGP(GP):
 
   def set_domain_lists_of_dists(self, domain_lists_of_dists):
     if any(d is not None for d in domain_lists_of_dists):
-      raise NotImplementedError('precomputed distance lists are outside the B200 hot-path scope.')
+      raise NotImplementedError('precomputed distance lists are outside the GPU hot-path scope.')
     self.domain_lists_of_dists = domain_lists_of_dists
 
   def _train_matrix(self):

@@ -321,8 +321,8 @@ static int prof_end(dfb_handle* h, int cls, double units) {
 // for independent dv_i (|v|^2 <= k(x,x) - sigma^2 <= k(x,x)).  A worst-case (n instead of sqrt(n), aligned signs
 // over i) bound would be ~sqrt(n) n / 8 ~ 4 10^4 times larger at N = 5000 and is as unattainable as LAPACK's own.
 //
-// The constant 8 keeps the bound above every maximum measured over the validation sweep (tools/sweep_i8_bound.py ->
-// profiles/r02_i8_bound_sweep.json: 480 configurations -- N 1024..5000, noise 1e-2..1e-8 of the scale, scale 1e-2..1e4,
+// The constant 8 keeps the bound above every maximum measured over the validation sweep (tools/sweep_i8_bound.py:
+// 480 configurations -- N 1024..5000, noise 1e-2..1e-8 of the scale, scale 1e-2..1e4,
 // SE / Matern-5/2 / Matern-1/2 / additive / product kernels, both digit schemes, 13056 candidates each, guard off): the
 // worst measured / bound ratio is 0.28 (Matern-1/2, N = 1024, radix 256), typically 0.02-0.15; the worst ABSOLUTE error
 // among the 185 configurations the guard admits is 1.05e-9 against the 1e-8 contract.  It is NOT a worst-case bound;
@@ -351,14 +351,14 @@ static bool i8_usable(const dfb_handle* h, const dfb_kernel_desc& desc) {
   return i8_sigma2_bound(h, desc) <= I8_BOUND_LIMIT;
 }
 
-// Digit planes of W = L^-1 for the tcgen05 path + the tensor maps of both operands.
+// Digit planes of W = L^-1 for the int8 wgmma path + the tensor maps of both operands.
 static int prepare_i8(dfb_handle* h) {
   const int64_t npad = h->npad;
   DFB_TRY(launch_row_exponent(h, h->W, npad, npad, npad, h->rowscale, h->rowinv));
   DFB_TRY(launch_vec_max(h, h->rowscale, h->n, h->red + 4));
   DFB_CUDA_OK(cudaMemcpyAsync(&h->i8_rowscale_max, h->red + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  // Digit scheme of the CTA-pair kernel: five radix-256 digits (15 products) when the a-priori bound of
+  // Digit scheme (i8_impl 2): five radix-256 digits (15 products) when the a-priori bound of
   // that coarser expansion passes for the training kernel, else six radix-128 digits (21 products).  The
   // radix-256 groups also need int32 headroom: 5 K 2^14 < 2^31.
   h->i8_radix256 = 0;
@@ -370,23 +370,10 @@ static int prepare_i8(dfb_handle* h) {
   }
   // pair-interleaved digit planes: 3 planes of rows x (2 * npad) bytes
   DFB_TRY(launch_slice_i8(h, h->W, npad, npad, npad, h->rowinv, 0.0, h->Wi8, 2 * npad * npad, 2 * npad));
-  if (h->i8_impl >= 1) {
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK2h, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 64, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK3h, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 64, 3));
-    // compact plane of the leading digit (row-major rows of npad bytes, SWIZZLE_128B boxes of 128 k-values)
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmW1c, h->Wi8 + 6 * npad * npad, npad, npad, 1, npad, npad * npad, 128, 128, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK1c, h->Ki8 + 6 * h->chunk * npad, npad, h->chunk, 1, npad, h->chunk * npad, 128, 64, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK2h_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 64, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK3h_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 64, 3));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK1c_b, h->Ki8b + 6 * h->chunk * npad, npad, h->chunk, 1, npad, h->chunk * npad, 128, 64, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmW2, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 64, 128, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmW3, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 64, 128, 3));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK2, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 128, 1));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmK3, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 128, 3));
-  } else {
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmWi8, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 128, 128, 3));
-    DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 128, 64, 3));
-  }
+  // one K = 32 block of all three planes per TMA box (64 B x rows x 3, SWIZZLE_64B): 128 rows of W, 32 candidates
+  DFB_TRY(make_tensor_map_3d_u8(&h->tmWi8, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 64, 128, 3));
+  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 32, 3));
+  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 32, 3));
   h->i8_ready = true;
   return 0;
 }
@@ -495,7 +482,7 @@ struct ChunkOut {
 // Scores m candidates chunk by chunk: K_* rows + mu -> |L^-1 k_*|^2 -> sd / acquisition / arg-max.
 struct ChunkMode {
   bool want_std, do_argmax;
-  bool use_i8;                 // int8-slice tcgen05 contraction instead of fp64 DMMA
+  bool use_i8;                 // int8-slice wgmma contraction instead of fp64 DMMA
   bool collect;                // gather the shortlist for the exact re-score
   I8ErrModel em;               // int8 error model (collect): bound on |d sigma^2|, score sensitivity
   double pad;                  // extra slack of the shortlist test
@@ -532,9 +519,8 @@ static int ensure_ks_stream(dfb_handle* h) {
 // Per chunk two stages:
 //   K: (host candidates: staging copy) K_* rows / digit planes + mu + k(x*,x*)      fp64 pipe
 //   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
-// With the CTA-pair int8 contraction the stages of consecutive chunks are software-pipelined over two streams: K(c+1)
-// runs on h->ks_stream into the second digit buffer while G(c) runs on the caller's stream (the lean K_* kernel
-// co-resides with the persistent tcgen05 kernel: 88 registers x 128 threads and < 1 KB of shared memory per CTA).
+// With option kstar_overlap and the int8 contraction the stages of consecutive chunks are software-pipelined over two
+// streams: K(c+1) runs on h->ks_stream into the second digit buffer while G(c) runs on the caller's stream.
 // Events carry the two dependencies per buffer: K(c) -> G(c) and G(c) -> K(c+2).  Everything else is unchanged: the
 // arithmetic per chunk, the order of the arg-max folds (G stages stay in stream order) and therefore every result.
 static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
@@ -692,16 +678,8 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
         const double colscale = i8_colscale(desc);
-        if (h->i8_impl == 2)
-          DFB_TRY(launch_score_i8c2_args(h, h->tmW2, h->tmW3, h->tmW1c, b ? h->tmK2h_b : h->tmK2h, b ? h->tmK3h_b : h->tmK3h,
-                                         b ? h->tmK1c_b : h->tmK1c, nb, (int)(m_rows / TILE), (int)npad,
-                                         h->partial, Mc, h->rowscale, colscale, abort_count));
-        else if (h->i8_impl == 1)
-          DFB_TRY(launch_score_i8x2_args(h, h->tmW2, h->tmW3, h->tmK2, h->tmK3, nb, (int)(m_rows / TILE), (int)npad,
-                                         h->partial, Mc, h->rowscale, colscale));
-        else
-          DFB_TRY(launch_score_i8_args(h, h->tmWi8, h->tmKi8, nb, (int)(m_rows / 64), (int)npad, h->partial, Mc,
-                                       h->rowscale, colscale));
+        DFB_TRY(launch_score_i8_args(h, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb, (int)(m_rows / I8_BN), (int)npad,
+                                     h->partial, Mc, h->rowscale, colscale, abort_count));
       } else if (h->gemm_impl == 1 && h->tma_ready) {
         ScoreTmaArgs ta;
         ta.n_rb = g.n_rb; ta.n_cb = g.n_cb; ta.K = g.K; ta.partial = g.partial; ta.ld_partial = g.ld_partial;
@@ -745,7 +723,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     }
   } else {
     // issue order: the contraction of chunk c is enqueued BEFORE the K_* of chunk c+1, so that the block scheduler
-    // places the persistent kernel's CTAs first and the K_* CTAs fill the registers / shared memory left over
+    // places the contraction's CTAs first and the K_* CTAs fill the registers / shared memory left over
     DFB_TRY(stage_k(0));
     for (int64_t ci = 0; ci < n_chunks; ci++) {
       DFB_TRY(stage_g(ci));
@@ -782,8 +760,8 @@ int dfb_create(dfb_handle** out, int device) {
   int cc_major = 0, cc_minor = 0;     // attribute queries: cudaGetDeviceProperties costs milliseconds per call
   DFB_CUDA_OK(cudaDeviceGetAttribute(&cc_major, cudaDevAttrComputeCapabilityMajor, device));
   DFB_CUDA_OK(cudaDeviceGetAttribute(&cc_minor, cudaDevAttrComputeCapabilityMinor, device));
-  if (cc_major < 10) {
-    set_error("device %d is sm_%d%d; libdfb200 is built for sm_100a (B200) only", device, cc_major, cc_minor);
+  if (cc_major != 9 || cc_minor != 0) {
+    set_error("device %d is sm_%d%d; libdfb200 is built for sm_90a (H100) only", device, cc_major, cc_minor);
     return -2;
   }
   dfb_handle* h = new (std::nothrow) dfb_handle();
@@ -791,7 +769,7 @@ int dfb_create(dfb_handle** out, int device) {
   h->device = device;
   const char* impl = getenv("DFB200_GEMM");       // "v1" = cp.async ring, "tma" = TMA + mbarrier ring
   h->gemm_impl = (impl != nullptr && strcmp(impl, "v1") == 0) ? 0 : 1;   // default: TMA ring
-  const char* simpl = getenv("DFB200_SCORE");     // "i8" = int8-slice tcgen05 contraction
+  const char* simpl = getenv("DFB200_SCORE");     // "i8" = int8-slice wgmma contraction
   h->score_impl = 2;                              // auto
   if (simpl != nullptr && strcmp(simpl, "i8") == 0) h->score_impl = 1;
   if (simpl != nullptr && strcmp(simpl, "fp64") == 0) h->score_impl = 0;
@@ -1396,16 +1374,15 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "kstar_fast") == 0) { h->kstar_fast = value ? 1 : 0; return 0; }
   if (strcmp(name, "lookahead") == 0) { h->lookahead = value ? 1 : 0; return 0; }
   if (strcmp(name, "small_eval") == 0) { h->small_eval = value ? 1 : 0; return 0; }
-  if (strcmp(name, "i8_ts") == 0) { h->i8_ts = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_fuse") == 0) { h->i8_fuse = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_seg") == 0) { h->kstar_seg = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_rows64") == 0) { h->kstar_rows64 = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_overlap") == 0) { h->kstar_overlap = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_unguarded") == 0) { h->i8_unguarded = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_impl") == 0) {
-    if (value < 0 || value > 2) { set_error("i8_impl must be 0 (N=64, one pass), 1 (N=128, two passes) or 2 (CTA pairs)"); return -1; }
+    if (value < 0 || value > 2) { set_error("i8_impl must be 0 or 1 (radix-128 digits only) or 2 (digit scheme by i8_radix)"); return -1; }
     h->i8_impl = (int)value;
-    if (h->i8_ready) { DFB_CUDA_OK(cudaSetDevice(h->device)); DFB_TRY(prepare_i8(h)); }   // re-slice W in the new layout
+    if (h->i8_ready) { DFB_CUDA_OK(cudaSetDevice(h->device)); DFB_TRY(prepare_i8(h)); }   // re-slice W in the new scheme
     return 0;
   }
   if (strcmp(name, "i8_radix") == 0) {
@@ -1415,11 +1392,9 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
     return 0;
   }
   if (strcmp(name, "tma_cb_group") == 0 && value >= 1) { h->tma_cb_group = (int)value; return 0; }
-  if (strcmp(name, "i8_cb_group") == 0 && value >= 1) { h->i8_cb_group = (int)value; return 0; }
   if (strcmp(name, "i8_c2_group") == 0 && value >= 0) { h->i8_c2_group = (int)value; return 0; }
-  if (strcmp(name, "i8_l2_hint") == 0 && value >= 0 && value <= 2) { h->i8_l2_hint = (int)value; return 0; }
   if (strcmp(name, "score_impl") == 0) {
-    if (value < 0 || value > 2) { set_error("score_impl must be 0 (fp64 DMMA), 1 (int8-slice tcgen05) or 2 (auto)"); return -1; }
+    if (value < 0 || value > 2) { set_error("score_impl must be 0 (fp64 DMMA), 1 (int8-slice wgmma) or 2 (auto)"); return -1; }
     h->score_impl = (int)value;
     h->i8_ready = false;
     if ((value == 1 || (value == 2 && h->n >= 1024)) && h->have_post && h->have_w) {

@@ -1,4 +1,4 @@
-// Shared declarations for libdfb200.so (sm_100a only).
+// Shared declarations for libdfb200.so (sm_90a: H100).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -9,8 +9,8 @@
 #include <math.h>
 #include "../../include/dfb200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libdfb200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900 || !defined(__CUDA_ARCH_FEAT_SM90_ALL))
+#error "libdfb200 is written for sm_90a (H100) only"
 #endif
 
 namespace dfb {
@@ -111,18 +111,16 @@ struct dfb_handle {
 
   // TMA path of the scoring contraction (gemm_tma.cuh)
   int gemm_impl = 1;          // 0 = v1 cp.async ring, 1 = v2 TMA + mbarrier ring (default)
-  int tma_cb_group = 1 << 20;       // candidate tiles per scheduling group (sweep: no gain, see profiles/)
-  int i8_cb_group = 12;        // int8 kernel: 12 candidate tiles per group keeps W's digits L2-resident (time-neutral, 9x less DRAM traffic)
-  int i8_c2_group = 0;        // pair kernel: candidate tiles per group of its tile order; 0 = chosen by simulation (kernels.cu)
+  int tma_cb_group = 1 << 20;       // candidate tiles per scheduling group (a sweep found no gain)
+  int i8_c2_group = 0;        // int8 kernel: candidate tiles per group of its tile order; 0 = 16 (kernels.cu)
   int last_c2_group = 0;
-  int i8_l2_hint = 0;         // pair kernel: L2 eviction priorities of its TMA loads (kernels.cu: launch_score_i8c2_args)
   int kstar_fast = 1;         // specialised K_* kernel for plain SE / Matern on <= 8 dims
   bool tma_ready = false;
   CUtensorMap tmW;            // W  (npad x npad)
   CUtensorMap tmK;            // Ks (chunk x npad)
 
-  // integer-slice tcgen05 path (gemm_i8.cuh)
-  int score_impl = 2;         // 0 = fp64 DMMA, 1 = int8-slice UTCIMMA everywhere, 2 = auto: int8 pass +
+  // integer-slice wgmma path (gemm_i8.cuh)
+  int score_impl = 2;         // 0 = fp64 DMMA, 1 = int8-slice wgmma everywhere, 2 = auto: int8 pass +
                               // exact fp64 re-score of the shortlist in dfb_score_argmax, fp64 in dfb_eval
   double i8_rowscale_max = 0.0;   // max_i 2^E_i of the current posterior
   int64_t* list_idx = nullptr;    // shortlist (cap entries)
@@ -142,9 +140,8 @@ struct dfb_handle {
   int kstar_seg = 1;          // second-generation digit kernel (kstar_seg_kernel) where it applies
   int kstar_rows64 = 1;       // ... and its fp64-row form for the materialising K_* build of the fp64 scoring paths
   int kstar_overlap = 0;      // option: chunk c+1's K_* on a second stream while chunk c is contracted (api.cu: run_chunks)
-  int i8_ts = 0;              // 1 = A digits staged in tensor memory (tcgen05.cp + TS-form MMA)
-  int8_t* Wi8 = nullptr;      // [6][npad][npad]
-  int8_t* Ki8 = nullptr;      // [6][chunk][npad]
+  int8_t* Wi8 = nullptr;      // 3 pair-interleaved planes [npad][2 npad] + the compact leading plane [npad][npad]
+  int8_t* Ki8 = nullptr;      // the same for the K_* chunk
   // K_* / contraction overlap (api.cu: run_chunks): second buffer of everything the K_* stage hands to the
   // contraction stage, the scratch of the second-generation K_* kernel, the second stream and its events
   int8_t* Ki8b = nullptr;
@@ -153,23 +150,19 @@ struct dfb_handle {
   double* cprep = nullptr;    // chunk x 10 scaled candidate rows (cand_prep_kernel)
   double* mu_part = nullptr;  // (npad / 64 + 2) x chunk
   cudaStream_t ks_stream = nullptr;   // K stage (least priority)
-  cudaStream_t gs_stream = nullptr;   // G stage (greatest priority: the persistent kernel's CTAs are placed first)
+  cudaStream_t gs_stream = nullptr;   // G stage (greatest priority: the contraction's CTAs are placed first)
   cudaEvent_t ks_join = nullptr;
   cudaStream_t cp_stream = nullptr;   // H2D copies of page-locked host candidates, one batch ahead (api.cu: run_chunks)
   cudaEvent_t cp_fork = nullptr, cp_done[2] = {nullptr, nullptr}, cp_free[2] = {nullptr, nullptr};
   cudaEvent_t ks_fork = nullptr, ks_k[2] = {nullptr, nullptr}, ks_g[2] = {nullptr, nullptr};
-  CUtensorMap tmK2h_b, tmK3h_b, tmK1c_b;   // maps of the second digit buffer
+  CUtensorMap tmKi8_b;                     // map of the second digit buffer
   int64_t last_overlapped = 0;             // diagnostics: chunks of the last call that went through the two-stream pipeline
   double* rowscale = nullptr; // npad  2^E_i
   double* rowinv = nullptr;   // npad  2^-E_i
   CUtensorMap tmWi8, tmKi8;
-  int i8_impl = 2;            // 0 = one pass, N = 64 MMAs (gemm_i8.cuh); 1 = two passes, N = 128 (gemm_i8x2.cuh);
-                              // 2 = as 1 with CTA-pair M256 MMAs (gemm_i8c2.cuh)
-  int i8_radix_opt = -1;      // digit scheme of the pair kernel: -1 auto (radix 256 when its bound allows), 0 = 128, 1 = 256
+  int i8_impl = 2;            // 0, 1 = radix-128 digits only; 2 = digit scheme chosen by i8_radix_opt
+  int i8_radix_opt = -1;      // digit scheme with i8_impl 2: -1 auto (radix 256 when its bound allows), 0 = 128, 1 = 256
   int i8_radix256 = 0;        // scheme in use for the current posterior (set by prepare_i8)
-  CUtensorMap tmW1c, tmK1c;             // compact leading-digit planes (pass B of the radix-256 scheme)
-  CUtensorMap tmK2h, tmK3h;             // 64-row boxes of the K_* digit planes (i8_impl 2: half tiles per CTA)
-  CUtensorMap tmW2, tmW3, tmK2, tmK3;   // 2- and 3-plane boxes of the digit planes (i8_impl 1)
 
   // model state
   dfb_kernel_desc desc_tr;

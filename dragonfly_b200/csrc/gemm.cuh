@@ -1,11 +1,11 @@
-// fp64 tensor-core (DMMA.8x8x4) "TN" GEMM for sm_100a:
+// fp64 tensor-core (DMMA.8x8x4) "TN" GEMM for sm_90a:
 //
 //     acc[i][j] = sum_{k in [0, k_hi)} A[i, k] * B[j, k]          (both operands K-contiguous)
 //
 // One CTA = one 128 x 128 output tile, 8 warps (2 x 4), warp tile 64 x 32, K pipelined in slabs of
-// 16 doubles (128 B per row) through a 4-stage cp.async ring in shared memory.  tcgen05 has no f64
-// kind, so the fp64 contraction runs on the legacy warp-level DMMA path (SASS: DMMA.8x8x4), which
-// on B200 issues at the full FP64 rate (64 FMA/clk/SM, measured 37.1 TFLOP/s; tools/ubench_fp64.cu).
+// 16 doubles (128 B per row) through a 4-stage cp.async ring in shared memory.  wgmma has no f64
+// kind, so the fp64 contraction runs on the warp-level DMMA path (SASS: DMMA.8x8x4), the FP64 tensor
+// core rate of the SM (dfb_measure_peak and tools/ubench_fp64.cu measure it).
 //
 // The same core serves every dense contraction of the path through a `mode` (which tiles exist and
 // which k-range each needs) and an epilogue:
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tn_kernel(const GemmArgs
 // Host-side launchers (defined in kernels.cu).  launch_gemm_splitk runs a MODE_GENERIC product with every tile's
 // k-range split over `ksplit` CTAs (scratch: ksplit * n_rb*128 * n_cb*128 doubles at `part`) followed by the
 // fixed-order reduction D = C + sum_s part_s: for the skinny products of dfb_extend_posterior, whose 1..40 tiles
-// would otherwise occupy 1..40 of the 148 SMs for a k-depth of ~N.
+// would otherwise occupy 1..40 of the 132 SMs for a k-depth of ~N.
 int launch_gemm(dfb_handle* h, const GemmArgs& g, int epi, int n_blocks);
 int launch_gemm_splitk(dfb_handle* h, GemmArgs g, int ksplit, double* part);
 

@@ -1,31 +1,32 @@
-// The scoring contraction on the 5th-generation tensor cores: an error-bounded integer-slice
-// (Ozaki-style) evaluation of V = W K_*^T followed by the fused |v|^2 column reduction.
+// The scoring contraction on the Hopper tensor cores: an error-bounded integer-slice (Ozaki-style)
+// evaluation of V = W K_*^T followed by the fused |v|^2 column reduction.
 //
-// tcgen05.mma has no f64 kind, and the fp64 DMMA path tops out at 37 TFLOP/s.  Instead both fp64
-// operands are expanded exactly into S = 6 signed 7-bit digits after a power-of-two scaling
-//     W[i,k]  = 2^E_i  * sum_{s=1..S} a_s[i,k] * 2^(-7s)  (+ rounding < 2^(E_i-43))
-//     K*[m,k] = 2^F    * sum_{t=1..S} b_t[m,k] * 2^(-7t)
-// (|a|,|b| <= 64, int8), so that
-//     V[i,m] = 2^(E_i+F) * sum_{d=2..S+1} 2^(-7d) * G_d[i,m],   G_d = sum_{s+t=d} A_s B_t^T   (int32, exact)
-// All 21 digit products of one K-block are issued as tcgen05.mma.kind::i8 (SASS UTCIMMA) into six
-// int32 accumulators living in tensor memory (6 x 64 columns of TMEM); the epilogue reads them with
-// tcgen05.ld, recombines in fp64, squares and reduces per candidate.  Dropped terms (s+t > S+1) and
-// the digit truncation are < 2^-42 relative to the row/column scales: |d sigma^2| ~ 1e-10 * scale,
-// two orders inside the 1e-8 contract (tests/test_gpu_parity.py::test_i8_*).
+// wgmma has no f64 kind, and the fp64 DMMA path is far below the int8 rate.  Instead both fp64 operands
+// are expanded exactly into small signed digits after a power-of-two scaling,
+//     W[i,k]  = 2^E_i * sum_s a_s[i,k] r^-s,    K*[m,k] = 2^F * sum_t b_t[m,k] r^-t,
+// so that V[i,m] = 2^(E_i+F) sum_d r^-d G_d[i,m] with G_d = sum_{s+t=d} A_s B_t^T (int32, exact).  Two digit
+// schemes (chosen per posterior by api.cu from the a-priori error bound):
+//   radix 128: six signed 7-bit digits, all 21 products (groups d = 2..7, weight 2^-7d);
+//   radix 256: five digits (top digit 7 bits, four balanced bytes: digits_radix256 in kernels.cu), the 15
+//              products with s + t <= 6 (groups d = 2..6, weight 2^-(8d-2)); the dropped terms are ~2^-40 of the
+//              operands' scale, the order of the digit truncation.  int32 headroom: 5 K 2^14 < 2^31 needs
+//              K <= 26214 (api.cu refuses the scheme beyond npad = 24576).
 //
-// CTA = one 128 (rows of W) x 64 (candidates) tile, 6 warps:
-//   warp 0  TMA producer: two 3-D boxes per stage (all 6 digit planes of A and of B for a K-block of
-//           64), SWIZZLE_128B, 3-stage full/empty mbarrier ring (72 KB per stage).  Digit planes are
-//           stored pair-interleaved -- every 128-byte row holds 64 k-values of digit 2p followed by the
-//           same 64 k-values of digit 2p+1 -- so that each TMA row request moves 128 B: the first
-//           version with 64-byte rows was bound by the TMA request rate (23 B/clk/SM, tensor pipe 42 %
-//           busy; profiles/r01_i8_ncu_summary.txt)
-//   warp 1  TMEM allocator + MMA issuer (one elected thread): 42 UTCIMMA (M128 N64 K32) per stage,
-//           tcgen05.commit releases the stage / signals the accumulators
-//   warps 2-9 epilogue (two per TMEM lane quarter): tcgen05.ld 32x32b, fp64 recombination, row scale,
-//           square, halving-butterfly column reduction, deterministic partial sums (same `partial`
-//           layout as the DMMA kernels)
-// W is lower triangular: row block rb only contracts k < 128 (rb + 1).
+// Digit planes are stored pair-interleaved at 32-k granularity: plane p holds digits 2p+1 and 2p+2 (1-based), and
+// every 64-byte row segment holds 32 k-values of the first followed by the same 32 k-values of the second.  One
+// TMA box (64 B x rows x 3 planes, SWIZZLE_64B) thus brings all digits of a K = 32 block, and the wgmma
+// descriptors of the two digits of a plane differ by a 32-byte start offset inside the swizzle atom.
+//
+// CTA = one 128 (rows of W) x 32 (candidates) output tile, 9 warps:
+//   warps 0-7  two consumer warpgroups, 64 rows each: per K = 32 block one wgmma.m64n32k32.s32.s8.s8 per kept digit
+//              product, both operands from shared memory, int32 accumulators in registers (one 16-register
+//              fragment per digit group); the epilogue recombines the groups in fp64 (smallest weight first),
+//              applies the row / column scales, squares and reduces every column over the tile's 128 rows in a
+//              fixed order (deterministic `partial`, same layout as the DMMA kernels);
+//   warp 8     TMA producer (one lane): full / empty mbarrier ring of I8_STAGES K-blocks.
+// W is lower triangular: row block rb only contracts k < 128 (rb + 1).  Tile order: groups of `cb_group` candidate
+// tiles; inside a group the heaviest row blocks first, so the CTAs resident at a time share a few K_* digit tiles and
+// sweep W.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -33,21 +34,18 @@
 
 namespace dfb {
 
-constexpr int I8_S = 6;                       // digits per operand
-constexpr int I8_BM = 128, I8_BN = 64, I8_BK = 64;
-constexpr int I8_STAGES = 3;
-constexpr int I8_A_PAIR = I8_BM * 2 * I8_BK;  // 16384 B: 128 rows x (64 B digit 2p | 64 B digit 2p+1)
-constexpr int I8_B_PAIR = I8_BN * 2 * I8_BK;  // 8192 B
-constexpr int I8_A_BYTES = (I8_S / 2) * I8_A_PAIR;
-constexpr int I8_B_BYTES = (I8_S / 2) * I8_B_PAIR;
-constexpr int I8_STAGE_BYTES = I8_A_BYTES + I8_B_BYTES;      // 73728
-constexpr int I8_THREADS = 320;                  // producer, MMA issuer, 8 epilogue warps
-constexpr int I8_TMEM_COLS = 512;
-constexpr size_t I8_SMEM_BYTES = (size_t)I8_STAGES * I8_STAGE_BYTES + 1024 + 4 * I8_BN * sizeof(double) +
-                                 (2 * I8_STAGES + 1) * 8 + 64;
-// M=128, N=64, A/B = signed int8 K-major, D = int32   (cute::UMMA::InstrDescriptor bit layout)
-constexpr uint32_t I8_IDESC = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(I8_BN >> 3) << 17) |
-                              ((uint32_t)(I8_BM >> 4) << 24);
+constexpr int I8_S = 6;                        // radix-128 digits per operand
+constexpr int I8_R256_DIGITS = 5;              // radix-256 digits per operand
+constexpr int I8_BM = 128, I8_BK = 32;          // I8_BN: gemm_tma.h
+constexpr int I8_STAGES = 7;
+constexpr int I8_A_PLANE = I8_BM * 2 * I8_BK;  // 8192 B: 128 rows x (32 B digit 2p+1 | 32 B digit 2p+2)
+constexpr int I8_B_PLANE = I8_BN * 2 * I8_BK;  // 2048 B
+constexpr int I8_A_BYTES = 3 * I8_A_PLANE;
+constexpr int I8_STAGE_BYTES = I8_A_BYTES + 3 * I8_B_PLANE;   // 30720
+constexpr int I8_CONSUMERS = 256;              // two warpgroups
+constexpr int I8_THREADS = I8_CONSUMERS + 32;  // + the producer warp
+constexpr size_t I8_SMEM_BYTES = (size_t)I8_STAGES * I8_STAGE_BYTES + 1024 + 8 * I8_BN * sizeof(double) +
+                                 2 * I8_STAGES * 8 + 64;
 
 struct ScoreI8Args {
   int n_rb, n_cb, K;
@@ -56,10 +54,8 @@ struct ScoreI8Args {
   int64_t ld_partial;
   const double* rowscale;   // 2^E_i per row of W
   double colscale;          // 2^F
-  unsigned long long* timing;   // diagnostics (DFB200_I8_TIMING): per-CTA clocks the MMA thread spent waiting; else NULL
-  const int* abort_count;       // CTA-pair kernel: the launch is a no-op once *abort_count > abort_cap (the arg-max
-  int abort_cap;                // shortlist overflowed, so this int8 pass will be discarded for an fp64 one); may be NULL
-  unsigned long long l2_a, l2_b;   // CTA-pair kernel: L2 eviction-priority descriptors of the W-digit / K_*-digit TMA loads
+  const int* abort_count;   // the launch is a no-op once *abort_count > abort_cap (the arg-max shortlist overflowed,
+  int abort_cap;            // so this int8 pass will be discarded for an fp64 one); may be NULL
 };
 
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, int c2,
@@ -70,96 +66,70 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
       "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4,
-// LBO = 1, SBO = 1024 B (8 rows x 128 B), version 1 (sm_100), layout type 2.
-__device__ __forceinline__ uint64_t umma_desc_sw128(unsigned smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// K-major SWIZZLE_64B shared-memory matrix descriptor of wgmma: start >> 4, LBO 1 (unused for swizzled K-major),
+// SBO = 512 B (8 rows x 64 B), layout type 2 = SWIZZLE_64B.
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(unsigned smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
 }
-__device__ __forceinline__ void umma_i8(unsigned tmem_d, uint64_t da, uint64_t db, unsigned accumulate) {
+// D (64 x 32, int32) (+)= A (64 x 32 int8) B^T (32 x 32 int8); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_i8_n32(int (&d)[16], uint64_t da, uint64_t db, unsigned accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(I8_IDESC), "r"(accumulate)
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
 }
-// A operand from tensor memory (TS form): the digit tile was copied there once with tcgen05.cp, so the
-// 21 products of a K-block re-read only B from shared memory.
-__device__ __forceinline__ void umma_i8_ts(unsigned tmem_d, unsigned tmem_a, uint64_t db, unsigned accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(db), "r"(I8_IDESC), "r"(accumulate)
-      : "memory");
-}
-// 128 rows x 256 bit (= one int8 digit tile of K = 32) shared -> tensor memory, 8 columns
-__device__ __forceinline__ void utccp_128x256b(unsigned tmem_dst, uint64_t src_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;\n" ::"r"(tmem_dst), "l"(src_desc) : "memory");
-}
-__device__ __forceinline__ void umma_commit(void* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(unsigned taddr, int (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+__device__ __forceinline__ void wgmma_fence_operands(int (&d)[16]) {
+#pragma unroll
+  for (int i = 0; i < 16; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 
-constexpr unsigned I8_TMEM_A0 = I8_S * I8_BN;          // first column of the A digit buffers (TS form)
-constexpr unsigned I8_TMEM_ABUF = I8_S * 8;            // columns per buffer: 6 digits x 32 bytes per row
-
-template <bool TS>
+template <bool R256>
 __global__ void __launch_bounds__(I8_THREADS, 1)
 score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const ScoreI8Args g) {
+  // uniform over the grid: the counter is only written by earlier kernels of the same stream
+  if (g.abort_count != nullptr && *g.abort_count > g.abort_cap) return;
+  constexpr int NS = R256 ? I8_R256_DIGITS : I8_S;      // digits per operand
+  constexpr int DMAX = R256 ? 6 : 7;                     // largest kept digit group s + t
+  constexpr int NG = DMAX - 1;                           // accumulators: groups 2..DMAX
   extern __shared__ unsigned char smem_raw[];
   unsigned char* tiles = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  double* colsum = reinterpret_cast<double*>(tiles + (size_t)I8_STAGES * I8_STAGE_BYTES);   // [4][64]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 4 * I8_BN);
+  double* colsum = reinterpret_cast<double*>(tiles + (size_t)I8_STAGES * I8_STAGE_BYTES);   // [8 warps][32]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 8 * I8_BN);
   uint64_t* empty_bar = full_bar + I8_STAGES;
-  uint64_t* accum_bar = empty_bar + I8_STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
-  // Tile order: groups of `cb_group` candidate tiles; inside a group the heaviest row blocks first.
-  // The CTAs resident at any time then share a few K_* digit tiles and sweep W, which stays L2
-  // resident across groups (W digits 79 MB + one group of K_* digits 16 MB < 126 MB of L2).
   const int bid = blockIdx.x;
-  const int per_group = g.cb_group * g.n_rb;
+  const int G = (g.cb_group > 0 && g.cb_group < g.n_cb) ? g.cb_group : g.n_cb;
+  const int per_group = G * g.n_rb;
   const int grp = bid / per_group, rem = bid - grp * per_group;
-  const int rb = g.n_rb - 1 - rem / g.cb_group;
-  const int cb = grp * g.cb_group + rem % g.cb_group;
-  if (cb >= g.n_cb) return;                         // ragged last group (uniform per CTA)
-  const int k_hi = min(g.K, (rb + 1) * TILE);
-  const int nk = k_hi / I8_BK;
+  const int cb0 = grp * G;
+  const int width = min(G, g.n_cb - cb0);               // the last group may be narrower
+  const int rb = g.n_rb - 1 - rem / width;
+  const int cb = cb0 + rem % width;
+  const int nk = min(g.K, (rb + 1) * TILE) / I8_BK;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   if (tid == 0) {
-    for (int s = 0; s < I8_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < I8_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], I8_CONSUMERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                     smem_u32(tmem_slot)),
-                 "r"(I8_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-  const unsigned tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
-  if (warp == 0) {
-    // ---------------- TMA producer --------------------------------------------------------------------
+  if (warp == I8_CONSUMERS / 32) {
+    // ---------------- TMA producer ----------------------------------------------------------------------
     if (lane == 0) {
       for (int kt = 0; kt < nk; kt++) {
         const int s = kt % I8_STAGES;
@@ -171,137 +141,94 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         tma_load_3d(dst + I8_A_BYTES, &tmB, kt * 2 * I8_BK, cb * I8_BN, 0, &full_bar[s]);
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer -------------------------------------------------------------------------
-    if (lane == 0) {
-      for (int kt = 0; kt < nk; kt++) {
-        const int s = kt % I8_STAGES;
-        const unsigned n = (unsigned)(kt / I8_STAGES);
-        mbar_wait(&full_bar[s], n & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-        const unsigned a0 = smem_u32(tiles + (size_t)s * I8_STAGE_BYTES);
-        // descriptor = {hi: SBO 1024 B | version 1 | SWIZZLE_128B, lo: (addr >> 4) | LBO 1}; within a
-        // stage only the 14-bit address field changes, by compile-time offsets.
-        const unsigned a_lo = ((a0 & 0x3FFFFu) >> 4) | 0x10000u;
-        const unsigned b_lo = (((a0 + I8_A_BYTES) & 0x3FFFFu) >> 4) | 0x10000u;
-        constexpr uint64_t DESC_HI = ((uint64_t)(64u | (1u << 14) | (2u << 29))) << 32;
-        if (TS) {
-          // K-half by K-half: copy the six A digit tiles of this K = 32 block into the tensor-memory
-          // buffer (double-buffered by kh), then issue the 21 products grouped by accumulator.  The
-          // tcgen05 pipeline executes cp and mma of one thread in issue order.
-#pragma unroll
-          for (int kh = 0; kh < I8_BK / 32; kh++) {
-            const unsigned abuf = I8_TMEM_A0 + (unsigned)kh * I8_TMEM_ABUF;
-#pragma unroll
-            for (int s0 = 0; s0 < I8_S; s0++) {
-              const unsigned aoff = (s0 >> 1) * I8_A_PAIR + (s0 & 1) * I8_BK + kh * 32;
-              utccp_128x256b(abuf + (unsigned)s0 * 8u, DESC_HI | (uint64_t)(a_lo + (aoff >> 4)));
-            }
-#pragma unroll
-            for (int d = 2; d <= I8_S + 1; d++) {
-              const unsigned acc = (unsigned)((d - 2) * I8_BN);
-#pragma unroll
-              for (int sa = 1; sa <= d - 1; sa++) {
-                const int tb = d - sa;
-                const unsigned boff = ((tb - 1) >> 1) * I8_B_PAIR + ((tb - 1) & 1) * I8_BK + kh * 32;
-                const uint64_t db = DESC_HI | (uint64_t)(b_lo + (boff >> 4));
-                umma_i8_ts(acc, abuf + (unsigned)(sa - 1) * 8u, db, (kt == 0 && kh == 0 && sa == 1) ? 0u : 1u);
-              }
-            }
-          }
-        } else {
-        // One digit-sum group (= one TMEM accumulator) at a time, so consecutive MMAs accumulate into
-        // the same tensor-memory tile like the k-loop of an ordinary GEMM.
-#pragma unroll
-        for (int d = 2; d <= I8_S + 1; d++) {
-          const unsigned acc = (unsigned)((d - 2) * I8_BN);   // literal TMEM address (base 0, see epilogue)
-#pragma unroll
-          for (int sa = 1; sa <= d - 1; sa++) {
-            const int tb = d - sa;
-#pragma unroll
-            for (int kh = 0; kh < I8_BK / 32; kh++) {
-              const unsigned aoff = ((sa - 1) >> 1) * I8_A_PAIR + ((sa - 1) & 1) * I8_BK + kh * 32;
-              const unsigned boff = ((tb - 1) >> 1) * I8_B_PAIR + ((tb - 1) & 1) * I8_BK + kh * 32;
-              const uint64_t da = DESC_HI | (uint64_t)(a_lo + (aoff >> 4));
-              const uint64_t db = DESC_HI | (uint64_t)(b_lo + (boff >> 4));
-              umma_i8(acc, da, db, (kt == 0 && sa == 1 && kh == 0) ? 0u : 1u);
-            }
-          }
-        }
-        }
-        umma_commit(&empty_bar[s]);          // stage reusable once these MMAs have read it
-      }
-      umma_commit(accum_bar);                // accumulators complete
-    }
-  } else {
-    // ---------------- epilogue warps 2..9: two warps per TMEM lane quarter, 32 columns each ---------------
-    const int q = warp & 3;                  // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;        // which 32 of the 64 candidate columns
-    const int row = q * 32 + lane;
-    mbar_wait(accum_bar, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    // tmem_base != 0 would mean the literal accumulator addresses above were wrong: poison the result
-    const double rs = (tmem_base == 0u) ? g.rowscale[(int64_t)rb * I8_BM + row] * g.colscale
-                                        : __longlong_as_double(0x7ff8000000000000ll);
-    const unsigned lane_addr = tmem_base + ((unsigned)(q * 32) << 16);
-    for (int c0 = half * 32; c0 < half * 32 + 32; c0 += 8) {
-      int r[I8_S][8];
-#pragma unroll
-      for (int d = 0; d < I8_S; d++) tmem_ld8(lane_addr + (unsigned)(d * I8_BN + c0), r[d]);
-      asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-      double sq[8];
-#pragma unroll
-      for (int j = 0; j < 8; j++) {
-        // v = sum_d G_d 2^(-7(d+2)), smallest weight first
-        double v = (double)r[5][j] * 0x1p-49;
-        v = fma((double)r[4][j], 0x1p-42, v);
-        v = fma((double)r[3][j], 0x1p-35, v);
-        v = fma((double)r[2][j], 0x1p-28, v);
-        v = fma((double)r[1][j], 0x1p-21, v);
-        v = fma((double)r[0][j], 0x1p-14, v);
-        v *= rs;
-        sq[j] = v * v;
-      }
-      // Sum each of the 8 columns over the warp's 32 rows with a halving butterfly: every exchange step
-      // keeps half of the columns per lane, so 4 + 2 + 1 + 1 + 1 shuffles replace 8 x 5.  The summation
-      // tree is fixed, so results are reproducible run to run.
-      const bool h16 = (lane & 16) != 0, h8 = (lane & 8) != 0, h4 = (lane & 4) != 0;
-      double w4[4], w2[2], w1;
-#pragma unroll
-      for (int j = 0; j < 4; j++) {
-        const double send = h16 ? sq[j] : sq[j + 4];
-        const double keep = h16 ? sq[j + 4] : sq[j];
-        w4[j] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-      }
-#pragma unroll
-      for (int j = 0; j < 2; j++) {
-        const double send = h8 ? w4[j] : w4[j + 2];
-        const double keep = h8 ? w4[j + 2] : w4[j];
-        w2[j] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-      }
-      {
-        const double send = h4 ? w2[0] : w2[1];
-        const double keep = h4 ? w2[1] : w2[0];
-        w1 = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-      }
-      w1 += __shfl_xor_sync(0xffffffffu, w1, 2);
-      w1 += __shfl_xor_sync(0xffffffffu, w1, 1);
-      // lanes with (lane & 3) == 0 now hold one column each: 4*[bit4] + 2*[bit3] + [bit2]
-      if ((lane & 3) == 0)
-        colsum[q * I8_BN + c0 + ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1)] = w1;
-    }
-    asm volatile("bar.sync 1, 256;\n" ::: "memory");     // the eight epilogue warps
-    const int et = tid - 64;
-    if (et < I8_BN)
-      g.partial[(int64_t)rb * g.ld_partial + (int64_t)cb * I8_BN + et] =
-          ((colsum[et] + colsum[I8_BN + et]) + colsum[2 * I8_BN + et]) + colsum[3 * I8_BN + et];
-    asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(I8_TMEM_COLS)
-                 : "memory");
+
+  // ---------------- consumer warpgroups ------------------------------------------------------------------
+  const int wg = warp >> 2;                              // rows [64 wg, 64 wg + 64) of the tile
+  int acc[NG][16];
+#pragma unroll
+  for (int a = 0; a < NG; a++)
+#pragma unroll
+    for (int i = 0; i < 16; i++) acc[a][i] = 0;
+  for (int kt = 0; kt < nk; kt++) {
+    const int s = kt % I8_STAGES;
+    mbar_wait(&full_bar[s], (unsigned)(kt / I8_STAGES) & 1u);
+    const unsigned a0 = smem_u32(tiles + (size_t)s * I8_STAGE_BYTES) + (unsigned)(wg * 64 * 2 * I8_BK);
+    const unsigned b0 = smem_u32(tiles + (size_t)s * I8_STAGE_BYTES + I8_A_BYTES);
+#pragma unroll
+    for (int a = 0; a < NG; a++) wgmma_fence_operands(acc[a]);
+    wgmma_fence();
+#pragma unroll
+    for (int d = 2; d <= DMAX; d++) {
+      bool lead = true;
+#pragma unroll
+      for (int sa = 1; sa <= NS; sa++) {
+        const int tb = d - sa;
+        if (tb < 1 || tb > NS) continue;
+        const unsigned aoff = (unsigned)(((sa - 1) >> 1) * I8_A_PLANE + ((sa - 1) & 1) * I8_BK);
+        const unsigned boff = (unsigned)(((tb - 1) >> 1) * I8_B_PLANE + ((tb - 1) & 1) * I8_BK);
+        wgmma_i8_n32(acc[d - 2], wgmma_desc_sw64(a0 + aoff), wgmma_desc_sw64(b0 + boff),
+                     (kt == 0 && lead) ? 0u : 1u);
+        lead = false;
+      }
+    }
+    wgmma_commit();
+#pragma unroll
+    for (int a = 0; a < NG; a++) wgmma_fence_operands(acc[a]);
+    // the products of block kt - 1 are complete: release its stage
+    wgmma_wait<1>();
+    if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % I8_STAGES]);
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int a = 0; a < NG; a++) wgmma_fence_operands(acc[a]);
+
+  // Accumulator fragment of m64nN: register 4j + e of lane l in warp w (of the warpgroup) holds row
+  // 16 w + l / 4 + 8 (e >> 1), column 8 j + 2 (l % 4) + (e & 1).
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const double rs0 = g.rowscale[(int64_t)rb * I8_BM + r0] * g.colscale;
+  const double rs1 = g.rowscale[(int64_t)rb * I8_BM + r0 + 8] * g.colscale;
+  double cs[8];
+#pragma unroll
+  for (int i = 0; i < 16; i++) {
+    // v = sum_d G_d w_d, smallest weight first
+    double v;
+    if constexpr (R256) {
+      v = (double)acc[4][i] * 0x1p-46;
+      v = fma((double)acc[3][i], 0x1p-38, v);
+      v = fma((double)acc[2][i], 0x1p-30, v);
+      v = fma((double)acc[1][i], 0x1p-22, v);
+      v = fma((double)acc[0][i], 0x1p-14, v);
+    } else {
+      v = (double)acc[NG - 1][i] * 0x1p-49;
+      v = fma((double)acc[4][i], 0x1p-42, v);
+      v = fma((double)acc[3][i], 0x1p-35, v);
+      v = fma((double)acc[2][i], 0x1p-28, v);
+      v = fma((double)acc[1][i], 0x1p-21, v);
+      v = fma((double)acc[0][i], 0x1p-14, v);
+    }
+    v *= ((i & 2) ? rs1 : rs0);
+    const int c = (i >> 2) * 2 + (i & 1);                // column slot of this thread (0..7)
+    if (i & 2) cs[c] += v * v; else cs[c] = v * v;
+  }
+  // sum each column slot over the 8 row groups of the warp (lanes with equal l % 4): fixed tree
+#pragma unroll
+  for (int c = 0; c < 8; c++) {
+    cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 4);
+    cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 8);
+    cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 16);
+  }
+  if (lane < 4) {
+#pragma unroll
+    for (int c = 0; c < 8; c++) colsum[warp * I8_BN + (c >> 1) * 8 + 2 * lane + (c & 1)] = cs[c];
+  }
+  asm volatile("bar.sync 1, %0;\n" ::"n"(I8_CONSUMERS) : "memory");
+  if (tid < I8_BN) {
+    double t = colsum[tid];
+#pragma unroll
+    for (int w = 1; w < 8; w++) t += colsum[w * I8_BN + tid];
+    g.partial[(int64_t)rb * g.ld_partial + (int64_t)cb * I8_BN + tid] = t;
   }
 }
 

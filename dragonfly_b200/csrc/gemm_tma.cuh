@@ -1,5 +1,5 @@
 // v2 of the dominant kernel: V = W K_*^T fused with |v|^2 per candidate column (MODE_SCORE + SUMSQ of
-// gemm.cuh), re-staged the Blackwell way:
+// gemm.cuh), re-staged with Hopper's TMA and mbarriers:
 //   * operand tiles arrive by TMA (cp.async.bulk.tensor.2d, SASS UTMALDG) from two tensor maps
 //     (W and the K_* chunk), 128 rows x 16 doubles per box, SWIZZLE_128B so the fragment reads below
 //     are bank-conflict free without padding;
@@ -79,7 +79,7 @@ score_tma_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant_
   uint64_t* empty_bar = full_bar + TMA_STAGES;
 
   // Tile order: groups of `cb_group` candidate tiles, heaviest row blocks first inside a group, so the
-  // resident CTAs share a few K_* panels while W (105 MB) stays in the 126 MB L2 across groups.
+  // resident CTAs share a few K_* panels while they sweep W.
   const int bid = blockIdx.x;
   const int per_group = g.cb_group * g.n_rb;
   const int grp = bid / per_group, rem = bid - grp * per_group;

@@ -15,7 +15,7 @@ from .kernel import build_descriptor
 
 def _require_cuda(device=None):
   if not torch.cuda.is_available():
-    raise RuntimeError('dragonfly_b200 needs a CUDA device (B200, sm_100a); none is visible and '
+    raise RuntimeError('dragonfly_b200 needs a CUDA device (H100, sm_90a); none is visible and '
                        'there is no CPU fallback.')
   if device is None:
     device = torch.cuda.current_device()
@@ -350,10 +350,10 @@ class DevicePosterior(object):
 
 
 def measure_peak(what, device=None):
-  """ dfb_measure_peak: 'i8' -> tcgen05 kind::i8 issue rate (int8 TOP/s), 'f64' -> DMMA issue rate (TFLOP/s). """
+  """ dfb_measure_peak: 'i8' -> int8 wgmma issue rate (int8 TOP/s), 'f64' -> DMMA issue rate (TFLOP/s). """
   dev = _require_cuda(device)
   out = C.c_double(0.0)
-  code = {'i8': _lib.DFB_PEAK_TCGEN05_I8, 'f64': _lib.DFB_PEAK_DMMA_F64}[what]
+  code = {'i8': _lib.DFB_PEAK_I8, 'f64': _lib.DFB_PEAK_DMMA_F64}[what]
   _lib.check(_lib.load().dfb_measure_peak(dev.index, code, C.byref(out)), 'dfb_measure_peak')
   return out.value
 

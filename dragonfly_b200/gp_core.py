@@ -1,5 +1,5 @@
 """
-Drop-in for dragonfly.gp.gp_core.GP (gp_core.py:86-304) whose numeric bodies run on a B200 through
+Drop-in for dragonfly.gp.gp_core.GP (gp_core.py:86-304) whose numeric bodies run on an H100 through
 libdfb200: same constructor, methods, option meaning, public attributes (X, Y lists, num_tr_data,
 kernel, noise_var, mean_func, L, alpha, K_trtr_wo_noise) and error behaviour.
 
@@ -286,7 +286,7 @@ class GP(object):
           self.handle_non_psd_kernels))
     if self.handle_non_psd_kernels == 'project_first':
       raise NotImplementedError('project_first needs an eigen-decomposition; every kernel on the '
-                                'B200 hot path is guaranteed PSD (no CPU fallback).')
+                                'GPU hot path is guaranteed PSD (no CPU fallback).')
     post = self._new_device_posterior(len(X_mat))
     post.set_kernel(build_descriptor(self.kernel, train_dim=X_mat.shape[1], cand_dim=X_mat.shape[1]))
     post.set_train(X_mat, y_centred)
@@ -296,7 +296,7 @@ class GP(object):
                                              flags=flags)
     except np.linalg.LinAlgError:
       raise NotImplementedError('try_before_project fell through to project_first, which needs '
-                                'an eigen-decomposition (out of the B200 hot-path scope).')
+                                'an eigen-decomposition (out of the GPU hot-path scope).')
     return post, lml, power
 
   def build_posterior(self):
@@ -665,7 +665,7 @@ class GP(object):
     return '%s, noise-var=%0.3f (n=%d)' % (self._child_str(), self.noise_var, len(self.Y))
 
   def _child_str(self):
-    return 'B200-GP %s' % (str(self.kernel))
+    return 'H100-GP %s' % (str(self.kernel))
 
   # Copies share the device posterior; while another live copy uses it a posterior is never extended for good
   # (add_data on either copy rebuilds into a fresh one), only temporarily for hallucinations (restored on exit).

@@ -40,7 +40,7 @@ def draw_candidates(bounds, max_evals):
 
 def _check_rand_euclidean(anc_data):
   if anc_data.domain.get_type() != 'euclidean':
-    raise NotImplementedError('Only Euclidean domains are on the B200 hot path.')
+    raise NotImplementedError('Only Euclidean domains are on the GPU hot path.')
   return anc_data.acq_opt_method in ['rand']
 
 
@@ -282,7 +282,7 @@ def _delegate_to_reference_maximiser(acq_fn, anc_data, deterministic=True):
     from dragonfly.exd.exd_utils import maximise_with_method  # pylint: disable=import-error
   except ImportError:
     raise NotImplementedError(
-        "acq_opt_method '%s' is a sequential host maximiser outside the B200 hot path; 'rand', 'pdoo' and "
+        "acq_opt_method '%s' is a sequential host maximiser outside the GPU hot path; 'rand', 'pdoo' and "
         "'direct' (as PDOO) are served without a Dragonfly install." % (anc_data.acq_opt_method))
   acquisition = lambda x: acq_fn(np.asarray(x).reshape((1, -1)))
   _, opt_pt = maximise_with_method(anc_data.acq_opt_method, acquisition, anc_data.domain,

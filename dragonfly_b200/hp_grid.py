@@ -29,7 +29,7 @@ class EuclideanHPLayout(object):
                noise_var_label=0.05, noise_var_value=0.1, use_additive_gp=False, add_max_group_size=6,
                num_groups_per_group_size=-1):
     if kernel_type not in ('se', 'matern'):
-      raise NotImplementedError('kernel_type %s is outside the B200 hot-path scope.' % (kernel_type))
+      raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kernel_type))
     self.dim, self.kernel_type, self.nu = dim, kernel_type, nu
     self.use_same_bandwidth = use_same_bandwidth
     self.mean_func_type, self.mean_func_const = mean_func_type, mean_func_const
@@ -133,7 +133,7 @@ class EuclideanMFHPLayout(EuclideanHPLayout):
                domain_nu=2.5, fidel_use_same_bandwidth=False, domain_use_same_bandwidth=False, **kwargs):
     for kt in (fidel_kernel_type, domain_kernel_type):
       if kt not in ('se', 'matern'):
-        raise NotImplementedError('kernel_type %s is outside the B200 hot-path scope.' % (kt))
+        raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kt))
     super(EuclideanMFHPLayout, self).__init__(fidel_dim + domain_dim, 'se', **kwargs)
     self.fidel_dim, self.domain_dim = fidel_dim, domain_dim
     self.fidel_kernel_type, self.domain_kernel_type = fidel_kernel_type, domain_kernel_type

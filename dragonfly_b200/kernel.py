@@ -235,7 +235,7 @@ def _kind_of(kern):
     if n in names:
       return n
   raise NotImplementedError(
-      'Kernel type %s is outside the B200 hot-path scope (supported: SEKernel, MaternKernel, '
+      'Kernel type %s is outside the GPU hot-path scope (supported: SEKernel, MaternKernel, '
       'AdditiveKernel, CoordinateProductKernel); there is no CPU fallback.' % (type(kern).__name__))
 
 

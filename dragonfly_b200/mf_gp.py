@@ -29,7 +29,7 @@ class EuclideanGP(GP):
       return gp_kernel.MaternKernel(kernel_hyperparams['dim'], kernel_hyperparams['nu'],
                                     kernel_hyperparams['scale'],
                                     kernel_hyperparams['dim_bandwidths'])
-    raise NotImplementedError('kernel_type %s is outside the B200 hot-path scope.' % (kernel_type))
+    raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kernel_type))
 
 
 def get_ZX_from_ZZ_XX(ZZ, XX):

@@ -1,5 +1,5 @@
 /*
- * dfb200.h -- C-ABI of libdfb200.so: the B200 (sm_100a) GP-BO inner loop behind Dragonfly's
+ * dfb200.h -- C-ABI of libdfb200.so: the H100 (sm_90a) GP-BO inner loop behind Dragonfly's
  * Kernel / GP / gpb_acquisitions surfaces.
  *
  * The reference (dragonfly-opt 0.1.7) is pure Python + NumPy/SciPy and has NO C/FFI boundary on this
@@ -275,7 +275,7 @@ int dfb_ts_draws(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, dou
 /* Counters for bench.py: number of kernels this handle has launched. */
 int64_t dfb_launch_count(dfb_handle* h);
 /* Diagnostics: arm (buf_dev = device buffer of 1 + 4 * cap_records 64-bit words, zeroed) or disarm (NULL) the per-CTA
- * trace of the K_* and contraction kernels of the overlapped scoring pipeline: record = (kind << 32 | SM id, start ns,
+ * trace of the K_* kernel of the overlapped scoring pipeline: record = (kind << 32 | SM id, start ns,
  * end ns, CTA index), buf[0] = number of records wanted.  tools/trace_overlap.py reads it. */
 int dfb_debug_trace(void* buf_dev, int64_t cap_records);
 
@@ -285,32 +285,27 @@ int dfb_debug_trace(void* buf_dev, int64_t cap_records);
  *  "score_impl" : how |L^-1 k_*|^2 is contracted (env DFB200_SCORE=fp64|i8|auto at dfb_create; default auto;
  *                 readable back through dfb_query "score_impl").  ONE switch -- score_impl = 0 -- puts every call
  *                 on the pure fp64 DMMA path:
- *                 0 = fp64 DMMA everywhere (no reduced-precision arithmetic anywhere; 1.2 M candidates/s at N = 5000);
- *                 1 = int8-slice tcgen05 path everywhere, sigma vectors included (exact digit expansion of both fp64
- *                     operands, int32 accumulation in tensor memory; a-priori bound: query "i8_sigma2_bound");
+ *                 0 = fp64 DMMA everywhere (no reduced-precision arithmetic anywhere);
+ *                 1 = int8-slice wgmma path everywhere, sigma vectors included (exact digit expansion of both fp64
+ *                     operands, exact int32 accumulation; a-priori bound: query "i8_sigma2_bound");
  *                 2 = auto: dfb_eval stays fp64; dfb_score_argmax screens with the int8 path, re-scores in fp64
  *                     every candidate whose int8 score -- widened by the error allowance that follows from the
  *                     bound -- could reach the fp64 maximum, returns the fp64 arg-max (index and score) of those,
  *                     and finally checks the int8 scores of that shortlist against the fp64 ones: a candidate
  *                     outside its allowance voids the screen and the call is redone in fp64 (queries
  *                     "last_selfcheck_violations", "last_selfcheck_ratio").  The bound (api.cu: i8_sigma2_bound) is
- *                     a sqrt(n) rounding-error model validated by a committed sweep (profiles/r02_i8_bound_sweep.json:
- *                     480 configurations, worst measured / bound 0.28), not a worst-case bound.  The screen is skipped when the
+ *                     a sqrt(n) rounding-error model validated by a sweep (tools/sweep_i8_bound.py: 480
+ *                     configurations), not a worst-case bound.  The screen is skipped when the
  *                     bound exceeds 5e-9 ABSOLUTE (half the 1e-8 sigma^2 contract, whatever the kernel scale;
  *                     query "i8_bound_limit") or n < 1024.
- *  "i8_impl"    : which tcgen05 kernel the int8 path uses (switching re-slices W: layouts differ):
- *                 2 (default) = persistent CTA-pair kernel: tcgen05.mma.cta_group::2 M256 N128 K32, two passes
- *                     per 256 x 128 tile (gemm_i8c2.cuh);
- *                 1 = the same two passes from single CTAs, M128 N128 K32 (gemm_i8x2.cuh);
- *                 0 = one pass of M128 N64 K32 MMAs over 128 x 64 tiles, one CTA per tile (gemm_i8.cuh).
- *  "i8_radix"   : digit scheme of the CTA-pair kernel: 1 = five radix-256 digits, 15 products (measured
- *                 |d sigma^2| 3.6e-10 at N = 5000); 0 = six radix-128 digits, 21 products (3e-11), the scheme
- *                 of i8_impl 0 and 1; -1 (default) = radix 256 whenever its a-priori bound is below
- *                 5e-9 (absolute) for the training kernel, else radix 128.
+ *  "i8_impl"    : digit schemes the int8 path (gemm_i8.cuh, one wgmma kernel) may use (switching re-slices W):
+ *                 2 (default) = as option "i8_radix" says; 0, 1 = six radix-128 digits only.
+ *  "i8_radix"   : digit scheme with i8_impl 2: 1 = five radix-256 digits, 15 products; 0 = six radix-128 digits,
+ *                 21 products (about 12x more accurate); -1 (default) = radix 256 whenever its a-priori bound is
+ *                 below 5e-9 (absolute) for the training kernel, else radix 128.
  *  "i8_fuse"    : 1 (default) = the K_* kernel emits the int8 digit planes directly, 0 = via an fp64 K_* buffer.
  *  "i8_unguarded": diagnostics only (tools/sweep_i8_bound.py): 1 = run the int8 path even when its a-priori bound exceeds
  *                 the limit, so that the bound can be compared with the measured error where it would refuse.
- *  "i8_ts"      : i8_impl 0 only: 1 = stage W's digits in tensor memory (tcgen05.cp), default 0.
  *  "lookahead"  : 1 (default) = look-ahead schedule of the blocked factorisation (next panel's column updated first,
  *                 chol_diag + panel solve of step k+1 overlap the bulk trailing update of step k on a second stream;
  *                 bit-identical results), 0 = one stream, step after step.
@@ -320,12 +315,10 @@ int dfb_debug_trace(void* buf_dev, int64_t cap_records);
  *                 plain SE / Matern on <= 8 dims; 0 = the round-1 kernels in the reference's operation order.
  *  "kstar_rows64": 1 (default) = the fp64 K_* rows of the fp64 scoring paths come from kstar_seg_kernel's row form too.
  *  "kstar_overlap": 1 = K_* of chunk c+1 on a second stream beside the contraction of chunk c (two-stream pipeline with
- *                 double-buffered digit planes); default 0 -- no net gain on B200 (DESIGN.md 5.1).
- *  "i8_c2_group": candidate tiles per group of the CTA-pair kernel's tile order; 0 (default) = chosen per geometry by
- *                 simulating the static deal (balance first, then the least HBM traffic); query "last_c2_group".
- *  "i8_l2_hint" : L2 eviction priorities of that kernel's TMA loads: 0 (default) none, 1 = K_* digits evict-last,
- *                 2 = also W digits evict-first (measured neutral / slower).
- *  "kstar_fast", "tma_cb_group", "i8_cb_group": kernel-selection / scheduling knobs used by tools/. */
+ *                 double-buffered digit planes); default 0.
+ *  "i8_c2_group": candidate tiles (of 32) per group of the int8 kernel's tile order; 0 (default) = 16; query
+ *                 "last_c2_group".
+ *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_impl", "i8_radix256", "score_impl",
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen
@@ -345,10 +338,10 @@ int dfb_profile_enable(dfb_handle* h, int on);
 int dfb_profile_read(dfb_handle* h, int cls, double* ms_total, int64_t* launches, double* units);
 
 /* Live roofline denominators for bench.py, measured on `device` in the calling process (best of 3 short launches):
- * DFB_PEAK_TCGEN05_I8 -> issue rate of tcgen05.mma kind::i8 M128 N256 K32 in int8 TOP/s (2 per MAC), the peak the
+ * DFB_PEAK_I8 -> issue rate of wgmma.m64n256k32.s32.s8.s8 from shared memory in int8 TOP/s (2 per MAC), the peak the
  * int8-slice contraction is quoted against; DFB_PEAK_DMMA_F64 -> fp64 DMMA.8x8x4 issue rate in TFLOP/s.
- * MEASURED_PEAKS.json carries neither.  Not on the product path; replaces nothing in the reference.  */
-#define DFB_PEAK_TCGEN05_I8 0
+ * Not on the product path; replaces nothing in the reference.  */
+#define DFB_PEAK_I8         0
 #define DFB_PEAK_DMMA_F64   1
 int dfb_measure_peak(int device, int what, double* out_host);
 

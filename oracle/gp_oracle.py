@@ -3,7 +3,7 @@ CPU oracle (NumPy/SciPy restatement) of Dragonfly's GP-BO inner loop.  TEST INFR
 see oracle/__init__.py for who may import this.  All arithmetic is IEEE fp64, evaluated in the same
 operation order as the reference so that differences to the reference are BLAS-summation-order only.
 
-Reference paths are relative to /root/reference (dragonfly-opt 0.1.7).
+Reference paths are relative to the reference source tree (dragonfly-opt 0.1.7).
 """
 import math
 import numpy as np

@@ -1,11 +1,11 @@
 """
 Generates tests/golden/*.npz by running the UNMODIFIED reference (dragonfly-opt 0.1.7 under
-/root/reference) on small seeded inputs.  Run in the authoring container only:
+$DRAGONFLY_REF) on small seeded inputs.  Run with the reference source tree in $DRAGONFLY_REF:
 
-    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:/root/reference \
+    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF \
         python -W ignore tests/golden/make_golden.py
 
-The GPU box has no /root/reference: the committed fixtures are what travels.  Each fixture holds
+The tests read only the committed fixtures.  Each fixture holds
 the inputs (X, Y, candidates, hyper-parameters, normal draws) and the reference's outputs, so both
 the NumPy oracle (tests/test_oracle_golden.py) and the CUDA path (tests/test_gpu_parity.py) are
 checked against the reference itself.
@@ -19,7 +19,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, '..', '..'))
 
-import dragonfly  # noqa: E402  (the reference; needs the shim + /root/reference on PYTHONPATH)
+import dragonfly  # noqa: E402  (the reference; needs the shim + $DRAGONFLY_REF on PYTHONPATH)
 from dragonfly.gp.kernel import SEKernel, MaternKernel, AdditiveKernel, CoordinateProductKernel  # noqa
 from dragonfly.gp.gp_core import GP  # noqa
 from dragonfly.gp.euclidean_gp import EuclideanMFGP  # noqa
@@ -29,7 +29,7 @@ from dragonfly.utils import general_utils as ref_gu  # noqa
 
 from dragonfly_b200 import synth_data  # noqa
 
-assert dragonfly.__file__.startswith('/root/reference'), dragonfly.__file__
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF']), dragonfly.__file__
 
 
 def const_mean(c):

@@ -3,8 +3,8 @@ Golden vectors for the Cartesian-product GP over Euclidean-type domains: the UNM
 dragonfly.gp.cartesian_product_gp.CPGP with dragonfly.gp.kernel.CartesianProductKernel (kernel.py:504-538) at its
 default handle_non_psd_kernels='project_first'.
 
-Run in the authoring container:
-  PYTHONPATH=/root/repo/oracle/ref_shim:/root/reference python tests/golden/make_golden_cpgp.py
+Run from the repository root with the reference source tree in $DRAGONFLY_REF:
+  PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF python tests/golden/make_golden_cpgp.py
 """
 import os
 import numpy as np
@@ -12,7 +12,7 @@ import dragonfly
 from dragonfly.gp.kernel import SEKernel, MaternKernel, CartesianProductKernel
 from dragonfly.gp.cartesian_product_gp import CPGP
 
-assert dragonfly.__file__.startswith('/root/reference')
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF'])
 
 
 def main():

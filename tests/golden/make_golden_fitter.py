@@ -1,9 +1,9 @@
 """
 Generates tests/golden/fitter.npz: the UNMODIFIED reference's EuclideanGPFitter.fit_gp (gp_core.py:783-821,
 euclidean_gp.py:153-345) with hp_tune_criterion='ml' and the three continuous-hp optimisers that the device path
-batches ('rand', 'rand_exp_sampling', 'pdoo'), under a seeded global RNG.  Authoring container only:
+batches ('rand', 'rand_exp_sampling', 'pdoo'), under a seeded global RNG.  Run with the reference source tree in $DRAGONFLY_REF:
 
-    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:/root/reference python -W ignore tests/golden/make_golden_fitter.py
+    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF python -W ignore tests/golden/make_golden_fitter.py
 """
 import os
 import sys
@@ -17,7 +17,7 @@ import dragonfly  # noqa: E402
 from dragonfly.gp.euclidean_gp import EuclideanGPFitter, euclidean_gp_args  # noqa
 from dragonfly.utils.option_handler import load_options  # noqa
 
-assert dragonfly.__file__.startswith('/root/reference')
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF'])
 
 
 def main():

@@ -2,7 +2,7 @@
 Generates tests/golden/fitter_add.npz: the UNMODIFIED reference's EuclideanGPFitter.fit_gp with use_additive_gp
 (euclidean_gp.py:312-323, 718-776) for ml_hp_tune_opt 'rand' and 'rand_exp_sampling', seeded.  Authoring container:
 
-    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:/root/reference python -W ignore tests/golden/make_golden_fitter_add.py
+    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF python -W ignore tests/golden/make_golden_fitter_add.py
 """
 import os
 import sys
@@ -16,7 +16,7 @@ import dragonfly  # noqa: E402
 from dragonfly.gp.euclidean_gp import EuclideanGPFitter, euclidean_gp_args  # noqa
 from dragonfly.utils.option_handler import load_options  # noqa
 
-assert dragonfly.__file__.startswith('/root/reference')
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF'])
 
 
 def main():

@@ -4,8 +4,8 @@ GP.compute_grad_log_marginal_likelihood (gp_core.py:229-240) with Kernel.gradien
 the UNMODIFIED reference.  The reference indexes hyperparams['dim_bandwidths'][0, j]; that is defined only when the
 bandwidths were handed over as a (d, 1) column, which is how the kernels are built here.
 
-Run in the authoring container:
-  PYTHONPATH=/root/repo/oracle/ref_shim:/root/reference python tests/golden/make_golden_grad.py
+Run from the repository root with the reference source tree in $DRAGONFLY_REF:
+  PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF python tests/golden/make_golden_grad.py
 """
 import os
 import numpy as np
@@ -13,7 +13,7 @@ import dragonfly
 from dragonfly.gp.kernel import SEKernel, MaternKernel
 from dragonfly.gp.gp_core import GP
 
-assert dragonfly.__file__.startswith('/root/reference')
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF'])
 
 
 def main():

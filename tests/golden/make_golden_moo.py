@@ -1,8 +1,8 @@
 """
 Generates tests/golden/moo.npz and tests/golden/incremental.npz by running the UNMODIFIED reference
-(dragonfly-opt 0.1.7 under /root/reference).  Authoring container only:
+(dragonfly-opt 0.1.7, source tree in $DRAGONFLY_REF).  Run with the reference source tree in $DRAGONFLY_REF:
 
-    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:/root/reference \
+    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF \
         python -W ignore tests/golden/make_golden_moo.py
 
 moo.npz          two objectives on one 6-D domain, the four multi-objective acquisitions
@@ -28,7 +28,7 @@ from dragonfly.exd.domains import EuclideanDomain  # noqa
 
 from dragonfly_b200 import synth_data  # noqa
 
-assert dragonfly.__file__.startswith('/root/reference'), dragonfly.__file__
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF']), dragonfly.__file__
 
 
 def const_mean(c):

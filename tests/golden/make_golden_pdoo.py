@@ -2,7 +2,7 @@
 Generates tests/golden/pdoo.npz by running the UNMODIFIED reference's PDOO maximiser
 (dragonfly/utils/oper_utils.py:257-271 -> dragonfly/utils/doo.py) on analytic objectives.  Authoring container:
 
-    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:/root/reference python -W ignore tests/golden/make_golden_pdoo.py
+    PYTHONDONTWRITEBYTECODE=1 PYTHONPATH=oracle/ref_shim:$DRAGONFLY_REF python -W ignore tests/golden/make_golden_pdoo.py
 
 Also records the reference's end-to-end recommendation for asy_ei / asy_ucb with acq_opt_method='pdoo' on the C1 GP
 (gpb_acquisitions.py:23-40: the non-vectorised branch of maximise_acquisition).
@@ -25,7 +25,7 @@ from dragonfly.opt import gpb_acquisitions as ref_acq  # noqa
 from dragonfly.exd.domains import EuclideanDomain  # noqa
 from dragonfly_b200 import synth_data  # noqa
 
-assert dragonfly.__file__.startswith('/root/reference')
+assert dragonfly.__file__.startswith(os.environ['DRAGONFLY_REF'])
 
 OBJECTIVES = {
   'neg_branin': (lambda x: -float(synth_data.branin(np.asarray(x, dtype=np.float64).reshape(1, -1))[0]),

@@ -1,7 +1,7 @@
 """
 CPU check of bench.py's reference arm (the driver runs `bench.py --impl reference` beside the GPU arm): exactly one
 JSON line on stdout with the contract's keys, the same metric / unit / config as the GPU arm would print, and a
-cpu_baseline block describing the run.  Small sizes so it takes seconds; the GPU arm itself needs the B200.
+cpu_baseline block describing the run.  Small sizes so it takes seconds; the GPU arm itself needs a GPU.
 """
 import json
 import os

@@ -25,7 +25,7 @@ N_CAND = 2560          # >= 2000 candidates per comparison
 @pytest.fixture(scope='module')
 def B():
   import torch
-  assert torch.cuda.is_available(), 'these tests need the B200'
+  assert torch.cuda.is_available(), 'these tests need a CUDA device'
   from dragonfly_b200 import kernel, gp_core, mf_gp, gpb_acquisitions, domains, device, _lib, synth_data
   from oracle import gp_oracle as O
   _lib.load()
@@ -78,7 +78,7 @@ def test_headline_posterior_state_against_oracle(B, headline):
 
 @pytest.mark.parametrize('score_impl', [0, 1])
 def test_headline_mu_sigma_against_oracle(B, headline, score_impl):
-  """ score_impl 0 = fp64 DMMA contraction, 1 = the tcgen05 int8 digit path also for the sigma vector. """
+  """ score_impl 0 = fp64 DMMA contraction, 1 = the int8 digit path also for the sigma vector. """
   gp = _headline_gp(B, headline, score_impl)
   mu, sd = gp.eval(headline.w['candidates'], 'std')
   assert gp._post.query('last_used_i8') == float(score_impl)

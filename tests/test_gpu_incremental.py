@@ -20,7 +20,7 @@ VAR_TOL = 1e-8
 @pytest.fixture(scope='module')
 def B():
   import torch
-  assert torch.cuda.is_available(), 'these tests need the B200'
+  assert torch.cuda.is_available(), 'these tests need a CUDA device'
   from dragonfly_b200 import kernel, gp_core, mf_gp, gpb_acquisitions, domains, device, _lib, synth_data
   from oracle import gp_oracle as O
   _lib.load()

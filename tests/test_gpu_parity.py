@@ -22,7 +22,7 @@ VAR_TOL = 1e-8
 @pytest.fixture(scope='module')
 def B():
   import torch
-  assert torch.cuda.is_available(), 'these tests need the B200'
+  assert torch.cuda.is_available(), 'these tests need a CUDA device'
   from dragonfly_b200 import kernel, gp_core, mf_gp, gpb_acquisitions, domains, device, _lib
   _lib.load()
   return Namespace(kernel=kernel, gp_core=gp_core, mf_gp=mf_gp, acq=gpb_acquisitions,
@@ -514,7 +514,7 @@ def test_tma_kernel_matches_cp_async_kernel(B):
   assert res[0][2][1] == res[1][2][1]
 
 
-# ---- the int8-slice tcgen05 contraction (score_impl 1 / auto) ------------------------------------------------
+# ---- the int8-slice wgmma contraction (score_impl 1 / auto) ------------------------------------------------
 def _post_pair(B, kern, X, Y, mean_const, noise_var, chunk=0, i8_impl=None, i8_radix=None):
   posts = []
   for impl in (0, 1):
@@ -552,8 +552,8 @@ def _i8_kernels(B):
 def test_i8_sigma2_within_contract(B, name, i8_impl, i8_radix):
   """ Digit-sliced tensor-core contraction vs fp64 DMMA on the same posterior: mu identical (it never
       leaves fp64), |d sigma^2| far inside the 1e-8 contract and inside the library's own a-priori
-      bound, for every kernel family, over several row blocks and ragged chunks; for all three tcgen05
-      kernels and both digit schemes of the CTA-pair kernel (forced, and as the library picks them). """
+      bound, for every kernel family, over several row blocks and ragged chunks; for every i8_impl setting and
+      both digit schemes (forced, and as the library picks them). """
   from dragonfly_b200 import synth_data
   rs = np.random.RandomState(3)
   X = rs.random_sample((1100, 6)); Y = synth_data.hartmann6(X)

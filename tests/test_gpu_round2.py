@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(scope='module')
 def B():
   import torch
-  assert torch.cuda.is_available(), 'these tests need the B200'
+  assert torch.cuda.is_available(), 'these tests need a CUDA device'
   from dragonfly_b200 import kernel, gp_core, gpb_acquisitions, domains, device, synth_data, _lib
   from oracle import gp_oracle as O
   _lib.load()

@@ -224,7 +224,7 @@ def test_pdoo_visits_the_cells_the_reference_visits(name):
   assert abs(val1 - val) <= 1e-13 * max(1.0, abs(val)) and (pt1 == pt).all()
 
 
-# ---- the int8 digit scheme of the tcgen05 contraction, emulated in integers on the CPU ----------------------------
+# ---- the int8 digit scheme of the wgmma contraction, emulated in integers on the CPU ----------------------------
 def _digits_radix256(x):
   """ NumPy restatement of digits_radix256 (dragonfly_b200/csrc/kernels.cu): five signed digits of |x| <= 1/2,
       x ~ a0 2^-7 + a1 2^-15 + a2 2^-23 + a3 2^-31 + a4 2^-39. """
@@ -278,7 +278,7 @@ def test_int8_slice_contraction_error_is_inside_the_a_priori_bound():
     for s in range(1, 6):
       t = dsum - s
       if 1 <= t <= 5:
-        G += A[s - 1] @ Bd[t - 1].T                 # what one chain of tcgen05.mma kind::i8 accumulates
+        G += A[s - 1] @ Bd[t - 1].T                 # what one chain of int8 wgmma accumulates
     assert np.abs(G).max() < 2 ** 31
     v += G.astype(np.float64) * 2.0 ** -(8 * dsum - 2)
   v *= rowscale[:, None] * colscale

@@ -1,6 +1,7 @@
 """A/B of the K_* stage at the headline geometry: (kstar_seg, kstar_overlap) in {0,1}^2 -- step time of
 gp._fused_score over M candidates, per-class launch times, and the arg-max each variant returns."""
 import json, os, sys, time
+import tempfile
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -38,5 +39,4 @@ gp._post.set_option('score_impl', 0); mu64, sd64 = gp._post.eval(sub, mean_const
 out['accuracy'] = dict(dsig2_seg=float((sd8 ** 2 - sd64 ** 2).abs().max()), dsig2_old=float((sd8o ** 2 - sd64 ** 2).abs().max()),
                        dmu_seg=float((mu8 - mu64).abs().max()), dmu_old=float((mu8o - mu64).abs().max()))
 print(out['accuracy'])
-os.makedirs('gpurun_out', exist_ok=True)
-json.dump(out, open('gpurun_out/ab_kstar.json', 'w'), indent=1)
+json.dump(out, open(os.path.join(tempfile.gettempdir(), 'ab_kstar.json'), 'w'), indent=1)

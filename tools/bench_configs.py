@@ -1,8 +1,9 @@
-"""Throughput of the other BASELINE.json configs on one B200 (candidates resident in HBM), with the
+"""Throughput of the other BASELINE.json configs on one GPU (candidates resident in HBM), with the
 default (auto) scoring mode and with the int8 path disabled.  Not the headline bench: evidence that
 every config of the scope table runs at scale.  Usage: python tools/bench_configs.py [scale]
   scale divides the candidate counts (default 4 -> C2 250k, C3 1M, C4 250k, C5 64k x 256 draws)."""
 import os, sys, time, json
+import tempfile
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -184,4 +185,4 @@ def incremental():
   return res
 out['incremental_N5000'] = incremental()
 print('inc', out['incremental_N5000'], flush=True)
-json.dump(out, open('gpurun_out/bench_configs.json', 'w'), indent=1)
+json.dump(out, open(os.path.join(tempfile.gettempdir(), 'bench_configs.json'), 'w'), indent=1)

@@ -1,4 +1,4 @@
-"""Measure the cuBLAS DGEMM peak on this B200 (roofline denominator for the fp64 contraction)."""
+"""Measure the cuBLAS DGEMM peak on this GPU (roofline denominator for the fp64 contraction)."""
 import json, sys, torch
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 8192
 a = torch.randn(n, n, dtype=torch.float64, device='cuda'); b = torch.randn(n, n, dtype=torch.float64, device='cuda')

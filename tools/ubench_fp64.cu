@@ -1,5 +1,5 @@
-// Micro-benchmark: fp64 DMMA.8x8x4 vs DFMA issue rate on B200 (sm_100a).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ubench_fp64 ubench_fp64.cu
+// Micro-benchmark: fp64 DMMA.8x8x4 vs DFMA issue rate on H100 (sm_90a).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ubench_fp64 ubench_fp64.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do{cudaError_t e=(x); if(e!=cudaSuccess){printf("CUDA error %s at %d\n",cudaGetErrorString(e),__LINE__); return 1;}}while(0)
