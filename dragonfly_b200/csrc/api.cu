@@ -370,10 +370,12 @@ static int prepare_i8(dfb_handle* h) {
   }
   // pair-interleaved digit planes: 3 planes of rows x (2 * npad) bytes
   DFB_TRY(launch_slice_i8(h, h->W, npad, npad, npad, h->rowinv, 0.0, h->Wi8, 2 * npad * npad, 2 * npad));
-  // one K = 32 block of all three planes per TMA box (64 B x rows x 3, SWIZZLE_64B): 128 rows of W, 32 candidates
+  // one K = 32 block of all three planes per TMA box (64 B x rows x 3, SWIZZLE_64B): 128 rows of W, one tile of
+  // candidates (the scheme's tile width)
+  const int bn = i8_tile_n(h->i8_radix256);
   DFB_TRY(make_tensor_map_3d_u8(&h->tmWi8, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 64, 128, 3));
-  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 32, 3));
-  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, 32, 3));
+  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, bn, 3));
+  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, bn, 3));
   h->i8_ready = true;
   return 0;
 }
@@ -678,8 +680,9 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
         const double colscale = i8_colscale(desc);
-        DFB_TRY(launch_score_i8_args(h, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb, (int)(m_rows / I8_BN), (int)npad,
-                                     h->partial, Mc, h->rowscale, colscale, abort_count));
+        DFB_TRY(launch_score_i8_args(h, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb,
+                                     (int)(m_rows / i8_tile_n(h->i8_radix256)), (int)npad, h->partial, Mc,
+                                     h->rowscale, colscale, abort_count));
       } else if (h->gemm_impl == 1 && h->tma_ready) {
         ScoreTmaArgs ta;
         ta.n_rb = g.n_rb; ta.n_cb = g.n_cb; ta.K = g.K; ta.partial = g.partial; ta.ld_partial = g.ld_partial;

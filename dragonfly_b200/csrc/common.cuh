@@ -112,7 +112,7 @@ struct dfb_handle {
   // TMA path of the scoring contraction (gemm_tma.cuh)
   int gemm_impl = 1;          // 0 = v1 cp.async ring, 1 = v2 TMA + mbarrier ring (default)
   int tma_cb_group = 1 << 20;       // candidate tiles per scheduling group (a sweep found no gain)
-  int i8_c2_group = 0;        // int8 kernel: candidate tiles per group of its tile order; 0 = 16 (kernels.cu)
+  int i8_c2_group = 0;        // int8 kernel: candidate tiles per group of its tile order; 0 = 8 (kernels.cu)
   int last_c2_group = 0;
   int kstar_fast = 1;         // specialised K_* kernel for plain SE / Matern on <= 8 dims
   bool tma_ready = false;

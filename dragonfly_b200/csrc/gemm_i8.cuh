@@ -17,13 +17,19 @@
 // TMA box (64 B x rows x 3 planes, SWIZZLE_64B) thus brings all digits of a K = 32 block, and the wgmma
 // descriptors of the two digits of a plane differ by a 32-byte start offset inside the swizzle atom.
 //
-// CTA = one 128 (rows of W) x 32 (candidates) output tile, 9 warps:
-//   warps 0-7  two consumer warpgroups, 64 rows each: per K = 32 block one wgmma.m64n32k32.s32.s8.s8 per kept digit
-//              product, both operands from shared memory, int32 accumulators in registers (one 16-register
-//              fragment per digit group); the epilogue recombines the groups in fp64 (smallest weight first),
-//              applies the row / column scales, squares and reduces every column over the tile's 128 rows in a
-//              fixed order (deterministic `partial`, same layout as the DMMA kernels);
-//   warp 8     TMA producer (one lane): full / empty mbarrier ring of I8_STAGES K-blocks.
+// CTA = one 128 (rows of W) x BN (candidates) output tile, BN = i8_tile_n(radix256): 64 for radix 256, 32 for
+// radix 128 (six accumulator groups of 32 columns would not fit the register file).  12 warps:
+//   warps 0-7  two consumer warpgroups, 64 rows each (setmaxnreg 232).  Per K = 32 block each warp loads its 16 x 32
+//              slice of every W digit once from shared memory into registers (ldmatrix.x4: the 8-bit A fragment of
+//              wgmma), then issues one wgmma.m64nBNk32.s32.s8.s8 per kept digit product with A from those registers
+//              and B (K_* digits) from a shared-memory descriptor, into int32 accumulators (one BN/2-register
+//              fragment per digit group).  Each W digit is thus read from shared memory once per block rather than
+//              once per product it takes part in; the fragments are double-buffered, and a buffer is reloaded only
+//              after wgmma.wait_group has retired the products that read it.  The epilogue recombines the groups in
+//              fp64 (smallest weight first), applies the row / column scales, squares and reduces every column over
+//              the tile's 128 rows in a fixed order (deterministic `partial`, same layout as the DMMA kernels);
+//   warps 8-11 the producer warpgroup (setmaxnreg 40): one lane runs the TMA side of a full / empty mbarrier ring of
+//              I8Tile::STAGES K-blocks.
 // W is lower triangular: row block rb only contracts k < 128 (rb + 1).  Tile order: groups of `cb_group` candidate
 // tiles; inside a group the heaviest row blocks first, so the CTAs resident at a time share a few K_* digit tiles and
 // sweep W.
@@ -36,16 +42,22 @@ namespace dfb {
 
 constexpr int I8_S = 6;                        // radix-128 digits per operand
 constexpr int I8_R256_DIGITS = 5;              // radix-256 digits per operand
-constexpr int I8_BM = 128, I8_BK = 32;          // I8_BN: gemm_tma.h
-constexpr int I8_STAGES = 7;
+constexpr int I8_BM = 128, I8_BK = 32;
 constexpr int I8_A_PLANE = I8_BM * 2 * I8_BK;  // 8192 B: 128 rows x (32 B digit 2p+1 | 32 B digit 2p+2)
-constexpr int I8_B_PLANE = I8_BN * 2 * I8_BK;  // 2048 B
 constexpr int I8_A_BYTES = 3 * I8_A_PLANE;
-constexpr int I8_STAGE_BYTES = I8_A_BYTES + 3 * I8_B_PLANE;   // 30720
 constexpr int I8_CONSUMERS = 256;              // two warpgroups
-constexpr int I8_THREADS = I8_CONSUMERS + 32;  // + the producer warp
-constexpr size_t I8_SMEM_BYTES = (size_t)I8_STAGES * I8_STAGE_BYTES + 1024 + 8 * I8_BN * sizeof(double) +
-                                 2 * I8_STAGES * 8 + 64;
+constexpr int I8_THREADS = I8_CONSUMERS + 128; // + the producer warpgroup
+constexpr int I8_CONSUMER_REGS = 232, I8_PRODUCER_REGS = 40;   // 2 * 128 * 232 + 128 * 40 <= 65536
+
+template <bool R256>
+struct I8Tile {
+  static constexpr int BN = i8_tile_n(R256);                   // candidates per tile
+  static constexpr int B_PLANE = BN * 2 * I8_BK;
+  static constexpr int STAGE_BYTES = I8_A_BYTES + 3 * B_PLANE; // 36864 (BN 64), 30720 (BN 32)
+  static constexpr int STAGES = R256 ? 6 : 7;
+  static constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 + 8 * BN * sizeof(double) +
+                                       2 * STAGES * 8 + 64;
+};
 
 struct ScoreI8Args {
   int n_rb, n_cb, K;
@@ -71,28 +83,53 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
 __device__ __forceinline__ uint64_t wgmma_desc_sw64(unsigned smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
 }
-// D (64 x 32, int32) (+)= A (64 x 32 int8) B^T (32 x 32 int8); accumulate = 0 overwrites D
-__device__ __forceinline__ void wgmma_i8_n32(int (&d)[16], uint64_t da, uint64_t db, unsigned accumulate) {
+// Four 8 x 16-byte matrices; lanes 8q .. 8q + 7 give the row addresses of matrix q, which lands in register q.
+__device__ __forceinline__ void ldmatrix_x4(unsigned (&r)[4], unsigned smem_addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];\n"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(smem_addr)
+               : "memory");
+}
+// D (64 x 32, int32) (+)= A (64 x 32 int8, registers) B^T (32 x 32 int8, shared); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_i8_rs(int (&d)[16], const unsigned (&a)[4], uint64_t db, unsigned accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %18, 0;\n"
+      "setp.ne.b32 p, %21, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p;\n"
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p;\n"
       "}\n"
       : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
         "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
-      : "l"(da), "l"(db), "r"(accumulate)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate)
+      : "memory");
+}
+// D (64 x 64, int32) (+)= A (64 x 32 int8, registers) B^T (32 x 64 int8, shared); accumulate = 0 overwrites D
+__device__ __forceinline__ void wgmma_i8_rs(int (&d)[32], const unsigned (&a)[4], uint64_t db, unsigned accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p;\n"
+      "}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate)
       : "memory");
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
-// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
-__device__ __forceinline__ void wgmma_fence_operands(int (&d)[16]) {
+// keeps the compiler from moving reads / writes of wgmma operand registers across an asynchronous wgmma
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_fence_operands(T (&r)[N]) {
 #pragma unroll
-  for (int i = 0; i < 16; i++) asm volatile("" : "+r"(d[i])::"memory");
+  for (int i = 0; i < N; i++) asm volatile("" : "+r"(r[i])::"memory");
 }
 
 template <bool R256>
@@ -101,15 +138,18 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 const ScoreI8Args g) {
   // uniform over the grid: the counter is only written by earlier kernels of the same stream
   if (g.abort_count != nullptr && *g.abort_count > g.abort_cap) return;
+  using T = I8Tile<R256>;
+  constexpr int BN = T::BN, STAGES = T::STAGES;
   constexpr int NS = R256 ? I8_R256_DIGITS : I8_S;      // digits per operand
   constexpr int DMAX = R256 ? 6 : 7;                     // largest kept digit group s + t
   constexpr int NG = DMAX - 1;                           // accumulators: groups 2..DMAX
+  constexpr int NACC = BN / 2;                           // int32 accumulator registers per group and thread
   extern __shared__ unsigned char smem_raw[];
   unsigned char* tiles = reinterpret_cast<unsigned char*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  double* colsum = reinterpret_cast<double*>(tiles + (size_t)I8_STAGES * I8_STAGE_BYTES);   // [8 warps][32]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 8 * I8_BN);
-  uint64_t* empty_bar = full_bar + I8_STAGES;
+  double* colsum = reinterpret_cast<double*>(tiles + (size_t)STAGES * T::STAGE_BYTES);   // [8 warps][BN]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(colsum + 8 * BN);
+  uint64_t* empty_bar = full_bar + STAGES;
 
   const int bid = blockIdx.x;
   const int G = (g.cb_group > 0 && g.cb_group < g.n_cb) ? g.cb_group : g.n_cb;
@@ -123,39 +163,56 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
   if (tid == 0) {
-    for (int s = 0; s < I8_STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], I8_CONSUMERS / 32); }
+    for (int s = 0; s < STAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], I8_CONSUMERS / 32); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
 
-  if (warp == I8_CONSUMERS / 32) {
+  if (warp >= I8_CONSUMERS / 32) {
     // ---------------- TMA producer ----------------------------------------------------------------------
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(I8_PRODUCER_REGS));
+    if (warp == I8_CONSUMERS / 32 && lane == 0) {
       for (int kt = 0; kt < nk; kt++) {
-        const int s = kt % I8_STAGES;
-        const unsigned n = (unsigned)(kt / I8_STAGES);
+        const int s = kt % STAGES;
+        const unsigned n = (unsigned)(kt / STAGES);
         mbar_wait(&empty_bar[s], (n & 1u) ^ 1u);
-        mbar_expect_tx(&full_bar[s], (unsigned)I8_STAGE_BYTES);
-        unsigned char* dst = tiles + (size_t)s * I8_STAGE_BYTES;
+        mbar_expect_tx(&full_bar[s], (unsigned)T::STAGE_BYTES);
+        unsigned char* dst = tiles + (size_t)s * T::STAGE_BYTES;
         tma_load_3d(dst, &tmA, kt * 2 * I8_BK, rb * I8_BM, 0, &full_bar[s]);
-        tma_load_3d(dst + I8_A_BYTES, &tmB, kt * 2 * I8_BK, cb * I8_BN, 0, &full_bar[s]);
+        tma_load_3d(dst + I8_A_BYTES, &tmB, kt * 2 * I8_BK, cb * BN, 0, &full_bar[s]);
       }
     }
     return;
   }
 
   // ---------------- consumer warpgroups ------------------------------------------------------------------
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(I8_CONSUMER_REGS));
   const int wg = warp >> 2;                              // rows [64 wg, 64 wg + 64) of the tile
-  int acc[NG][16];
+  // ldmatrix.x4 of a warp's 16 x 32 slice of one W digit: matrices (rows 0-7 | 8-15) x (bytes 0-15 | 16-31) give the
+  // four registers of the 8-bit A fragment of wgmma (register q: row l / 4 + 8 (q & 1), bytes 4 (l % 4) + 16 (q >> 1)
+  // .. + 3).  Lane l addresses row (l & 7) + 8 ((l >> 3) & 1), 16-byte chunk l >> 4 of the digit's 32 bytes.
+  // SWIZZLE_64B (as TMA wrote the tile) stores 16-byte chunk c of the 64-byte row r at chunk c ^ ((r >> 1) & 3); the
+  // warp's rows start at a multiple of 16, so (r >> 1) & 3 = (l & 7) >> 1.
+  const int arow = wg * 64 + (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+  const unsigned a_lane = (unsigned)(arow * 2 * I8_BK);
+  const unsigned a_chunk[2] = {(unsigned)(((0 + (lane >> 4)) ^ ((lane & 7) >> 1)) * 16),   // digit 2p+1 of a plane
+                               (unsigned)(((2 + (lane >> 4)) ^ ((lane & 7) >> 1)) * 16)};  // digit 2p+2
+  int acc[NG][NACC];
 #pragma unroll
   for (int a = 0; a < NG; a++)
 #pragma unroll
-    for (int i = 0; i < 16; i++) acc[a][i] = 0;
-  for (int kt = 0; kt < nk; kt++) {
-    const int s = kt % I8_STAGES;
-    mbar_wait(&full_bar[s], (unsigned)(kt / I8_STAGES) & 1u);
-    const unsigned a0 = smem_u32(tiles + (size_t)s * I8_STAGE_BYTES) + (unsigned)(wg * 64 * 2 * I8_BK);
-    const unsigned b0 = smem_u32(tiles + (size_t)s * I8_STAGE_BYTES + I8_A_BYTES);
+    for (int i = 0; i < NACC; i++) acc[a][i] = 0;
+  unsigned fa0[NS][4], fa1[NS][4];                      // A fragments of the even / odd K blocks
+
+  // one K block: A fragments into fa, all kept digit products, release of the previous block's stage
+  auto block = [&](const int kt, unsigned (&fa)[NS][4], unsigned (&fa_prev)[NS][4]) {
+    const int s = kt % STAGES;
+    mbar_wait(&full_bar[s], (unsigned)(kt / STAGES) & 1u);
+    const unsigned st = smem_u32(tiles + (size_t)s * T::STAGE_BYTES);
+#pragma unroll
+    for (int sa = 1; sa <= NS; sa++)
+      ldmatrix_x4(fa[sa - 1], st + (unsigned)(((sa - 1) >> 1) * I8_A_PLANE) + a_lane + a_chunk[(sa - 1) & 1]);
+    const unsigned b0 = st + (unsigned)I8_A_BYTES;
 #pragma unroll
     for (int a = 0; a < NG; a++) wgmma_fence_operands(acc[a]);
     wgmma_fence();
@@ -166,19 +223,24 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int sa = 1; sa <= NS; sa++) {
         const int tb = d - sa;
         if (tb < 1 || tb > NS) continue;
-        const unsigned aoff = (unsigned)(((sa - 1) >> 1) * I8_A_PLANE + ((sa - 1) & 1) * I8_BK);
-        const unsigned boff = (unsigned)(((tb - 1) >> 1) * I8_B_PLANE + ((tb - 1) & 1) * I8_BK);
-        wgmma_i8_n32(acc[d - 2], wgmma_desc_sw64(a0 + aoff), wgmma_desc_sw64(b0 + boff),
-                     (kt == 0 && lead) ? 0u : 1u);
+        const unsigned boff = (unsigned)(((tb - 1) >> 1) * T::B_PLANE + ((tb - 1) & 1) * I8_BK);
+        wgmma_i8_rs(acc[d - 2], fa[sa - 1], wgmma_desc_sw64(b0 + boff), (kt == 0 && lead) ? 0u : 1u);
         lead = false;
       }
     }
     wgmma_commit();
 #pragma unroll
     for (int a = 0; a < NG; a++) wgmma_fence_operands(acc[a]);
-    // the products of block kt - 1 are complete: release its stage
+    // the products of block kt - 1 are complete: its stage and its A fragments are free
     wgmma_wait<1>();
-    if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % I8_STAGES]);
+#pragma unroll
+    for (int sa = 0; sa < NS; sa++) wgmma_fence_operands(fa_prev[sa]);
+    if (kt > 0 && lane == 0) mbar_arrive(&empty_bar[(kt - 1) % STAGES]);
+  };
+  for (int kt = 0; kt < nk; kt += 2) {
+    block(kt, fa0, fa1);
+    if (kt + 1 == nk) break;
+    block(kt + 1, fa1, fa0);
   }
   wgmma_wait<0>();
 #pragma unroll
@@ -189,9 +251,10 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const double rs0 = g.rowscale[(int64_t)rb * I8_BM + r0] * g.colscale;
   const double rs1 = g.rowscale[(int64_t)rb * I8_BM + r0 + 8] * g.colscale;
-  double cs[8];
+  constexpr int NC = BN / 4;                             // column slots of a thread
+  double cs[NC];
 #pragma unroll
-  for (int i = 0; i < 16; i++) {
+  for (int i = 0; i < NACC; i++) {
     // v = sum_d G_d w_d, smallest weight first
     double v;
     if constexpr (R256) {
@@ -209,26 +272,26 @@ score_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       v = fma((double)acc[0][i], 0x1p-14, v);
     }
     v *= ((i & 2) ? rs1 : rs0);
-    const int c = (i >> 2) * 2 + (i & 1);                // column slot of this thread (0..7)
+    const int c = (i >> 2) * 2 + (i & 1);                // column slot of this thread
     if (i & 2) cs[c] += v * v; else cs[c] = v * v;
   }
   // sum each column slot over the 8 row groups of the warp (lanes with equal l % 4): fixed tree
 #pragma unroll
-  for (int c = 0; c < 8; c++) {
+  for (int c = 0; c < NC; c++) {
     cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 4);
     cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 8);
     cs[c] += __shfl_xor_sync(0xffffffffu, cs[c], 16);
   }
   if (lane < 4) {
 #pragma unroll
-    for (int c = 0; c < 8; c++) colsum[warp * I8_BN + (c >> 1) * 8 + 2 * lane + (c & 1)] = cs[c];
+    for (int c = 0; c < NC; c++) colsum[warp * BN + (c >> 1) * 8 + 2 * lane + (c & 1)] = cs[c];
   }
   asm volatile("bar.sync 1, %0;\n" ::"n"(I8_CONSUMERS) : "memory");
-  if (tid < I8_BN) {
+  if (tid < BN) {
     double t = colsum[tid];
 #pragma unroll
-    for (int w = 1; w < 8; w++) t += colsum[w * I8_BN + tid];
-    g.partial[(int64_t)rb * g.ld_partial + (int64_t)cb * I8_BN + tid] = t;
+    for (int w = 1; w < 8; w++) t += colsum[w * BN + tid];
+    g.partial[(int64_t)rb * g.ld_partial + (int64_t)cb * BN + tid] = t;
   }
 }
 

@@ -18,7 +18,8 @@ int launch_score_tma(dfb_handle* h, const CUtensorMap& tmW, const CUtensorMap& t
                      const ScoreTmaArgs& g);
 
 struct ScoreI8Args;
-constexpr int I8_BN = 32;    // candidates per tile of the int8 contraction (gemm_i8.cuh)
+// candidates per tile of the int8 contraction (gemm_i8.cuh) and rows of its K_* TMA box, per digit scheme
+constexpr int i8_tile_n(bool radix256) { return radix256 ? 64 : 32; }
 int make_tensor_map_3d_u8(CUtensorMap* out, const void* base, int64_t cols, int64_t rows, int64_t planes,
                           int64_t row_ld_bytes, int64_t plane_stride_bytes, int box_cols, int box_rows,
                           int box_planes);

@@ -316,8 +316,8 @@ int dfb_debug_trace(void* buf_dev, int64_t cap_records);
  *  "kstar_rows64": 1 (default) = the fp64 K_* rows of the fp64 scoring paths come from kstar_seg_kernel's row form too.
  *  "kstar_overlap": 1 = K_* of chunk c+1 on a second stream beside the contraction of chunk c (two-stream pipeline with
  *                 double-buffered digit planes); default 0.
- *  "i8_c2_group": candidate tiles (of 32) per group of the int8 kernel's tile order; 0 (default) = 16; query
- *                 "last_c2_group".
+ *  "i8_c2_group": candidate tiles per group of the int8 kernel's tile order (tiles of 64 candidates with radix-256
+ *                 digits, 32 with radix-128); 0 (default) = 8; query "last_c2_group".
  *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_impl", "i8_radix256", "score_impl",
