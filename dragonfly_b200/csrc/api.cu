@@ -680,7 +680,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
         const double colscale = i8_colscale(desc);
-        DFB_TRY(launch_score_i8_args(h, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb,
+        DFB_TRY(launch_score_i8_args(h, h->i8_radix256 != 0, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb,
                                      (int)(m_rows / i8_tile_n(h->i8_radix256)), (int)npad, h->partial, Mc,
                                      h->rowscale, colscale, abort_count));
       } else if (h->gemm_impl == 1 && h->tma_ready) {
@@ -1338,6 +1338,58 @@ int64_t dfb_launch_count(dfb_handle* h) { return h ? h->launches : 0; }
 
 int dfb_debug_trace(void* buf_dev, int64_t cap_records) { return debug_set_trace(buf_dev, (long long)cap_records); }
 
+// The production int8 contraction on caller-owned digit planes (tests/test_gpu_i8_exact.py): A = n_rb * 128 rows of
+// W digits, B = n_cb tiles of K_* digits, K = n_rb * 128, both in the pair-interleaved three-plane layout of
+// gemm_i8.cuh.  Tensor maps and launch as in prepare_i8 / run_chunks; the handle's digit scheme and buffers are untouched.
+int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev, const void* b_planes_dev, int32_t n_rb,
+                       int32_t n_cb, const double* rowscale_dev, double colscale, const int32_t* abort_count_dev,
+                       double* partial_dev, int64_t ld_partial) {
+  DFB_TRY(need(h, false, false, false, false, false));
+  const int bn = i8_tile_n(radix256 != 0);
+  if (a_planes_dev == nullptr || b_planes_dev == nullptr || rowscale_dev == nullptr || partial_dev == nullptr ||
+      n_rb < 1 || n_cb < 1 || ld_partial < (int64_t)n_cb * bn) {
+    set_error("bad debug_score_i8 arguments (n_rb %d, n_cb %d, ld_partial %lld)", n_rb, n_cb, (long long)ld_partial);
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  const int64_t K = (int64_t)n_rb * TILE, a_rows = K, b_rows = (int64_t)n_cb * bn;
+  CUtensorMap tmA, tmB;
+  DFB_TRY(make_tensor_map_3d_u8(&tmA, a_planes_dev, 2 * K, a_rows, 3, 2 * K, 2 * K * a_rows, 64, 128, 3));
+  DFB_TRY(make_tensor_map_3d_u8(&tmB, b_planes_dev, 2 * K, b_rows, 3, 2 * K, 2 * K * b_rows, 64, bn, 3));
+  const int keep_group = h->last_c2_group;
+  DFB_TRY(launch_score_i8_args(h, radix256 != 0, tmA, tmB, n_rb, n_cb, (int)K, partial_dev, ld_partial, rowscale_dev,
+                               colscale, abort_count_dev));
+  h->last_c2_group = keep_group;
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// Device-to-device copy of one internal buffer of the current state (tests/test_gpu_i8_exact.py); sizes follow from
+// the queries "npad" and "chunk".
+int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if (name == nullptr || dst_dev == nullptr) { set_error("bad debug_copy arguments"); return -1; }
+  const int64_t npad = h->npad, chunk = h->chunk;
+  const void* src = nullptr;
+  int64_t size = 0;
+  if (strcmp(name, "W") == 0) { src = h->W; size = (int64_t)sizeof(double) * npad * npad; }
+  else if (strcmp(name, "Wi8") == 0) { src = h->Wi8; size = 3 * 2 * npad * npad; }
+  else if (strcmp(name, "rowscale") == 0) { src = h->rowscale; size = (int64_t)sizeof(double) * npad; }
+  else if (strcmp(name, "Ki8") == 0) { src = h->Ki8; size = 3 * 2 * chunk * npad; }
+  else if (strcmp(name, "Ks") == 0) { src = h->Ks; size = (int64_t)sizeof(double) * chunk * npad; }
+  else if (strcmp(name, "partial") == 0) { src = h->partial; size = (int64_t)sizeof(double) * (npad / TILE) * chunk; }
+  else { set_error("unknown debug_copy buffer '%s'", name); return -1; }
+  if (bytes != size) {
+    set_error("debug_copy '%s': %lld bytes requested, the buffer has %lld", name, (long long)bytes, (long long)size);
+    return -1;
+  }
+  if (size == 0) return 0;
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  DFB_CUDA_OK(cudaMemcpyAsync(dst_dev, src, (size_t)size, cudaMemcpyDeviceToDevice, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
 int dfb_query(dfb_handle* h, const char* name, double* out) {
   DFB_TRY(need(h, false, false, false, false, false));
   if (name == nullptr || out == nullptr) { set_error("bad query arguments"); return -1; }
@@ -1348,6 +1400,7 @@ int dfb_query(dfb_handle* h, const char* name, double* out) {
   if (strcmp(name, "last_selfcheck_violations") == 0) { *out = (double)h->last_selfcheck_violations; return 0; }
   if (strcmp(name, "last_selfcheck_ratio") == 0) { *out = h->last_selfcheck_ratio; return 0; }
   if (strcmp(name, "chunk") == 0) { *out = (double)h->chunk; return 0; }
+  if (strcmp(name, "npad") == 0) { *out = (double)h->npad; return 0; }
   if (strcmp(name, "last_c2_group") == 0) { *out = (double)h->last_c2_group; return 0; }
   if (strcmp(name, "last_overlapped") == 0) { *out = (double)h->last_overlapped; return 0; }     // chunks of the last PIPELINED pass
   if (strcmp(name, "i8_bound_limit") == 0) { *out = I8_BOUND_LIMIT; return 0; }

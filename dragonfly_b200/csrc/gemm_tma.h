@@ -28,8 +28,9 @@ int launch_row_exponent(dfb_handle* h, const double* M, int64_t ld, int64_t rows
 int launch_slice_i8(dfb_handle* h, const double* M, int64_t ld, int64_t rows, int64_t cols,
                     const double* rowinv, double inv_const, void* out, int64_t plane_bytes,
                     int64_t out_ld_bytes);
-int launch_score_i8_args(dfb_handle* h, const CUtensorMap& tmA, const CUtensorMap& tmB, int n_rb, int n_cb, int K,
-                         double* partial, int64_t ld_partial, const double* rowscale, double colscale,
+// radix256 selects the digit scheme of the planes behind tmA / tmB (the scoring path passes h->i8_radix256)
+int launch_score_i8_args(dfb_handle* h, bool radix256, const CUtensorMap& tmA, const CUtensorMap& tmB, int n_rb,
+                         int n_cb, int K, double* partial, int64_t ld_partial, const double* rowscale, double colscale,
                          const int* abort_count = nullptr);
 
 }  // namespace dfb

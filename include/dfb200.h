@@ -278,6 +278,21 @@ int64_t dfb_launch_count(dfb_handle* h);
  * trace of the K_* kernel of the overlapped scoring pipeline: record = (kind << 32 | SM id, start ns,
  * end ns, CTA index), buf[0] = number of records wanted.  tools/trace_overlap.py reads it. */
 int dfb_debug_trace(void* buf_dev, int64_t cap_records);
+/* Diagnostics (tests/test_gpu_i8_exact.py), not on the product path: runs the int8 scoring contraction (gemm_i8.cuh)
+ * on caller-owned digit planes in its pair-interleaved layout, three planes each: A = n_rb * 128 rows of W digits,
+ * B = n_cb * BN rows of K_* digits (BN = 64 with radix256 = 1, 32 with radix-128 digits), both with K = n_rb * 128
+ * columns.  partial_dev receives the n_rb x (n_cb * BN) partial sums, leading dimension ld_partial >= n_cb * BN;
+ * rowscale_dev holds n_rb * 128 row scales; abort_count_dev may be NULL (else the launch writes nothing while
+ * *abort_count_dev > 4096, the shortlist capacity).  Tile grouping as option "i8_c2_group".  Synchronises. */
+int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev, const void* b_planes_dev, int32_t n_rb,
+                       int32_t n_cb, const double* rowscale_dev, double colscale, const int32_t* abort_count_dev,
+                       double* partial_dev, int64_t ld_partial);
+/* Diagnostics: device-to-device copy of one internal buffer of the current state; bytes must equal its size (query
+ * "npad" and "chunk"): "W" (fp64 L^-1, npad^2), "Wi8" (its three digit planes, 6 npad^2 bytes), "rowscale" (npad
+ * doubles), "Ki8" (the three K_* digit planes of the first chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
+ * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk).
+ * Synchronises. */
+int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
 
 /* Tuning switches.
  *  "gemm_impl"  : 0 = cp.async-ring DMMA kernel, 1 = TMA + mbarrier warp-specialised DMMA kernel for the
@@ -323,7 +338,7 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_impl", "i8_radix256", "score_impl",
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen
  * was voided and the call redone in fp64), "last_selfcheck_ratio" (max |s_int8 - s_fp64| / allowance over the last
- * shortlist; the model's margin is its inverse), "chunk", "last_c2_group", "last_overlapped". */
+ * shortlist; the model's margin is its inverse), "chunk", "npad", "last_c2_group", "last_overlapped". */
 int dfb_query(dfb_handle* h, const char* name, double* out);
 
 /* Per-kernel-class device timing with CUDA events on the handle's stream (bench.py's roofline):

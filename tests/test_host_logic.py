@@ -12,6 +12,8 @@ from dragonfly_b200 import kernel as K
 from dragonfly_b200 import _lib
 from oracle import gp_oracle as O
 
+import i8_exact as IX
+
 
 def test_matern_constants_match_oracle():
   for nu in [0.5, 1.5, 2.5, 3.5]:
@@ -224,69 +226,127 @@ def test_pdoo_visits_the_cells_the_reference_visits(name):
   assert abs(val1 - val) <= 1e-13 * max(1.0, abs(val)) and (pt1 == pt).all()
 
 
-# ---- the int8 digit scheme of the wgmma contraction, emulated in integers on the CPU ----------------------------
-def _digits_radix256(x):
-  """ NumPy restatement of digits_radix256 (dragonfly_b200/csrc/kernels.cu): five signed digits of |x| <= 1/2,
-      x ~ a0 2^-7 + a1 2^-15 + a2 2^-23 + a3 2^-31 + a4 2^-39. """
-  x = np.asarray(x, dtype=np.float64)
-  hi = np.rint(x * 2.0 ** 15)                      # round-half-even, like the magic-number trick
-  rem = x * 2.0 ** 15 - hi                         # exact
-  lo = np.rint(rem * 2.0 ** 24).astype(np.int64)
-  hi = hi.astype(np.int64)
-  s8 = lambda v: ((v + 128) % 256) - 128           # sign-extended low byte
-  a4 = s8(lo); r = (lo - a4) >> 8
-  a3 = s8(r); r = (r - a3) >> 8
-  a2 = s8(r); hi = hi + ((r - a2) >> 8)
-  a1 = s8(hi); a0 = (hi - a1) >> 8
-  return [a0, a1, a2, a3, a4]
+# ---- the int8 digit scheme of the wgmma contraction, emulated in integers on the CPU (tests/i8_exact.py) ----------
+_DIGIT_EDGES = [0.5, -0.5, 0.0, 2.0 ** -41, -2.0 ** -41, 0.49999999999, -0.49999999999, 2.0 ** -8, 2.0 ** -16 * 255.5,
+                1.0 / 3, -1.0 / 3, 2.0 ** -7 * 0.5, 2.0 ** -14 * 64.5, np.nextafter(0.5, 0.0), 2.0 ** -1074]
 
 
 def test_radix256_digits_are_int8_and_exact_to_2_pow_minus_40():
   rs = np.random.RandomState(0)
-  x = np.concatenate((rs.uniform(-0.5, 0.5, 200000), [0.5, -0.5, 0.0, 2.0 ** -41, -2.0 ** -41, 0.49999999999,
-                                                        2.0 ** -8, 2.0 ** -16 * 255.5, 1.0 / 3, -1.0 / 3]))
-  d = _digits_radix256(x)
+  x = np.concatenate((rs.uniform(-0.5, 0.5, 200000), _DIGIT_EDGES))
+  d = IX.digits_radix256(x)
+  assert len(d) == 5
   assert all(int(a.min()) >= -128 and int(a.max()) <= 127 for a in d)
   assert int(d[0].min()) >= -64 and int(d[0].max()) <= 64                    # the top digit keeps 7 bits
   recon = sum(a.astype(np.float64) * 2.0 ** -(8 * (s + 1) - 1) for s, a in enumerate(d))
+  assert (recon == IX.reconstruct(d, True)).all()
   assert np.abs(recon - x).max() <= 2.0 ** -40
 
 
-def test_int8_slice_contraction_error_is_inside_the_a_priori_bound():
-  """ The scheme of gemm_i8c2.cuh in exact integer arithmetic: W = L^-1-like rows scaled by 2^-E_i, K_* columns by
-      2^-F, five radix-256 digits each, the 15 products with s + t <= 6 accumulated as integers per power of 256,
-      recombined in fp64 -- against the fp64 contraction.  The sigma^2 error must sit inside api.cu's a-priori
-      bound 8 rowscale_max sqrt(n) colscale 2^-40 sqrt(kss) (i8_sigma2_bound), and the group sums inside int32. """
+def test_radix128_digits_are_in_range_and_exact_to_2_pow_minus_43():
+  rs = np.random.RandomState(10)
+  # slice_i8_kernel's operands are strictly inside (-1/2, 1/2) (row_exponent_kernel's 2^(e+1)); 1/2 itself included
+  x = np.concatenate((rs.uniform(-0.5, 0.5, 200000), _DIGIT_EDGES))
+  d = IX.digits_radix128(x)
+  assert len(d) == 6
+  assert all(int(a.min()) >= -64 and int(a.max()) <= 64 for a in d)
+  recon = IX.reconstruct(d, False)
+  assert np.abs(recon - x).max() <= 2.0 ** -43
+
+
+@pytest.mark.parametrize('n', [5, 6])
+def test_plane_pack_and_unpack_are_inverse(n):
+  rs = np.random.RandomState(n)
+  rows, cols = 40, 96
+  dg = [rs.randint(-128, 128, size=(rows, cols)) for _ in range(n)]
+  planes = IX.pack_planes(dg)
+  assert planes.shape == (3, rows, 2 * cols) and planes.dtype == np.int8
+  back = IX.unpack_planes(planes, n)
+  assert all((a == b).all() for a, b in zip(dg, back))
+  assert (IX.pack_planes(back) == planes).all()
+  # the byte of (digit s, row r, column k), spelled out
+  flat = planes.reshape(-1)
+  plane_bytes = rows * 2 * cols
+  for s, r, k in [(0, 0, 0), (1, 3, 31), (2, 7, 32), (3, 39, 95), (n - 1, 21, 64), (n - 1, 1, 33)]:
+    assert flat[(s // 2) * plane_bytes + r * 2 * cols + (k // 32) * 64 + (s % 2) * 32 + k % 32] == dg[s][r, k]
+  if n == 5:                      # radix 256 leaves the sixth slot alone
+    assert (planes[2].reshape(rows, cols // 32, 2, 32)[:, :, 1, :] == 0).all()
+
+
+def test_fma_emulation_is_correctly_rounded():
+  rs = np.random.RandomState(11)
+  a = rs.standard_normal(4000) * np.exp2(rs.randint(-60, 60, 4000))
+  b = np.where(rs.random_sample(4000) < 0.5, a, rs.standard_normal(4000))
+  c = np.where(rs.random_sample(4000) < 0.5, -a * b, rs.standard_normal(4000) * np.exp2(rs.randint(-120, 120, 4000)))
+  # near-cancellation and half-way cases: c = -(a b) rounded, c = a^2 rounded (the epilogue's use), exact zeros
+  c[:500] = -(a[:500] * b[:500])
+  c[500:1000] = a[500:1000] * a[500:1000]; b[500:1000] = a[500:1000]
+  a[1000:1010] = 0.0
+  a[1010:1020] = 2.0 ** -540                         # product below 2^-900: the Fraction path
+  got = IX.fma_vec(a, b, c)
+  want = np.array([IX.fma_fraction(float(x), float(y), float(z)) for x, y, z in zip(a, b, c)])
+  assert np.array_equal(got.view(np.int64), want.view(np.int64))
+  naive = a * b + c
+  assert (naive != want).sum() > 100                 # the emulation is not the unfused expression
+
+
+def _small_posterior(seed=1, n=640, m=48, kss=2.7):
   from oracle import gp_oracle as O
-  rs = np.random.RandomState(1)
-  n, m, kss = 640, 48, 2.7
+  rs = np.random.RandomState(seed)
   # a genuine posterior: W = L^-1 of K + noise I, K_* = k(X*, X) (the bound uses |v|^2 = k** - sigma^2 <= k(x, x))
   X, Xs = rs.random_sample((n, 4)), rs.random_sample((m, 4))
   kern = O.OMaternKernel(4, 2.5, kss, [0.3] * 4)
   L = np.linalg.cholesky(kern(X, X) + 0.01 * kss * np.eye(n))
-  W = np.linalg.inv(L)
-  W = np.tril(W)
-  Kst = kern(Xs, X)
-  e_row = np.frexp(np.abs(W).max(axis=1))[1] + 1
-  rowscale = np.ldexp(1.0, e_row)
-  colscale = np.ldexp(1.0, np.frexp(kss * (1 + 1e-9))[1] + 1)
-  A = _digits_radix256(W / rowscale[:, None])
-  Bd = _digits_radix256(Kst / colscale)
-  v = np.zeros((n, m))
-  for dsum in range(2, 7):                          # groups d = s + t (1-based digits), weight 2^-(8 d - 2)
-    G = np.zeros((n, m), dtype=np.int64)
-    for s in range(1, 6):
-      t = dsum - s
-      if 1 <= t <= 5:
-        G += A[s - 1] @ Bd[t - 1].T                 # what one chain of int8 wgmma accumulates
-    assert np.abs(G).max() < 2 ** 31
-    v += G.astype(np.float64) * 2.0 ** -(8 * dsum - 2)
+  W = np.tril(np.linalg.inv(L))
+  return W, kern(Xs, X), kss
+
+
+def test_int8_slice_contraction_error_is_inside_the_a_priori_bound():
+  """ The scheme of gemm_i8.cuh in exact integer arithmetic: W = L^-1-like rows scaled by 2^-E_i, K_* columns by
+      2^-F, five radix-256 digits each, the 15 products with s + t <= 6 accumulated as integers per power of 256,
+      recombined in fp64 -- against the fp64 contraction.  The sigma^2 error must sit inside api.cu's a-priori
+      bound 8 rowscale_max sqrt(n) colscale 2^-40 sqrt(kss) (i8_sigma2_bound), and the group sums inside int32. """
+  W, Kst, kss = _small_posterior()
+  n = W.shape[0]
+  rowscale = IX.row_scales(W)
+  colscale = IX.col_scale(kss)
+  A = IX.digits_radix256(W / rowscale[:, None])
+  Bd = IX.digits_radix256(Kst / colscale)
+  G = IX.group_sums(A, Bd, True)
+  v = np.zeros_like(G[2])
+  for d, w in IX.groups(True):                      # groups d = s + t (1-based digits), weight 2^-(8 d - 2)
+    assert np.abs(G[d]).max() < 2 ** 31
+    v += G[d] * w
   v *= rowscale[:, None] * colscale
   v_ref = (W.astype(np.longdouble) @ Kst.T.astype(np.longdouble)).astype(np.float64)
   err_sigma2 = np.abs((v ** 2).sum(axis=0) - (v_ref ** 2).sum(axis=0)).max()
   bound = 8.0 * rowscale.max() * np.sqrt(n) * colscale * 2.0 ** -40 * np.sqrt(kss)
   assert err_sigma2 <= bound, (err_sigma2, bound)
   assert err_sigma2 > 0.0                            # (it is an approximation: 2^-40 digits, dropped s + t = 7 terms)
+
+
+@pytest.mark.parametrize('radix256', [True, False])
+def test_emulated_partial_of_a_posterior_is_inside_the_a_priori_bound(radix256):
+  """ The kernel's `partial` as tests/i8_exact.py computes it (digits -> planes -> group sums -> epilogue in the
+      kernel's order), summed over the row blocks: |v|^2 per candidate inside the a-priori bound of the longdouble
+      contraction, for a ragged n padded to the 128-row blocks of W. """
+  W, Kst, kss = _small_posterior(seed=12, n=300, m=70)
+  n, m = W.shape[0], Kst.shape[0]
+  npad, bn = 384, IX.tile_n(radix256)
+  m_rows = (m + 127) // 128 * 128
+  Wp = np.eye(npad); Wp[:n, :n] = W                 # identity on the padding rows, as the factorisation leaves it
+  Kp = np.zeros((m_rows, npad)); Kp[:m, :n] = Kst
+  rowscale = IX.row_scales(Wp)
+  colscale = IX.col_scale(kss)
+  A = IX.unpack_planes(IX.pack_planes(IX.digits(Wp / rowscale[:, None], radix256)), IX.n_digits(radix256))
+  Bd = IX.unpack_planes(IX.pack_planes(IX.digits(Kp / colscale, radix256)), IX.n_digits(radix256))
+  part = IX.partial_reference(A, Bd, rowscale, colscale, radix256)
+  assert part.shape == (npad // 128, m_rows) and m_rows % bn == 0
+  assert (part[:, m:] == 0.0).all()
+  v_ref = (W.astype(np.longdouble) @ Kst.T.astype(np.longdouble)).astype(np.float64)
+  err = np.abs(part[:, :m].sum(axis=0) - (v_ref ** 2).sum(axis=0)).max()
+  bound = 8.0 * rowscale[:n].max() * np.sqrt(n) * colscale * 2.0 ** (-40 if radix256 else -43) * np.sqrt(kss)
+  assert err <= bound, (err, bound)
 
 
 # ---- incremental posterior: the host's decisions (no device: a NumPy-backed stand-in for DevicePosterior) -----------
