@@ -370,12 +370,10 @@ static int prepare_i8(dfb_handle* h) {
   }
   // pair-interleaved digit planes: 3 planes of rows x (2 * npad) bytes
   DFB_TRY(launch_slice_i8(h, h->W, npad, npad, npad, h->rowinv, 0.0, h->Wi8, 2 * npad * npad, 2 * npad));
-  // one K = 32 block of all three planes per TMA box (64 B x rows x 3, SWIZZLE_64B): 128 rows of W, one tile of
-  // candidates (the scheme's tile width)
-  const int bn = i8_tile_n(h->i8_radix256);
-  DFB_TRY(make_tensor_map_3d_u8(&h->tmWi8, h->Wi8, 2 * npad, npad, 3, 2 * npad, 2 * npad * npad, 64, 128, 3));
-  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8, h->Ki8, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, bn, 3));
-  DFB_TRY(make_tensor_map_3d_u8(&h->tmKi8_b, h->Ki8b, 2 * npad, h->chunk, 3, 2 * npad, 2 * h->chunk * npad, 64, bn, 3));
+  // TMA maps of one K = 32 block per box: one CTA's share of W's 128-row block, one tile of candidates
+  DFB_TRY(make_i8_maps(&h->tmWi8, h->Wi8, npad, npad, true, h->i8_radix256 != 0));
+  DFB_TRY(make_i8_maps(&h->tmKi8, h->Ki8, npad, h->chunk, false, h->i8_radix256 != 0));
+  DFB_TRY(make_i8_maps(&h->tmKi8_b, h->Ki8b, npad, h->chunk, false, h->i8_radix256 != 0));
   h->i8_ready = true;
   return 0;
 }
@@ -1353,9 +1351,9 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
   }
   DFB_CUDA_OK(cudaSetDevice(h->device));
   const int64_t K = (int64_t)n_rb * TILE, a_rows = K, b_rows = (int64_t)n_cb * bn;
-  CUtensorMap tmA, tmB;
-  DFB_TRY(make_tensor_map_3d_u8(&tmA, a_planes_dev, 2 * K, a_rows, 3, 2 * K, 2 * K * a_rows, 64, 128, 3));
-  DFB_TRY(make_tensor_map_3d_u8(&tmB, b_planes_dev, 2 * K, b_rows, 3, 2 * K, 2 * K * b_rows, 64, bn, 3));
+  I8Maps tmA, tmB;
+  DFB_TRY(make_i8_maps(&tmA, a_planes_dev, K, a_rows, true, radix256 != 0));
+  DFB_TRY(make_i8_maps(&tmB, b_planes_dev, K, b_rows, false, radix256 != 0));
   const int keep_group = h->last_c2_group;
   DFB_TRY(launch_score_i8_args(h, radix256 != 0, tmA, tmB, n_rb, n_cb, (int)K, partial_dev, ld_partial, rowscale_dev,
                                colscale, abort_count_dev));

@@ -53,6 +53,11 @@ struct ProfClass {
   double acc_ms = 0.0, acc_units = 0.0;
   int64_t acc_launches = 0;
 };
+// TMA maps of one operand of the int8 contraction (make_i8_maps in kernels.cu): its pair-interleaved digit planes and,
+// with radix-256 digits, digit 5 alone (the first half of plane 3; the second half is the unused sixth slot)
+struct I8Maps {
+  CUtensorMap planes, digit5;
+};
 }  // namespace dfb
 
 // The opaque handle of the C-ABI.
@@ -155,11 +160,11 @@ struct dfb_handle {
   cudaStream_t cp_stream = nullptr;   // H2D copies of page-locked host candidates, one batch ahead (api.cu: run_chunks)
   cudaEvent_t cp_fork = nullptr, cp_done[2] = {nullptr, nullptr}, cp_free[2] = {nullptr, nullptr};
   cudaEvent_t ks_fork = nullptr, ks_k[2] = {nullptr, nullptr}, ks_g[2] = {nullptr, nullptr};
-  CUtensorMap tmKi8_b;                     // map of the second digit buffer
+  dfb::I8Maps tmKi8_b;                     // maps of the second digit buffer
   int64_t last_overlapped = 0;             // diagnostics: chunks of the last call that went through the two-stream pipeline
   double* rowscale = nullptr; // npad  2^E_i
   double* rowinv = nullptr;   // npad  2^-E_i
-  CUtensorMap tmWi8, tmKi8;
+  dfb::I8Maps tmWi8, tmKi8;
   int i8_impl = 2;            // 0, 1 = radix-128 digits only; 2 = digit scheme chosen by i8_radix_opt
   int i8_radix_opt = -1;      // digit scheme with i8_impl 2: -1 auto (radix 256 when its bound allows), 0 = 128, 1 = 256
   int i8_radix256 = 0;        // scheme in use for the current posterior (set by prepare_i8)

@@ -23,13 +23,16 @@ constexpr int i8_tile_n(bool radix256) { return radix256 ? 64 : 32; }
 int make_tensor_map_3d_u8(CUtensorMap* out, const void* base, int64_t cols, int64_t rows, int64_t planes,
                           int64_t row_ld_bytes, int64_t plane_stride_bytes, int box_cols, int box_rows,
                           int box_planes);
+// Maps of one operand of score_i8_kernel: three pair-interleaved planes of rows x 2K bytes each, back to back.  W
+// (w_operand) is read in boxes of the rows one CTA of a cluster loads, K_* in boxes of one candidate tile.
+int make_i8_maps(I8Maps* out, const void* planes, int64_t K, int64_t rows, bool w_operand, bool radix256);
 int launch_row_exponent(dfb_handle* h, const double* M, int64_t ld, int64_t rows, int64_t cols,
                         double* rowscale, double* rowinv);
 int launch_slice_i8(dfb_handle* h, const double* M, int64_t ld, int64_t rows, int64_t cols,
                     const double* rowinv, double inv_const, void* out, int64_t plane_bytes,
                     int64_t out_ld_bytes);
 // radix256 selects the digit scheme of the planes behind tmA / tmB (the scoring path passes h->i8_radix256)
-int launch_score_i8_args(dfb_handle* h, bool radix256, const CUtensorMap& tmA, const CUtensorMap& tmB, int n_rb,
+int launch_score_i8_args(dfb_handle* h, bool radix256, const I8Maps& tmA, const I8Maps& tmB, int n_rb,
                          int n_cb, int K, double* partial, int64_t ld_partial, const double* rowscale, double colscale,
                          const int* abort_count = nullptr);
 

@@ -332,7 +332,9 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *  "kstar_overlap": 1 = K_* of chunk c+1 on a second stream beside the contraction of chunk c (two-stream pipeline with
  *                 double-buffered digit planes); default 0.
  *  "i8_c2_group": candidate tiles per group of the int8 kernel's tile order (tiles of 64 candidates with radix-256
- *                 digits, 32 with radix-128); 0 (default) = 8; query "last_c2_group".
+ *                 digits, 32 with radix-128); 0 (default) = 8.  The kernel runs in clusters of two CTAs on adjacent
+ *                 tiles that share one load of the W digits, so an odd group is rounded up by one tile; query
+ *                 "last_c2_group" gives the group in effect.
  *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_impl", "i8_radix256", "score_impl",
