@@ -92,7 +92,6 @@ PROTOTYPES = {
   'dfb_fill_candidates': (C.c_int, [_P, C.c_uint64, _I64, _I64, _I32, C.POINTER(_D), C.POINTER(_D), _P]),
   'dfb_measure_peak': (C.c_int, [C.c_int, C.c_int, C.POINTER(_D)]),
   'dfb_launch_count': (_I64, [_P]),
-  'dfb_debug_trace': (C.c_int, [_P, _I64]),
   'dfb_debug_score_i8': (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _P, _D, _P, _P, _I64]),
   'dfb_debug_copy': (C.c_int, [_P, C.c_char_p, _P, _I64]),
   'dfb_set_option': (C.c_int, [_P, C.c_char_p, _I64]),

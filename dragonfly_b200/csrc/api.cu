@@ -56,12 +56,9 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   double* te_xs = c.take<double>((size_t)npad * DFB_MAX_SLOTS);
   double* te_nrm = c.take<double>((size_t)npad * DFB_MAX_FACTORS);
   double* Ks = c.take<double>((size_t)chunk * npad);
-  // three pair-interleaved digit planes (2 bytes per entry each) + one compact plane of the leading digit
-  int8_t* Wi8 = c.take<int8_t>((size_t)7 * npad * npad);
-  int8_t* Ki8 = c.take<int8_t>((size_t)7 * chunk * npad);
-  int8_t* Ki8b = c.take<int8_t>((size_t)7 * chunk * npad);
-  double* mu_b = c.take<double>((size_t)chunk);
-  double* kssv_b = c.take<double>((size_t)chunk);
+  // three pair-interleaved digit planes (2 bytes per entry each)
+  int8_t* Wi8 = c.take<int8_t>((size_t)6 * npad * npad);
+  int8_t* Ki8 = c.take<int8_t>((size_t)6 * chunk * npad);
   double* cprep = c.take<double>((size_t)chunk * 10);
   double* mu_part = c.take<double>((size_t)(npad / 64 + 2) * chunk);      // per 64-point block partial sums of mu
   double* rowscale = c.take<double>((size_t)npad);
@@ -93,7 +90,7 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   double* ext_save = c.take<double>((size_t)(2 * TILE + 1) * npad + TILE);
   if (h != nullptr && base != nullptr) {
     h->ext_save = ext_save;
-    h->Ki8b = Ki8b; h->mu_b = mu_b; h->kssv_b = kssv_b; h->cprep = cprep; h->mu_part = mu_part;
+    h->cprep = cprep; h->mu_part = mu_part;
     h->T = T; h->W = W; h->Dinv = Dinv; h->X = X; h->yc = yc; h->alpha = alpha;
     h->tr.xs = tr_xs; h->tr.nrm = tr_nrm; h->te.xs = te_xs; h->te.nrm = te_nrm;
     h->Ks = Ks; h->Wi8 = Wi8; h->Ki8 = Ki8; h->rowscale = rowscale; h->rowinv = rowinv; h->list_idx = list_idx; h->list_X = list_X; h->list_count = list_count; h->list_s8 = list_s8; h->list_err = list_err; h->blk_lb = blk_lb; h->best_lb = best_lb; h->partial = partial; h->mu = mu; h->sd = sd; h->score = score; h->kssv = kssv; h->stage = stage;
@@ -358,11 +355,11 @@ static int prepare_i8(dfb_handle* h) {
   DFB_TRY(launch_vec_max(h, h->rowscale, h->n, h->red + 4));
   DFB_CUDA_OK(cudaMemcpyAsync(&h->i8_rowscale_max, h->red + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  // Digit scheme (i8_impl 2): five radix-256 digits (15 products) when the a-priori bound of
+  // Digit scheme: five radix-256 digits (15 products) when the a-priori bound of
   // that coarser expansion passes for the training kernel, else six radix-128 digits (21 products).  The
   // radix-256 groups also need int32 headroom: 5 K 2^14 < 2^31.
   h->i8_radix256 = 0;
-  if (h->i8_impl == 2 && h->i8_radix_opt != 0 && npad <= 24576) {
+  if (h->i8_radix_opt != 0 && npad <= 24576) {
     h->i8_radix256 = 1;
     const dfb_kernel_desc& dtr = h->desc_tr;
     if (h->i8_radix_opt < 0 && dtr.kss > 0.0 && i8_sigma2_bound(h, dtr) > I8_BOUND_LIMIT)
@@ -373,8 +370,25 @@ static int prepare_i8(dfb_handle* h) {
   // TMA maps of one K = 32 block per box: one CTA's share of W's 128-row block, one tile of candidates
   DFB_TRY(make_i8_maps(&h->tmWi8, h->Wi8, npad, npad, true, h->i8_radix256 != 0));
   DFB_TRY(make_i8_maps(&h->tmKi8, h->Ki8, npad, h->chunk, false, h->i8_radix256 != 0));
-  DFB_TRY(make_i8_maps(&h->tmKi8_b, h->Ki8b, npad, h->chunk, false, h->i8_radix256 != 0));
   h->i8_ready = true;
+  return 0;
+}
+
+// The scoring state of the current posterior, rebuilt on request: with i8 the int8 digit planes of W (when option
+// score_impl asks for them), with tma the fp64 TMA maps of W and Ks (when option gemm_impl does).  Both need W = L^-1;
+// without it they are only marked not ready.  The TMA maps describe (address, npad) only, so a posterior that changed W
+// but not npad keeps them.
+static int prepare_scoring(dfb_handle* h, bool i8, bool tma) {
+  if (i8) h->i8_ready = false;
+  if (tma) h->tma_ready = false;
+  if (!h->have_post || !h->have_w) return 0;
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  if (i8 && (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024))) DFB_TRY(prepare_i8(h));
+  if (tma && h->gemm_impl == 1) {
+    DFB_TRY(make_tensor_map_2d_f64(&h->tmW, h->W, h->npad, h->npad, h->npad));
+    DFB_TRY(make_tensor_map_2d_f64(&h->tmK, h->Ks, h->chunk, h->npad, h->npad));
+    h->tma_ready = true;
+  }
   return 0;
 }
 
@@ -465,9 +479,7 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   }
   h->have_post = true;
   h->have_w = true;
-  h->i8_ready = false;
-  if (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024)) DFB_TRY(prepare_i8(h));
-  // the fp64 TMA maps of W and Ks describe (address, npad) only: still valid
+  DFB_TRY(prepare_scoring(h, true, false));     // npad is unchanged: the fp64 TMA maps stay valid
   if (lml_out_host != nullptr) {
     const double quad = (flags == DFB_BUILD_FULL) ? red[1] : red[2];
     *lml_out_host = -0.5 * quad - red[0] - 0.5 * (double)n * log(2.0 * M_PI);
@@ -498,31 +510,9 @@ static ChunkMode chunk_mode(bool want_std, bool do_argmax, bool use_i8, const in
 }
 constexpr int64_t SMALL_EVAL_M = 32;      // up to four 8-wide passes over W's rows (105 MB each at N = 5000): still ~10x cheaper than one 128-wide tile pass
 
-static int ensure_ks_stream(dfb_handle* h) {
-  if (h->ks_stream != nullptr) return 0;
-  int lo = 0, hi = 0;
-  DFB_CUDA_OK(cudaDeviceGetStreamPriorityRange(&lo, &hi));      // lo = least priority: the contraction's CTAs go first
-  if (getenv("DFB200_KS_PRIO") != nullptr) {                    // diagnostics: 0 = equal priorities, 1 = swapped
-    if (atoi(getenv("DFB200_KS_PRIO")) == 0) hi = lo; else { const int t = lo; lo = hi; hi = t; }
-  }
-  DFB_CUDA_OK(cudaStreamCreateWithPriority(&h->ks_stream, cudaStreamNonBlocking, lo));
-  DFB_CUDA_OK(cudaStreamCreateWithPriority(&h->gs_stream, cudaStreamNonBlocking, hi));
-  DFB_CUDA_OK(cudaEventCreateWithFlags(&h->ks_fork, cudaEventDisableTiming));
-  DFB_CUDA_OK(cudaEventCreateWithFlags(&h->ks_join, cudaEventDisableTiming));
-  for (int i = 0; i < 2; i++) {
-    DFB_CUDA_OK(cudaEventCreateWithFlags(&h->ks_k[i], cudaEventDisableTiming));
-    DFB_CUDA_OK(cudaEventCreateWithFlags(&h->ks_g[i], cudaEventDisableTiming));
-  }
-  return 0;
-}
-
-// Per chunk two stages:
+// Per chunk two stages, back to back on the handle's stream:
 //   K: (host candidates: staging copy) K_* rows / digit planes + mu + k(x*,x*)      fp64 pipe
 //   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
-// With option kstar_overlap and the int8 contraction the stages of consecutive chunks are software-pipelined over two
-// streams: K(c+1) runs on h->ks_stream into the second digit buffer while G(c) runs on the caller's stream.
-// Events carry the two dependencies per buffer: K(c) -> G(c) and G(c) -> K(c+2).  Everything else is unchanged: the
-// arithmetic per chunk, the order of the arg-max folds (G stages stay in stream order) and therefore every result.
 static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
                       int32_t space, double mean_const, ChunkOut out, const ChunkMode& md) {
   const bool want_std = md.want_std, do_argmax = md.do_argmax;
@@ -540,18 +530,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   const int nb = (int)(npad / TILE);
   if (do_argmax) DFB_TRY(launch_reset_best(h));
   const bool i8 = want_std && md.use_i8;
-  const bool seg_ok = i8 && h->i8_fuse && h->kstar_fast && h->kstar_seg && h->i8_impl == 2 && h->i8_radix256;
-  const bool pipelined = i8 && h->i8_impl == 2 && h->kstar_overlap && m > Mc;
-  StreamSwap guard(h);
-  cudaStream_t s_user = guard.user, s_k = s_user, s_g = s_user;
-  if (pipelined) {
-    DFB_TRY(ensure_ks_stream(h));
-    s_k = h->ks_stream;
-    s_g = h->gs_stream;
-    DFB_CUDA_OK(cudaEventRecord(h->ks_fork, s_user));
-    DFB_CUDA_OK(cudaStreamWaitEvent(s_k, h->ks_fork, 0));
-    DFB_CUDA_OK(cudaStreamWaitEvent(s_g, h->ks_fork, 0));
-  }
+  const bool seg_ok = i8 && h->i8_fuse && h->kstar_fast && h->kstar_seg && h->i8_radix256;
   // host candidates are staged in batches of as many whole chunks as the staging buffer holds
   // (chunk x DFB_MAX_SLOTS doubles), so a 6-column candidate matrix needs 1 copy per ~21 chunks
   const int64_t stage_rows = (Mc * DFB_MAX_SLOTS / dc) / Mc * Mc;
@@ -576,7 +555,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       }
       DFB_CUDA_OK(cudaEventCreateWithFlags(&h->cp_fork, cudaEventDisableTiming));
     }
-    DFB_CUDA_OK(cudaEventRecord(h->cp_fork, s_user));     // the copy stream starts after everything already on the caller's stream
+    DFB_CUDA_OK(cudaEventRecord(h->cp_fork, h->stream));  // the copy stream starts after everything already on the caller's stream
     DFB_CUDA_OK(cudaStreamWaitEvent(h->cp_stream, h->cp_fork, 0));
   }
   auto issue_copy = [&](int64_t bi) -> int {               // batch bi -> half bi % 2, on the copy stream
@@ -589,81 +568,61 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     return 0;
   };
   const int64_t n_chunks = (m + Mc - 1) / Mc;
-  const double* xc_of[2] = {nullptr, nullptr};
+  const int* abort_count = md.collect ? h->list_count : nullptr;
+  const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
+                     (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
 
-  auto stage_k = [&](int64_t ci) -> int {
-    const int b = pipelined ? (int)(ci & 1) : 0;
+  for (int64_t ci = 0; ci < n_chunks; ci++) {
     const int64_t c0 = ci * Mc;
     const int64_t mc = (m - c0 < Mc) ? (m - c0) : Mc;
     const int64_t m_rows = round_up(mc, TILE);
-    h->stream = s_k;
-    if (pipelined && ci >= 2) DFB_CUDA_OK(cudaStreamWaitEvent(s_k, h->ks_g[b], 0));     // G(ci-2) is done with buffer b
     const double* xc_dev;
     if (space == DFB_HOST && dbuf) {
       const int64_t bi = c0 / half_rows;
       if (c0 % half_rows == 0) {                           // first chunk of a batch
         if (bi == 0) DFB_TRY(issue_copy(0));
         if ((bi + 1) * half_rows < m) DFB_TRY(issue_copy(bi + 1));
-        DFB_CUDA_OK(cudaStreamWaitEvent(s_k, h->cp_done[bi & 1], 0));
+        DFB_CUDA_OK(cudaStreamWaitEvent(h->stream, h->cp_done[bi & 1], 0));
       }
       xc_dev = h->stage + (bi & 1) * half_rows * dc + (c0 - bi * half_rows) * dc;
     } else if (space == DFB_HOST) {
       if (c0 >= staged_hi) {
-        // the shortlist collection of earlier chunks reads the staged rows: wait for the latest G stage
-        if (pipelined && ci >= 1) DFB_CUDA_OK(cudaStreamWaitEvent(s_k, h->ks_g[(ci - 1) & 1], 0));
         staged_lo = c0;
         staged_hi = (m - c0 < stage_rows) ? m : c0 + stage_rows;
         DFB_CUDA_OK(cudaMemcpyAsync(h->stage, Xc + staged_lo * dc, sizeof(double) * (staged_hi - staged_lo) * dc,
-                                    cudaMemcpyHostToDevice, s_k));
+                                    cudaMemcpyHostToDevice, h->stream));
       }
       xc_dev = h->stage + (c0 - staged_lo) * dc;
     } else {
       xc_dev = Xc + c0 * dc;
     }
-    xc_of[b] = xc_dev;
-    double* mu_dev = (space == DFB_DEVICE && out.mu) ? out.mu + c0 : (b ? h->mu_b : h->mu);
-    double* kss_dev = b ? h->kssv_b : h->kssv;
-    int8_t* planes = b ? h->Ki8b : h->Ki8;
-    const int* abort_count = md.collect ? h->list_count : nullptr;
+    double* mu_dev = (space == DFB_DEVICE && out.mu) ? out.mu + c0 : h->mu;
+    double* sd_dev = (space == DFB_DEVICE && out.sd) ? out.sd + c0 : h->sd;
+    double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
+                                                         : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
+
+    // K stage
     DFB_TRY(prof_begin(h, DFB_PROF_KSTAR));
     int fused_digits = 0;
     if (seg_ok)
       DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
-                               mu_dev, kss_dev, planes, 2 * h->chunk * npad, 2 * npad, 1.0 / i8_colscale(desc), h->cprep,
+                               mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad, 1.0 / i8_colscale(desc), h->cprep,
                                h->mu_part, Mc, &fused_digits, abort_count));
     if (!fused_digits && i8 && h->i8_fuse)
       DFB_TRY(launch_kstar_i8(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, xc_dev, mc, dc, m_rows, h->n, npad,
-                              mean_const, mu_dev, kss_dev, planes, 2 * h->chunk * npad, 2 * npad,
+                              mean_const, mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad,
                               1.0 / i8_colscale(desc), &fused_digits, abort_count));
     if (!fused_digits) {
       DFB_TRY(launch_kstar(h, d_desc, desc, 0, ss.xs, ss.nrm, npad, h->alpha, xc_dev, mc, dc, m_rows,
-                           h->Ks, npad, h->n, npad, mean_const, mu_dev, want_std ? kss_dev : nullptr));
+                           h->Ks, npad, h->n, npad, mean_const, mu_dev, want_std ? h->kssv : nullptr));
       if (i8)     // K_* = 2^F * digits: |K_*| <= k(x,x) for every supported (stationary, non-negative) kernel
-        DFB_TRY(launch_slice_i8(h, h->Ks, npad, m_rows, npad, nullptr, 1.0 / i8_colscale(desc), planes,
+        DFB_TRY(launch_slice_i8(h, h->Ks, npad, m_rows, npad, nullptr, 1.0 / i8_colscale(desc), h->Ki8,
                                 2 * h->chunk * npad, 2 * npad));
     }
     DFB_TRY(prof_end(h, DFB_PROF_KSTAR, (double)mc));
-    if (pipelined) DFB_CUDA_OK(cudaEventRecord(h->ks_k[b], s_k));
-    return 0;
-  };
 
-  auto stage_g = [&](int64_t ci) -> int {
-    const int b = pipelined ? (int)(ci & 1) : 0;
-    const int64_t c0 = ci * Mc;
-    const int64_t mc = (m - c0 < Mc) ? (m - c0) : Mc;
-    const int64_t m_rows = round_up(mc, TILE);
-    h->stream = s_g;
-    if (pipelined) DFB_CUDA_OK(cudaStreamWaitEvent(s_g, h->ks_k[b], 0));
-    const double* xc_dev = xc_of[b];
-    double* mu_dev = (space == DFB_DEVICE && out.mu) ? out.mu + c0 : (b ? h->mu_b : h->mu);
-    double* kss_dev = b ? h->kssv_b : h->kssv;
-    double* sd_dev = (space == DFB_DEVICE && out.sd) ? out.sd + c0 : h->sd;
-    double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
-                                                         : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
-    const int* abort_count = md.collect ? h->list_count : nullptr;
+    // G stage
     int small_warps = 0;
-    const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
-                       (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
     if (small) {
       // the padded rows of K_* beyond mc are zero, so an 8-wide pass may run past mc (within the 128-row tile)
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
@@ -678,7 +637,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
         const double colscale = i8_colscale(desc);
-        DFB_TRY(launch_score_i8_args(h, h->i8_radix256 != 0, h->tmWi8, b ? h->tmKi8_b : h->tmKi8, nb,
+        DFB_TRY(launch_score_i8_args(h, h->i8_radix256 != 0, h->tmWi8, h->tmKi8, nb,
                                      (int)(m_rows / i8_tile_n(h->i8_radix256)), (int)npad, h->partial, Mc,
                                      h->rowscale, colscale, abort_count));
       } else if (h->gemm_impl == 1 && h->tma_ready) {
@@ -693,7 +652,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     }
     if (want_std || do_argmax || sc_dev != nullptr) {
       DFB_TRY(prof_begin(h, DFB_PROF_ACQ));
-      DFB_TRY(launch_acq(h, acq, mu_dev, h->partial, small ? SMALL_EVAL_M : Mc, small ? small_warps : nb, kss_dev, mc, c0,
+      DFB_TRY(launch_acq(h, acq, mu_dev, h->partial, small ? SMALL_EVAL_M : Mc, small ? small_warps : nb, h->kssv, mc, c0,
                          want_std ? 1 : 0, want_std ? sd_dev : nullptr, sc_dev, do_argmax, md.idx_map,
                          md.collect ? &md.em : nullptr));
       if (md.collect)
@@ -702,37 +661,17 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     }
     if (space == DFB_HOST) {
       if (out.mu)
-        DFB_CUDA_OK(cudaMemcpyAsync(out.mu + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, s_g));
+        DFB_CUDA_OK(cudaMemcpyAsync(out.mu + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
       if (out.sd && want_std)
-        DFB_CUDA_OK(cudaMemcpyAsync(out.sd + c0, sd_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, s_g));
+        DFB_CUDA_OK(cudaMemcpyAsync(out.sd + c0, sd_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
       if (out.score)
-        DFB_CUDA_OK(cudaMemcpyAsync(out.score + c0, sc_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, s_g));
+        DFB_CUDA_OK(cudaMemcpyAsync(out.score + c0, sc_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
     }
-    if (pipelined) DFB_CUDA_OK(cudaEventRecord(h->ks_g[b], s_g));
     if (dbuf) {                                            // last chunk of its batch: the half may be overwritten
       const int64_t bi = c0 / half_rows;
       const int64_t b_hi = (m - bi * half_rows < half_rows) ? m : (bi + 1) * half_rows;
-      if (c0 + Mc >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], s_g));
+      if (c0 + Mc >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
     }
-    return 0;
-  };
-
-  if (!pipelined) {
-    for (int64_t ci = 0; ci < n_chunks; ci++) {
-      DFB_TRY(stage_k(ci));
-      DFB_TRY(stage_g(ci));
-    }
-  } else {
-    // issue order: the contraction of chunk c is enqueued BEFORE the K_* of chunk c+1, so that the block scheduler
-    // places the contraction's CTAs first and the K_* CTAs fill the registers / shared memory left over
-    DFB_TRY(stage_k(0));
-    for (int64_t ci = 0; ci < n_chunks; ci++) {
-      DFB_TRY(stage_g(ci));
-      if (ci + 1 < n_chunks) DFB_TRY(stage_k(ci + 1));
-    }
-    DFB_CUDA_OK(cudaEventRecord(h->ks_join, s_g));          // every K stage precedes a G stage: joining G joins both
-    DFB_CUDA_OK(cudaStreamWaitEvent(s_user, h->ks_join, 0));
-    h->last_overlapped = n_chunks;
   }
   return 0;
 }
@@ -788,10 +727,6 @@ void dfb_destroy(dfb_handle* h) {
   if (h->cp_stream != nullptr) {
     cudaStreamDestroy(h->cp_stream); cudaEventDestroy(h->cp_fork);
     for (int i = 0; i < 2; i++) { cudaEventDestroy(h->cp_done[i]); cudaEventDestroy(h->cp_free[i]); }
-  }
-  if (h->ks_stream != nullptr) {
-    cudaStreamDestroy(h->ks_stream); cudaStreamDestroy(h->gs_stream); cudaEventDestroy(h->ks_fork); cudaEventDestroy(h->ks_join);
-    for (int i = 0; i < 2; i++) { cudaEventDestroy(h->ks_k[i]); cudaEventDestroy(h->ks_g[i]); }
   }
   if (h->prof != nullptr) {
     for (int c = 0; c < PROF_CLASSES; c++)
@@ -912,14 +847,7 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   h->noise_plus_jitter = noise_var + jitter;
   h->have_post = true;
   h->have_w = with_bottom;
-  h->i8_ready = false;
-  if (with_bottom && (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024))) DFB_TRY(prepare_i8(h));
-  h->tma_ready = false;
-  if (with_bottom && h->gemm_impl == 1) {
-    DFB_TRY(make_tensor_map_2d_f64(&h->tmW, h->W, npad, npad, npad));
-    DFB_TRY(make_tensor_map_2d_f64(&h->tmK, h->Ks, h->chunk, npad, npad));
-    h->tma_ready = true;
-  }
+  DFB_TRY(prepare_scoring(h, true, true));
   if (lml_out_host != nullptr) {
     const double quad = (flags == DFB_BUILD_FULL) ? red[1] : red[2];
     *lml_out_host = -0.5 * quad - red[0] - 0.5 * (double)n * log(2.0 * M_PI);
@@ -989,8 +917,7 @@ int dfb_restore_posterior(dfb_handle* h) {
   h->tr_prepped = h->te_prepped = false;
   DFB_TRY(launch_transpose(h, h->T + npad * npad, h->W, npad));
   h->have_post = h->have_w = true;
-  h->i8_ready = false;
-  if (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024)) DFB_TRY(prepare_i8(h));
+  DFB_TRY(prepare_scoring(h, true, false));     // npad is unchanged: the fp64 TMA maps stay valid
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -1334,8 +1261,6 @@ int dfb_ts_argmax(dfb_handle* h, const double* samples_dev, int64_t ld, int32_t 
 
 int64_t dfb_launch_count(dfb_handle* h) { return h ? h->launches : 0; }
 
-int dfb_debug_trace(void* buf_dev, int64_t cap_records) { return debug_set_trace(buf_dev, (long long)cap_records); }
-
 // The production int8 contraction on caller-owned digit planes (tests/test_gpu_i8_exact.py): A = n_rb * 128 rows of
 // W digits, B = n_cb tiles of K_* digits, K = n_rb * 128, both in the pair-interleaved three-plane layout of
 // gemm_i8.cuh.  Tensor maps and launch as in prepare_i8 / run_chunks; the handle's digit scheme and buffers are untouched.
@@ -1400,11 +1325,10 @@ int dfb_query(dfb_handle* h, const char* name, double* out) {
   if (strcmp(name, "chunk") == 0) { *out = (double)h->chunk; return 0; }
   if (strcmp(name, "npad") == 0) { *out = (double)h->npad; return 0; }
   if (strcmp(name, "last_c2_group") == 0) { *out = (double)h->last_c2_group; return 0; }
-  if (strcmp(name, "last_overlapped") == 0) { *out = (double)h->last_overlapped; return 0; }     // chunks of the last PIPELINED pass
   if (strcmp(name, "i8_bound_limit") == 0) { *out = I8_BOUND_LIMIT; return 0; }
   if (strcmp(name, "score_impl") == 0) { *out = (double)h->score_impl; return 0; }
   if (strcmp(name, "i8_ready") == 0) { *out = h->i8_ready ? 1.0 : 0.0; return 0; }
-  if (strcmp(name, "i8_impl") == 0) { *out = (double)h->i8_impl; return 0; }
+  if (strcmp(name, "i8_impl") == 0) { *out = 2.0; return 0; }     // bench.py reads it; the digit scheme is option i8_radix
   if (strcmp(name, "i8_radix256") == 0) { *out = (double)h->i8_radix256; return 0; }
   set_error("unknown query '%s'", name);
   return -1;
@@ -1416,14 +1340,7 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "gemm_impl") == 0) {
     if (value != 0 && value != 1) { set_error("gemm_impl must be 0 (cp.async) or 1 (TMA)"); return -1; }
     h->gemm_impl = (int)value;
-    h->tma_ready = false;
-    if (value == 1 && h->have_post && h->have_w) {
-      DFB_CUDA_OK(cudaSetDevice(h->device));
-      DFB_TRY(make_tensor_map_2d_f64(&h->tmW, h->W, h->npad, h->npad, h->npad));
-      DFB_TRY(make_tensor_map_2d_f64(&h->tmK, h->Ks, h->chunk, h->npad, h->npad));
-      h->tma_ready = true;
-    }
-    return 0;
+    return prepare_scoring(h, false, true);
   }
   if (strcmp(name, "kstar_fast") == 0) { h->kstar_fast = value ? 1 : 0; return 0; }
   if (strcmp(name, "lookahead") == 0) { h->lookahead = value ? 1 : 0; return 0; }
@@ -1431,14 +1348,7 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "i8_fuse") == 0) { h->i8_fuse = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_seg") == 0) { h->kstar_seg = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_rows64") == 0) { h->kstar_rows64 = value ? 1 : 0; return 0; }
-  if (strcmp(name, "kstar_overlap") == 0) { h->kstar_overlap = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_unguarded") == 0) { h->i8_unguarded = value ? 1 : 0; return 0; }
-  if (strcmp(name, "i8_impl") == 0) {
-    if (value < 0 || value > 2) { set_error("i8_impl must be 0 or 1 (radix-128 digits only) or 2 (digit scheme by i8_radix)"); return -1; }
-    h->i8_impl = (int)value;
-    if (h->i8_ready) { DFB_CUDA_OK(cudaSetDevice(h->device)); DFB_TRY(prepare_i8(h)); }   // re-slice W in the new scheme
-    return 0;
-  }
   if (strcmp(name, "i8_radix") == 0) {
     if (value < -1 || value > 1) { set_error("i8_radix must be -1 (auto), 0 (radix 128) or 1 (radix 256)"); return -1; }
     h->i8_radix_opt = (int)value;
@@ -1450,12 +1360,7 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "score_impl") == 0) {
     if (value < 0 || value > 2) { set_error("score_impl must be 0 (fp64 DMMA), 1 (int8-slice wgmma) or 2 (auto)"); return -1; }
     h->score_impl = (int)value;
-    h->i8_ready = false;
-    if ((value == 1 || (value == 2 && h->n >= 1024)) && h->have_post && h->have_w) {
-      DFB_CUDA_OK(cudaSetDevice(h->device));
-      DFB_TRY(prepare_i8(h));
-    }
-    return 0;
+    return prepare_scoring(h, true, false);
   }
   set_error("unknown option '%s'", name);
   return -1;

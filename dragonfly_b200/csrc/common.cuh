@@ -144,29 +144,16 @@ struct dfb_handle {
   int i8_fuse = 1;            // K_* kernel emits the digit planes itself (no fp64 K_* round trip)
   int kstar_seg = 1;          // second-generation digit kernel (kstar_seg_kernel) where it applies
   int kstar_rows64 = 1;       // ... and its fp64-row form for the materialising K_* build of the fp64 scoring paths
-  int kstar_overlap = 0;      // option: chunk c+1's K_* on a second stream while chunk c is contracted (api.cu: run_chunks)
-  int8_t* Wi8 = nullptr;      // 3 pair-interleaved planes [npad][2 npad] + the compact leading plane [npad][npad]
+  int8_t* Wi8 = nullptr;      // 3 pair-interleaved planes [npad][2 npad]
   int8_t* Ki8 = nullptr;      // the same for the K_* chunk
-  // K_* / contraction overlap (api.cu: run_chunks): second buffer of everything the K_* stage hands to the
-  // contraction stage, the scratch of the second-generation K_* kernel, the second stream and its events
-  int8_t* Ki8b = nullptr;
-  double* mu_b = nullptr;
-  double* kssv_b = nullptr;
   double* cprep = nullptr;    // chunk x 10 scaled candidate rows (cand_prep_kernel)
   double* mu_part = nullptr;  // (npad / 64 + 2) x chunk
-  cudaStream_t ks_stream = nullptr;   // K stage (least priority)
-  cudaStream_t gs_stream = nullptr;   // G stage (greatest priority: the contraction's CTAs are placed first)
-  cudaEvent_t ks_join = nullptr;
   cudaStream_t cp_stream = nullptr;   // H2D copies of page-locked host candidates, one batch ahead (api.cu: run_chunks)
   cudaEvent_t cp_fork = nullptr, cp_done[2] = {nullptr, nullptr}, cp_free[2] = {nullptr, nullptr};
-  cudaEvent_t ks_fork = nullptr, ks_k[2] = {nullptr, nullptr}, ks_g[2] = {nullptr, nullptr};
-  dfb::I8Maps tmKi8_b;                     // maps of the second digit buffer
-  int64_t last_overlapped = 0;             // diagnostics: chunks of the last call that went through the two-stream pipeline
   double* rowscale = nullptr; // npad  2^E_i
   double* rowinv = nullptr;   // npad  2^-E_i
   dfb::I8Maps tmWi8, tmKi8;
-  int i8_impl = 2;            // 0, 1 = radix-128 digits only; 2 = digit scheme chosen by i8_radix_opt
-  int i8_radix_opt = -1;      // digit scheme with i8_impl 2: -1 auto (radix 256 when its bound allows), 0 = 128, 1 = 256
+  int i8_radix_opt = -1;      // digit scheme: -1 auto (radix 256 when its bound allows), 0 = 128, 1 = 256
   int i8_radix256 = 0;        // scheme in use for the current posterior (set by prepare_i8)
 
   // model state

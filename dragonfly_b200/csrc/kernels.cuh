@@ -66,7 +66,6 @@ int launch_add_row_vector(dfb_handle* h, double* M, int64_t ld, int64_t rows, in
 int launch_diag_max(dfb_handle* h, const double* M, int64_t ld, int64_t n, double* out);
 int launch_fill(dfb_handle* h, double* p, int64_t n, double v);
 int launch_set_diag(dfb_handle* h, double* M, int64_t ld, int64_t from, int64_t to, double v, int add);
-int debug_set_trace(void* buf, long long cap_records);
 // LML gradients: reduction of (alpha alpha^T - K^-1) o dK/dparam over lower tiles of row blocks [rb0, rb0 + n_rb)
 int launch_lml_grad_tiles(dfb_handle* h, const dfb_kernel_desc* d_desc, const double* xs, const double* nrm, int64_t npad,
                           const double* alpha, const double* Kinv, int64_t ldk, int rb0, int n_rb, int nb, int64_t n,

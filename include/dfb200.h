@@ -274,10 +274,6 @@ int dfb_ts_draws(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, dou
 
 /* Counters for bench.py: number of kernels this handle has launched. */
 int64_t dfb_launch_count(dfb_handle* h);
-/* Diagnostics: arm (buf_dev = device buffer of 1 + 4 * cap_records 64-bit words, zeroed) or disarm (NULL) the per-CTA
- * trace of the K_* kernel of the overlapped scoring pipeline: record = (kind << 32 | SM id, start ns,
- * end ns, CTA index), buf[0] = number of records wanted.  tools/trace_overlap.py reads it. */
-int dfb_debug_trace(void* buf_dev, int64_t cap_records);
 /* Diagnostics (tests/test_gpu_i8_exact.py), not on the product path: runs the int8 scoring contraction (gemm_i8.cuh)
  * on caller-owned digit planes in its pair-interleaved layout, three planes each: A = n_rb * 128 rows of W digits,
  * B = n_cb * BN rows of K_* digits (BN = 64 with radix256 = 1, 32 with radix-128 digits), both with K = n_rb * 128
@@ -289,7 +285,7 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
                        double* partial_dev, int64_t ld_partial);
 /* Diagnostics: device-to-device copy of one internal buffer of the current state; bytes must equal its size (query
  * "npad" and "chunk"): "W" (fp64 L^-1, npad^2), "Wi8" (its three digit planes, 6 npad^2 bytes), "rowscale" (npad
- * doubles), "Ki8" (the three K_* digit planes of the first chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
+ * doubles), "Ki8" (the three K_* digit planes of the chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
  * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk).
  * Synchronises. */
 int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
@@ -313,11 +309,10 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *                     configurations), not a worst-case bound.  The screen is skipped when the
  *                     bound exceeds 5e-9 ABSOLUTE (half the 1e-8 sigma^2 contract, whatever the kernel scale;
  *                     query "i8_bound_limit") or n < 1024.
- *  "i8_impl"    : digit schemes the int8 path (gemm_i8.cuh, one wgmma kernel) may use (switching re-slices W):
- *                 2 (default) = as option "i8_radix" says; 0, 1 = six radix-128 digits only.
- *  "i8_radix"   : digit scheme with i8_impl 2: 1 = five radix-256 digits, 15 products; 0 = six radix-128 digits,
- *                 21 products (about 12x more accurate); -1 (default) = radix 256 whenever its a-priori bound is
- *                 below 5e-9 (absolute) for the training kernel, else radix 128.
+ *  "i8_radix"   : digit scheme of the int8 path (gemm_i8.cuh, one wgmma kernel; switching re-slices W): 1 = five
+ *                 radix-256 digits, 15 products; 0 = six radix-128 digits, 21 products (about 12x more accurate);
+ *                 -1 (default) = radix 256 whenever its a-priori bound is below 5e-9 (absolute) for the training
+ *                 kernel, else radix 128.
  *  "i8_fuse"    : 1 (default) = the K_* kernel emits the int8 digit planes directly, 0 = via an fp64 K_* buffer.
  *  "i8_unguarded": diagnostics only (tools/sweep_i8_bound.py): 1 = run the int8 path even when its a-priori bound exceeds
  *                 the limit, so that the bound can be compared with the measured error where it would refuse.
@@ -329,18 +324,17 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *  "kstar_seg"  : 1 (default) = second-generation K_* kernels (kstar_seg_kernel: training-stationary, digits from one FMA) for
  *                 plain SE / Matern on <= 8 dims; 0 = the round-1 kernels in the reference's operation order.
  *  "kstar_rows64": 1 (default) = the fp64 K_* rows of the fp64 scoring paths come from kstar_seg_kernel's row form too.
- *  "kstar_overlap": 1 = K_* of chunk c+1 on a second stream beside the contraction of chunk c (two-stream pipeline with
- *                 double-buffered digit planes); default 0.
  *  "i8_c2_group": candidate tiles per group of the int8 kernel's tile order (tiles of 64 candidates with radix-256
  *                 digits, 32 with radix-128); 0 (default) = 8.  The kernel runs in clusters of two CTAs on adjacent
  *                 tiles that share one load of the W digits, so an odd group is rounded up by one tile; query
  *                 "last_c2_group" gives the group in effect.
  *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
-/* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_impl", "i8_radix256", "score_impl",
+/* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_radix256", "score_impl",
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen
  * was voided and the call redone in fp64), "last_selfcheck_ratio" (max |s_int8 - s_fp64| / allowance over the last
- * shortlist; the model's margin is its inverse), "chunk", "npad", "last_c2_group", "last_overlapped". */
+ * shortlist; the model's margin is its inverse), "chunk", "npad", "last_c2_group"; "i8_impl" is always 2 (bench.py
+ * reports it). */
 int dfb_query(dfb_handle* h, const char* name, double* out);
 
 /* Per-kernel-class device timing with CUDA events on the handle's stream (bench.py's roofline):

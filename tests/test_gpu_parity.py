@@ -515,13 +515,11 @@ def test_tma_kernel_matches_cp_async_kernel(B):
 
 
 # ---- the int8-slice wgmma contraction (score_impl 1 / auto) ------------------------------------------------
-def _post_pair(B, kern, X, Y, mean_const, noise_var, chunk=0, i8_impl=None, i8_radix=None):
+def _post_pair(B, kern, X, Y, mean_const, noise_var, chunk=0, i8_radix=None):
   posts = []
   for impl in (0, 1):
     post = B.device.DevicePosterior(len(X), chunk=chunk)
     post.set_option('score_impl', impl)
-    if i8_impl is not None:      # None: the library default (2: scheme by option i8_radix)
-      post.set_option('i8_impl', i8_impl)
     if i8_radix is not None:
       post.set_option('i8_radix', i8_radix)
     post.set_kernel(B.kernel.build_descriptor(kern, train_dim=X.shape[1], cand_dim=X.shape[1]))
@@ -547,20 +545,19 @@ def _i8_kernels(B):
   }
 
 
-@pytest.mark.parametrize('i8_impl,i8_radix', [(2, 0), (2, 1), (2, -1)])
+@pytest.mark.parametrize('i8_radix', [0, 1, -1])
 @pytest.mark.parametrize('name', ['se', 'matern05', 'matern15', 'matern25', 'additive', 'mf_product'])
-def test_i8_sigma2_within_contract(B, name, i8_impl, i8_radix):
+def test_i8_sigma2_within_contract(B, name, i8_radix):
   """ Digit-sliced tensor-core contraction vs fp64 DMMA on the same posterior: mu identical (it never
       leaves fp64), |d sigma^2| far inside the 1e-8 contract and inside the library's own a-priori
       bound, for every kernel family, over several row blocks and ragged chunks; for both digit schemes (forced,
-      and as the library picks them).  i8_impl 0 and 1 select the same radix-128 scheme as (2, 0). """
+      and as the library picks them). """
   from dragonfly_b200 import synth_data
   rs = np.random.RandomState(3)
   X = rs.random_sample((1100, 6)); Y = synth_data.hartmann6(X)
   C = rs.random_sample((5000, 6))
   kern = _i8_kernels(B)[name]
-  fp, i8 = _post_pair(B, kern, X, Y, float(np.median(Y)), 0.01 * 0.7, chunk=2048, i8_impl=i8_impl,
-                      i8_radix=i8_radix)
+  fp, i8 = _post_pair(B, kern, X, Y, float(np.median(Y)), 0.01 * 0.7, chunk=2048, i8_radix=i8_radix)
   assert i8.query('i8_ready') == 1.0
   radix256 = i8.query('i8_radix256') == 1.0
   assert radix256 == (i8_radix == 1) or i8_radix == -1
@@ -580,9 +577,9 @@ def test_i8_sigma2_within_contract(B, name, i8_impl, i8_radix):
   err = np.abs(sd0 ** 2 - sd1 ** 2).max()
   assert err <= (5e-9 if radix256 else 1e-9), err
   assert err <= bound
-  # i8_impl 0 runs the radix-128 scheme through the same kernels on the same digits: bit-identical to any radix-128
-  # run here; the radix-256 expansion is a different, coarser one
-  _, ref = _post_pair(B, kern, X, Y, float(np.median(Y)), 0.01 * 0.7, chunk=2048, i8_impl=0)
+  # a fresh radix-128 posterior runs the same kernels on the same digits: bit-identical to any radix-128 run here; the
+  # radix-256 expansion is a different, coarser one
+  _, ref = _post_pair(B, kern, X, Y, float(np.median(Y)), 0.01 * 0.7, chunk=2048, i8_radix=0)
   _, sd_ref = ref.eval(C, mean_const=1.0)
   if radix256:
     close(sd1 ** 2, sd_ref ** 2, atol=2.0 * bound)

@@ -1,7 +1,7 @@
 """
 -m gpu, round-2 features of the scoring path:
-  * the K_* / contraction two-stream pipeline (option kstar_overlap) and the pair kernel's tile-order option return
-    bit-identical results to the default single-stream order;
+  * the pair kernel's tile-order option returns bit-identical results to the default order;
+  * int8 dfb_eval gives identical mu / sigma for host and device candidates;
   * the second-generation digit kernel (kstar_seg) against the round-1 digit kernel and against fp64;
   * the `rand` maximiser's device candidate source (anc_data.candidate_rng = 'device'): the returned point is the
     arg-max over exactly the candidates dfb_fill_candidates generates for that seed, scored by the oracle;
@@ -35,7 +35,7 @@ def gp1500(B):
   return w, gp
 
 
-def test_pipeline_and_tile_order_options_do_not_change_results(B, gp1500):
+def test_tile_order_and_kstar_options_do_not_change_results(B, gp1500):
   w, gp = gp1500
   acq = B.device.make_acq_desc('ei', best=float(w['Y'].max()))
   C = B.torch.from_numpy(np.random.RandomState(4).random_sample((90000, 6))).cuda()
@@ -45,15 +45,14 @@ def test_pipeline_and_tile_order_options_do_not_change_results(B, gp1500):
   base = gp._fused_score(acq, C)
   assert post.query('last_used_i8') == 1.0
   results = {}
-  for name, opts in [('overlap', {'kstar_overlap': 1}), ('group4', {'i8_c2_group': 4}), ('nogroup', {'i8_c2_group': 100000}),
-                     ('old_kstar', {'kstar_seg': 0}), ('old_kstar_overlap', {'kstar_seg': 0, 'kstar_overlap': 1})]:
+  for name, opts in [('group4', {'i8_c2_group': 4}), ('nogroup', {'i8_c2_group': 100000}), ('old_kstar', {'kstar_seg': 0})]:
     for k, v in opts.items():
       post.set_option(k, v)
     results[name] = gp._fused_score(acq, C)
-    post.set_option('kstar_overlap', 0); post.set_option('i8_c2_group', 0); post.set_option('kstar_seg', 1)
+    post.set_option('i8_c2_group', 0); post.set_option('kstar_seg', 1)
   for name, r in results.items():
     assert r[1] == base[1], (name, r[:2], base[:2])
-    if name.startswith('old_kstar'):     # kstar_seg = 0 also re-scores through the reference-order fp64 K_* kernel: ulps apart
+    if name == 'old_kstar':              # kstar_seg = 0 also re-scores through the reference-order fp64 K_* kernel: ulps apart
       assert abs(r[0] - base[0]) <= 1e-13 * abs(base[0]), (name, r[:2], base[:2])
     else:
       assert r[0] == base[0], (name, r[:2], base[:2])
@@ -64,20 +63,20 @@ def test_pipeline_and_tile_order_options_do_not_change_results(B, gp1500):
   assert exact[1] == base[1] and exact[0] == base[0]
 
 
-def test_overlapped_eval_matches_sequential_eval_bit_for_bit(B, gp1500):
-  """ dfb_eval forced onto the int8 pass (score_impl 1): mu and sigma of every candidate with and without the two-stream
-      pipeline, host and device candidates, ragged last chunk. """
+def test_i8_eval_of_host_and_device_candidates_matches_bit_for_bit(B, gp1500):
+  """ dfb_eval forced onto the int8 pass (score_impl 1): mu and sigma of every candidate, host and device candidates,
+      several chunks with a ragged last one; within tolerance of fp64. """
   w, gp = gp1500
   post = gp._post
   Ch = np.random.RandomState(5).random_sample((50001, 6))
   post.set_option('score_impl', 1)
   try:
     mu0, sd0 = post.eval(Ch, mean_const=w['mean_const'])
-    post.set_option('kstar_overlap', 1)
     mu1, sd1 = post.eval(Ch, mean_const=w['mean_const'])
     mu2, sd2 = post.eval(B.torch.from_numpy(Ch).cuda(), mean_const=w['mean_const'])
   finally:
-    post.set_option('kstar_overlap', 0); post.set_option('score_impl', 2)
+    post.set_option('score_impl', 2)
+  assert post.query('chunk') < len(Ch) / 2
   assert (mu0 == mu1).all() and (sd0 == sd1).all()
   assert (mu2.cpu().numpy() == mu0).all() and (sd2.cpu().numpy() == sd0).all()
   mu64, sd64 = post.eval(Ch, mean_const=w['mean_const'])
@@ -174,7 +173,7 @@ def test_cartesian_product_gp_against_the_reference(B):
   assert idx == int(np.argmax(g['mu'] + 2.0 * g['sd']))
 
 
-def test_page_locked_host_candidates_are_copied_one_batch_ahead(B, gp1500):
+def test_page_locked_host_candidates_match_device_and_pageable_bit_for_bit(B, gp1500):
   """ Host candidates in page-locked memory take the double-buffered staging path of run_chunks (copy of batch b+1 on a
       copy stream while batch b is scored): same results as device-resident and as pageable candidates, bit for bit,
       over several batches, for the fused arg-max and for eval. """
@@ -189,12 +188,9 @@ def test_page_locked_host_candidates_are_copied_one_batch_ahead(B, gp1500):
   Cd = B.torch.from_numpy(Cpage).cuda()
   acq = B.device.make_acq_desc('ucb', beta=2.0)
   want = post.score_argmax(acq, Cd, mean_const=w['mean_const'])
-  for overlap in (0, 1):
-    post.set_option('kstar_overlap', overlap)
-    got_pinned = post.score_argmax(acq, Cp, mean_const=w['mean_const'])
-    got_page = post.score_argmax(acq, Cpage, mean_const=w['mean_const'])
-    assert got_pinned[:2] == want[:2] and got_page[:2] == want[:2], (overlap, got_pinned[:2], got_page[:2], want[:2])
-  post.set_option('kstar_overlap', 0)
+  got_pinned = post.score_argmax(acq, Cp, mean_const=w['mean_const'])
+  got_page = post.score_argmax(acq, Cpage, mean_const=w['mean_const'])
+  assert got_pinned[:2] == want[:2] and got_page[:2] == want[:2], (got_pinned[:2], got_page[:2], want[:2])
   mu_d, sd_d = post.eval(Cd, mean_const=w['mean_const'])
   mu_p, sd_p = post.eval(Cp, mean_const=w['mean_const'])
   assert (mu_p == mu_d.cpu().numpy()).all() and (sd_p == sd_d.cpu().numpy()).all()

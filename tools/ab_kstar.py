@@ -1,5 +1,5 @@
-"""A/B of the K_* stage at the headline geometry: (kstar_seg, kstar_overlap) in {0,1}^2 -- step time of
-gp._fused_score over M candidates, per-class launch times, and the arg-max each variant returns."""
+"""A/B of the K_* stage at the headline geometry: kstar_seg in {0,1} -- step time of gp._fused_score over M
+candidates, per-class launch times, and the arg-max each variant returns."""
 import json, os, sys, time
 import tempfile
 import numpy as np
@@ -14,25 +14,24 @@ acq = device.make_acq_desc('ei', best=float(w['Y'].max()))
 cd = torch.from_numpy(np.random.RandomState(1000).random_sample((M, 6))).cuda()
 out = {}
 for seg in (0, 1):
-  for ov in (0, 1):
-    gp._post.set_option('kstar_seg', seg); gp._post.set_option('kstar_overlap', ov)
-    gp._fused_score(acq, cd[:200000])
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(3):
-      t0 = time.perf_counter(); r = gp._fused_score(acq, cd); torch.cuda.synchronize(); ts.append(1e3 * (time.perf_counter() - t0))
-    gp._post.profile_enable(True)
-    gp._fused_score(acq, cd)
-    prof = {n: gp._post.profile_read(c) for n, c in [('kstar', 0), ('gemm', 1), ('acq', 2)]}
-    gp._post.profile_enable(False)
-    out['seg%d_overlap%d' % (seg, ov)] = dict(ms=ts, best=float(r[0]), argmax=int(r[1]), overlapped=gp._post.query('last_overlapped'),
-                                              kstar_ms_per_launch=prof['kstar'][0] / max(prof['kstar'][1], 1),
-                                              gemm_ms_per_launch=prof['gemm'][0] / max(prof['gemm'][1], 1),
-                                              shortlist=gp._post.query('last_shortlist'))
-    print('seg%d_overlap%d' % (seg, ov), out['seg%d_overlap%d' % (seg, ov)], flush=True)
+  gp._post.set_option('kstar_seg', seg)
+  gp._fused_score(acq, cd[:200000])
+  torch.cuda.synchronize()
+  ts = []
+  for _ in range(3):
+    t0 = time.perf_counter(); r = gp._fused_score(acq, cd); torch.cuda.synchronize(); ts.append(1e3 * (time.perf_counter() - t0))
+  gp._post.profile_enable(True)
+  gp._fused_score(acq, cd)
+  prof = {n: gp._post.profile_read(c) for n, c in [('kstar', 0), ('gemm', 1), ('acq', 2)]}
+  gp._post.profile_enable(False)
+  out['seg%d' % seg] = dict(ms=ts, best=float(r[0]), argmax=int(r[1]),
+                            kstar_ms_per_launch=prof['kstar'][0] / max(prof['kstar'][1], 1),
+                            gemm_ms_per_launch=prof['gemm'][0] / max(prof['gemm'][1], 1),
+                            shortlist=gp._post.query('last_shortlist'))
+  print('seg%d' % seg, out['seg%d' % seg], flush=True)
 # accuracy of the seg path's sigma^2 / mu against fp64 on 4 chunks
 sub = cd[:26112]
-gp._post.set_option('kstar_seg', 1); gp._post.set_option('kstar_overlap', 1)
+gp._post.set_option('kstar_seg', 1)
 gp._post.set_option('score_impl', 1); mu8, sd8 = gp._post.eval(sub, mean_const=w['mean_const'], want_std=True)
 gp._post.set_option('kstar_seg', 0); mu8o, sd8o = gp._post.eval(sub, mean_const=w['mean_const'], want_std=True)
 gp._post.set_option('score_impl', 0); mu64, sd64 = gp._post.eval(sub, mean_const=w['mean_const'], want_std=True)

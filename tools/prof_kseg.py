@@ -1,4 +1,4 @@
-"""One small scoring call for ncu captures of the K_* kernels (headline geometry, 2 chunks, no stream overlap)."""
+"""One small scoring call for ncu captures of the K_* kernels (headline geometry, 3 chunks)."""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -8,7 +8,6 @@ w = synth_data.make_workload('headline_hartmann6_matern_ei', n_train=5000, n_can
 gp = gp_core.GP(w['X'], w['Y'], kernel.kernel_from_spec(w['kernel']), gp_core.ConstantMean(w['mean_const']), w['noise_var'])
 acq = device.make_acq_desc('ei', best=float(w['Y'].max()))
 cd = torch.from_numpy(np.random.RandomState(1000).random_sample((3 * 6528, 6))).cuda()
-gp._post.set_option('kstar_overlap', int(os.environ.get('OVERLAP', '0')))
 for _ in range(2):
   r = gp._fused_score(acq, cd)
 torch.cuda.synchronize()
