@@ -5,7 +5,8 @@ shared by the CPU tests (test_host_logic.py) and the GPU tests (test_gpu_i8_exac
 Everything the kernel does before its epilogue is integer arithmetic, and its epilogue is a fixed sequence of fp64
 operations, so `partial` is a deterministic function of the digit planes, the row scales and the column scale.  This
 module computes that function:
-  * digit expansions of both schemes (radix 256: digits_radix256; radix 128: the loop of slice_i8_kernel);
+  * digit expansions of both schemes (radix 256: digits_radix256; radix 128: the loop of slice_i8_kernel, and the
+    split form kstar_fast_kernel writes, which expands the same integer);
   * the pair-interleaved plane layout the producers write and the kernel reads (kb = 32);
   * the group sums G_d = sum_{s+t=d} A_s B_t^T with the triangular skip of W: every product and every partial sum
     is an integer below 15 K 2^14 < 2^53, so any fp64 GEMM (numpy's, or torch's on the device) is exact;
@@ -68,6 +69,24 @@ def digits_radix128(x):
     a = np.rint(y)
     x = y - a
     out.append(a.astype(np.int64))
+  return out
+
+
+def digits_radix128_split(x):
+  """ NumPy restatement of the radix-128 digits of kstar_fast_kernel<..., I8OUT> (kernels.cu): hi = rint(x 2^21) and
+      lo = rint((x 2^21 - hi) 2^21), each 21-bit half split into three digits by a1 = (w + 8192) >> 14,
+      a2 = (r1 + 64) >> 7, a3 = r1 - 128 a2.  The same integer rint(x 2^42) as digits_radix128, but where a half's
+      low bits sit exactly half-way its digits are rounded up, not to the nearest of the remainder: a different,
+      equally valid expansion (digits in [-64, 64]). """
+  x = np.asarray(x, dtype=np.float64)
+  hi = np.rint(x * 2.0 ** 21)
+  lo = np.rint((x * 2.0 ** 21 - hi) * 2.0 ** 21).astype(np.int64)
+  out = []
+  for w in (hi.astype(np.int64), lo):
+    a1 = (w + 8192) >> 14
+    r1 = w - (a1 << 14)
+    a2 = (r1 + 64) >> 7
+    out += [a1, a2, r1 - (a2 << 7)]
   return out
 
 

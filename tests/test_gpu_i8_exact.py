@@ -248,7 +248,7 @@ def test_production_digit_planes_and_partial_are_bit_exact(D, producer, n):
   post.set_kernel(desc)
   post.set_train(X, Y - float(np.median(Y)))
   assert post.build(0.01 * 0.7)[0] == 0
-  post.eval(Cand, mean_const=1.0)
+  mu_i8, _ = post.eval(Cand, mean_const=1.0)
   assert post.query('last_used_i8') == 1.0
   radix256 = post.query('i8_radix256') == 1.0
   if want_r256 is not None:
@@ -296,6 +296,21 @@ def test_production_digit_planes_and_partial_are_bit_exact(D, producer, n):
     recon = IX.reconstruct([a[:M_CAND, :n] for a in Kd], radix256) * colscale
     tol = 2.0 ** (-40 if radix256 else -43) * colscale + 2.0 ** -45 * np.abs(Kref)
     assert (np.abs(recon - Kref) <= tol).all(), np.max(np.abs(recon - Kref) / tol)
+    # the exact check: the fp64-row twin of the producer (kstar_seg<ROWS64>, or kstar_fast's fp64 rows) forms the same
+    # values, so the planes are exactly its digits -- in kstar_fast's own radix-128 expansion for that scheme -- and
+    # kstar_seg's mu is the twin's, bit for bit
+    post.set_option('score_impl', 0)
+    if producer != 'kstar_seg':
+      post.set_option('kstar_rows64', 0)
+    mu_twin, _ = post.eval(Cand, mean_const=1.0)
+    assert post.query('last_used_i8') == 0.0
+    Ks = _copy(D, post, 'Ks', (chunk, npad), torch.float64).cpu().numpy()[:m_rows]
+    want = IX.digits_radix256(Ks * (1.0 / colscale)) if radix256 else IX.digits_radix128_split(Ks * (1.0 / colscale))
+    for s in range(nd):
+      bad = np.argwhere(Kd[s] != want[s])
+      assert len(bad) == 0, ('digit', s, 'differs from the twin in', len(bad), 'entries; first', tuple(bad[0]))
+    if producer == 'kstar_seg':
+      assert _bits_equal(mu_i8, mu_twin)
   del Kd
 
   # D: the production `partial`, from the copied planes, row scales and column scale
