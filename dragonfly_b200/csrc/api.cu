@@ -3,6 +3,7 @@
 #include <stdarg.h>
 #include <new>
 #include <stdlib.h>
+#include <float.h>
 #include "kernels.cuh"
 #include "gemm_tma.h"
 
@@ -24,6 +25,8 @@ static int64_t default_chunk(int64_t npad) {
   if (c > 65536) c = 65536;
   return c;
 }
+
+constexpr int PRUNE_MAX_DC = 8;       // candidate columns the survivor list of the bound pass holds
 
 struct Carver {
   char* base;
@@ -78,6 +81,11 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   double* stage = c.take<double>((size_t)chunk * DFB_MAX_SLOTS);
   double* blk_score = c.take<double>((size_t)chunk / 128 + 16);
   int64_t* blk_index = c.take<int64_t>((size_t)chunk / 128 + 16);
+  const int64_t surv_cap = 4 * chunk;
+  int64_t* surv_idx = c.take<int64_t>((size_t)surv_cap);
+  double* surv_X = c.take<double>((size_t)surv_cap * PRUNE_MAX_DC);
+  int* surv_count = c.take<int>(4);
+  uint32_t* keep_words = c.take<uint32_t>((size_t)chunk / 32 + 1);
   double* best_score = c.take<double>(1);
   int64_t* best_index = c.take<int64_t>(1);
   double* red = c.take<double>(8);
@@ -95,6 +103,8 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
     h->tr.xs = tr_xs; h->tr.nrm = tr_nrm; h->te.xs = te_xs; h->te.nrm = te_nrm;
     h->Ks = Ks; h->Wi8 = Wi8; h->Ki8 = Ki8; h->rowscale = rowscale; h->rowinv = rowinv; h->list_idx = list_idx; h->list_X = list_X; h->list_count = list_count; h->list_s8 = list_s8; h->list_err = list_err; h->blk_lb = blk_lb; h->best_lb = best_lb; h->partial = partial; h->mu = mu; h->sd = sd; h->score = score; h->kssv = kssv; h->stage = stage;
     h->blk_score = blk_score; h->blk_index = blk_index; h->best_score = best_score;
+    h->surv_cap = surv_cap; h->surv_idx = surv_idx; h->surv_X = surv_X; h->surv_count = surv_count;
+    h->keep_words = keep_words;
     h->best_index = best_index; h->red = red; h->info = info;
     h->d_desc_tr = d0; h->d_desc_te = d1; h->d_desc_tmp = d2;
     h->n_max = n_max; h->npad_max = npad; h->chunk = chunk;
@@ -498,9 +508,12 @@ struct ChunkMode {
   bool collect;                // gather the shortlist for the exact re-score
   I8ErrModel em;               // int8 error model (collect): bound on |d sigma^2|, score sensitivity
   double pad;                  // extra slack of the shortlist test
-  const int64_t* idx_map;      // global index of each row (re-score pass), NULL = c0 + i
+  const int64_t* idx_map;      // global index of each row (re-score passes), NULL = idx_base + row
+  int64_t idx_base;            // global index of row 0 when idx_map is NULL
   bool allow_small;            // dfb_eval of <= SMALL_EVAL_M points: row-streaming kernel instead of the tile GEMM
   bool keep_scores;            // leave the scores of a single-chunk pass in h->score (self-check of the shortlist)
+  bool keep_best;              // continue the running arg-max and best_lb of an earlier pass instead of resetting them
+  bool bound_pass;             // mu only + the upper-bound screen into the survivor list (dfb_score_argmax)
 };
 static ChunkMode chunk_mode(bool want_std, bool do_argmax, bool use_i8, const int64_t* idx_map = nullptr) {
   ChunkMode md;
@@ -513,6 +526,8 @@ constexpr int64_t SMALL_EVAL_M = 32;      // up to four 8-wide passes over W's r
 // Per chunk two stages, back to back on the handle's stream:
 //   K: (host candidates: staging copy) K_* rows / digit planes + mu + k(x*,x*)      fp64 pipe
 //   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
+// The bound pass (md.bound_pass) replaces both by mu + k(x*,x*) alone and the screen that appends the candidates whose
+// acquisition bound reaches best_lb to the survivor list.
 static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
                       int32_t space, double mean_const, ChunkOut out, const ChunkMode& md) {
   const bool want_std = md.want_std, do_argmax = md.do_argmax;
@@ -528,7 +543,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   DFB_TRY(ensure_test_scaled(h));
   const int64_t npad = h->npad, Mc = h->chunk;
   const int nb = (int)(npad / TILE);
-  if (do_argmax) DFB_TRY(launch_reset_best(h));
+  if (do_argmax && !md.keep_best) DFB_TRY(launch_reset_best(h));
   const bool i8 = want_std && md.use_i8;
   const bool seg_ok = i8 && h->i8_fuse && h->kstar_fast && h->kstar_seg && h->i8_radix256;
   // host candidates are staged in batches of as many whole chunks as the staging buffer holds
@@ -567,6 +582,13 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     DFB_CUDA_OK(cudaEventRecord(h->cp_done[bi & 1], h->cp_stream));
     return 0;
   };
+  auto release_half = [&](int64_t c0) -> int {             // last chunk of its batch: the half may be overwritten
+    if (!dbuf) return 0;
+    const int64_t bi = c0 / half_rows;
+    const int64_t b_hi = (m - bi * half_rows < half_rows) ? m : (bi + 1) * half_rows;
+    if (c0 + Mc >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
+    return 0;
+  };
   const int64_t n_chunks = (m + Mc - 1) / Mc;
   const int* abort_count = md.collect ? h->list_count : nullptr;
   const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
@@ -601,6 +623,20 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
                                                          : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
 
+    if (md.bound_pass) {
+      // mu (bit-identical to the digit kernel's) and k(x*, x*); no K_* rows, no contraction.  Void once the seed's
+      // shortlist has overflowed, like every other launch of the int8 pass.
+      DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
+      int emitted = 0;
+      DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
+                               h->mu, h->kssv, nullptr, 0, 0, 0.0, h->cprep, h->mu_part, Mc, &emitted, h->list_count));
+      if (!emitted) { set_error("bound pass: the mu-only K_* kernel does not serve this kernel"); return -1; }
+      DFB_TRY(launch_prune(h, acq, h->mu, h->kssv, mc, md.pad, md.idx_base + c0, xc_dev, dc));
+      DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
+      DFB_TRY(release_half(c0));
+      continue;
+    }
+
     // K stage
     DFB_TRY(prof_begin(h, DFB_PROF_KSTAR));
     int fused_digits = 0;
@@ -608,6 +644,9 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
                                mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad, 1.0 / i8_colscale(desc), h->cprep,
                                h->mu_part, Mc, &fused_digits, abort_count));
+    else if (!want_std && h->kstar_rows64)    // mu alone: the row kernel's mu without writing its rows
+      DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
+                               mu_dev, nullptr, nullptr, 0, 0, 0.0, h->cprep, h->mu_part, Mc, &fused_digits, nullptr));
     if (!fused_digits && i8 && h->i8_fuse)
       DFB_TRY(launch_kstar_i8(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, xc_dev, mc, dc, m_rows, h->n, npad,
                               mean_const, mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad,
@@ -652,11 +691,12 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     }
     if (want_std || do_argmax || sc_dev != nullptr) {
       DFB_TRY(prof_begin(h, DFB_PROF_ACQ));
-      DFB_TRY(launch_acq(h, acq, mu_dev, h->partial, small ? SMALL_EVAL_M : Mc, small ? small_warps : nb, h->kssv, mc, c0,
-                         want_std ? 1 : 0, want_std ? sd_dev : nullptr, sc_dev, do_argmax, md.idx_map,
+      const int64_t* idx_map = md.idx_map ? md.idx_map + c0 : nullptr;
+      DFB_TRY(launch_acq(h, acq, mu_dev, h->partial, small ? SMALL_EVAL_M : Mc, small ? small_warps : nb, h->kssv, mc,
+                         md.idx_base + c0, want_std ? 1 : 0, want_std ? sd_dev : nullptr, sc_dev, do_argmax, idx_map,
                          md.collect ? &md.em : nullptr));
       if (md.collect)
-        DFB_TRY(launch_collect_shortlist(h, sc_dev, sd_dev, mc, c0, md.em, md.pad, xc_dev, dc));
+        DFB_TRY(launch_collect_shortlist(h, sc_dev, sd_dev, mc, md.idx_base + c0, idx_map, md.em, md.pad, xc_dev, dc));
       DFB_TRY(prof_end(h, DFB_PROF_ACQ, (double)mc));
     }
     if (space == DFB_HOST) {
@@ -667,11 +707,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       if (out.score)
         DFB_CUDA_OK(cudaMemcpyAsync(out.score + c0, sc_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
     }
-    if (dbuf) {                                            // last chunk of its batch: the half may be overwritten
-      const int64_t bi = c0 / half_rows;
-      const int64_t b_hi = (m - bi * half_rows < half_rows) ? m : (bi + 1) * half_rows;
-      if (c0 + Mc >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
-    }
+    DFB_TRY(release_half(c0));
   }
   return 0;
 }
@@ -1013,6 +1049,68 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
   return 0;
 }
 
+// ---- bound pass of dfb_score_argmax ---------------------------------------------------------------------------------
+// Most candidates of a large random batch cannot reach the arg-max, and proving so needs mu alone:
+//   (1) ub = acq(mu, sqrt(k**)) >= the fp64 score of the exact pass.  EI (d/d sigma = phi(z) > 0), UCB with beta >= 0
+//       and PI for mu < the incumbent (z < 0) are non-decreasing in sigma, and the device's fp64 variance
+//       fl(k** - sum of partials) with every partial >= 0 is at most k** in floating point as well.  The ulp-level
+//       non-monotonicity of the ndtr / erfc formulas is dwarfed by the shortlist's pad (1e-9 of the score scale).
+//   (2) best_lb <= the final fp64 maximum (argmax_merge_kernel: a maximum of certain lower bounds).
+// So a candidate with ub < best_lb - pad has an fp64 score below the maximum: every candidate whose fp64 score equals
+// the maximum, ties included, survives, the shortlist of the passes that follow contains all of them, and the fp64
+// arg-max over it -- index and score -- is the one the full pass returns, bit for bit.
+// (3) No dropped candidate can be a NaN winner (a negative fp64 variance gives a NaN score, and np.argmax takes the
+//     first NaN): see bound_pass_applies.
+// Order: (a) chunk 0 scored as today (collect mode) seeds best, best_lb and the shortlist; (b) the bound pass over
+// chunks 1.. fills the survivor list; (c) one read-back of the survivor count; (d) the survivors are scored like any
+// other chunk (collect mode, indices mapped back), continuing the arg-max of (a); the caller then re-scores the
+// shortlist in fp64 and runs the self-check unchanged.  A survivor list that overflows (4 chunks) voids the screen:
+// chunks 1.. are then scored as today, still continuing the seed's state.
+static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, int64_t m,
+                               int32_t dc, double b2) {
+  if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC) return false;
+  if (!(h->i8_fuse && h->i8_radix256 && kstar_seg_applies(h, desc))) return false;    // run_chunks' digit kernel
+  if (!(acq.kind == DFB_ACQ_EI || acq.kind == DFB_ACQ_PI || (acq.kind == DFB_ACQ_UCB && acq.beta >= 0.0))) return false;
+  // Variance floor.  K: the noiseless training kernel matrix, s: the diagonal actually added (noise + jitter, for every
+  // point, hallucinated ones included), k = K(X, x*).  The joint covariance [[K, k], [k^T, k**]] is PSD, so
+  // k^T K^+ k <= k**, and in the eigenbasis of K (c_i = u_i^T k, eigenvalues l_i <= l_max <= tr K = n k(x, x)):
+  //   k^T (K + s I)^-1 k = sum_i (c_i^2 / l_i) l_i / (l_i + s) <= k** l_max / (l_max + s)
+  //   sigma^2 = k** - k^T (K + s I)^-1 k >= k** s / (l_max + s) >= k** s / (tr K + s).
+  // Screening is allowed only when this floor exceeds both the int8 error bound b2 and n eps k** (a worst-case bound
+  // on the fp64 contraction's own rounding): then no candidate's fp64 variance is negative.  At the headline
+  // (N = 5000) the floor is ~3e-7 against b2 ~ 3e-9.
+  const double s = h->noise_plus_jitter, kss = desc.kss;
+  const double floor = kss * s / ((double)h->n * kss + s);
+  return floor > b2 && floor > (double)h->n * DBL_EPSILON * kss;
+}
+
+static int run_chunks_pruned(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
+                             int32_t space, double mean_const, const ChunkMode& md) {
+  const int64_t Mc = h->chunk;
+  const ChunkOut none = {nullptr, nullptr, nullptr};
+  const double* rest = Xc + Mc * dc;
+  DFB_TRY(run_chunks(h, acq, Xc, Mc, dc, space, mean_const, none, md));                 // (a)
+  ChunkMode bp = md;
+  bp.bound_pass = true; bp.keep_best = true; bp.idx_base = Mc;
+  DFB_CUDA_OK(cudaMemsetAsync(h->surv_count, 0, sizeof(int), h->stream));
+  DFB_TRY(run_chunks(h, acq, rest, m - Mc, dc, space, mean_const, none, bp));            // (b)
+  int surv = 0;
+  DFB_CUDA_OK(cudaMemcpyAsync(&surv, h->surv_count, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));                                        // (c)
+  h->last_survivors = surv;
+  ChunkMode cont = md;
+  cont.keep_best = true;
+  if (surv > h->surv_cap) {                         // overflow: every candidate of chunks 1.. is contracted
+    h->last_pruned = 0;
+    cont.idx_base = Mc;
+    return run_chunks(h, acq, rest, m - Mc, dc, space, mean_const, none, cont);
+  }
+  h->last_pruned = m - Mc - surv;
+  if (surv == 0) return 0;
+  cont.idx_map = h->surv_idx;
+  return run_chunks(h, acq, h->surv_X, surv, dc, DFB_DEVICE, mean_const, none, cont);   // (d)
+}
+
 int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m, int32_t dc,
                      int32_t space, double mean_const, double* scores, double* best_score_host,
                      int64_t* best_index_host) {
@@ -1033,6 +1131,8 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
   h->last_shortlist = 0;
   h->last_selfcheck_violations = 0;
   h->last_selfcheck_ratio = 0.0;
+  h->last_survivors = 0;
+  h->last_pruned = 0;
   double bs = 0.0;
   int64_t bi = -1;
   bool need_exact_pass = !fast;
@@ -1050,7 +1150,10 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
     md.em.sens = (acq->kind == DFB_ACQ_UCB) ? fabs(acq->beta) : (acq->kind == DFB_ACQ_PI ? 0.25 : 0.4);
     md.pad = 1e-9 * scale;
     DFB_CUDA_OK(cudaMemsetAsync(h->list_count, 0, sizeof(int) * 4, h->stream));
-    DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, md));
+    if (scores == nullptr && bound_pass_applies(h, *acq, desc, m, dc, md.em.b2))
+      DFB_TRY(run_chunks_pruned(h, *acq, Xc, m, dc, space, mean_const, md));
+    else
+      DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, md));
     int count = 0;
     DFB_CUDA_OK(cudaMemcpyAsync(&count, h->list_count, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
@@ -1322,6 +1425,8 @@ int dfb_query(dfb_handle* h, const char* name, double* out) {
   if (strcmp(name, "last_shortlist") == 0) { *out = (double)h->last_shortlist; return 0; }
   if (strcmp(name, "last_selfcheck_violations") == 0) { *out = (double)h->last_selfcheck_violations; return 0; }
   if (strcmp(name, "last_selfcheck_ratio") == 0) { *out = h->last_selfcheck_ratio; return 0; }
+  if (strcmp(name, "last_survivors") == 0) { *out = (double)h->last_survivors; return 0; }
+  if (strcmp(name, "last_pruned_candidates") == 0) { *out = (double)h->last_pruned; return 0; }
   if (strcmp(name, "chunk") == 0) { *out = (double)h->chunk; return 0; }
   if (strcmp(name, "npad") == 0) { *out = (double)h->npad; return 0; }
   if (strcmp(name, "last_c2_group") == 0) { *out = (double)h->last_c2_group; return 0; }
@@ -1348,6 +1453,7 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "i8_fuse") == 0) { h->i8_fuse = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_seg") == 0) { h->kstar_seg = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_rows64") == 0) { h->kstar_rows64 = value ? 1 : 0; return 0; }
+  if (strcmp(name, "prune") == 0) { h->prune = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_unguarded") == 0) { h->i8_unguarded = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_radix") == 0) {
     if (value < -1 || value > 1) { set_error("i8_radix must be -1 (auto), 0 (radix 128) or 1 (radix 256)"); return -1; }

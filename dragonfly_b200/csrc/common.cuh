@@ -42,7 +42,7 @@ struct ScaledSet {        // scaled training coordinates for one kernel descript
 }  // namespace dfb
 
 namespace dfb {
-constexpr int PROF_CLASSES = 4;
+constexpr int PROF_CLASSES = 5;
 constexpr int PROF_RING = 1024;
 struct ProfClass {
   cudaEvent_t start[PROF_RING];
@@ -135,6 +135,14 @@ struct dfb_handle {
   double* list_err = nullptr;     // its error allowance E_i (< 0: none -- suspect / NaN)
   double* blk_lb = nullptr;       // per-block max of (score - E): certain lower bounds of the fp64 maximum
   double* best_lb = nullptr;      // running maximum of those
+  // survivor list of the bound pass of dfb_score_argmax (api.cu)
+  int prune = 1;                  // option "prune": 0 = contract every candidate
+  int64_t surv_cap = 0;           // 4 chunks
+  int64_t* surv_idx = nullptr;    // surv_cap global indices
+  double* surv_X = nullptr;       // surv_cap x PRUNE_MAX_DC candidate rows
+  int* surv_count = nullptr;      // [0] survivors wanted (> surv_cap = overflow)
+  uint32_t* keep_words = nullptr; // chunk / 32 ballot words of one chunk
+  int64_t last_survivors = 0, last_pruned = 0;
   int64_t last_selfcheck_violations = 0;
   double last_selfcheck_ratio = 0.0;   // max |s_int8 - s_fp64| / E_i over the last shortlist
   int64_t last_shortlist = 0;     // diagnostics: size of the last shortlist, -1 = overflow -> exact pass

@@ -17,7 +17,9 @@ int launch_kstar_i8(dfb_handle* h, const dfb_kernel_desc* d_desc, const dfb_kern
                     const double* Xc, int64_t m, int dc, int64_t m_rows, int64_t n_valid, int64_t n_write,
                     double mean_const, double* mu, double* kss_out, void* planes, int64_t plane_bytes,
                     int64_t row_bytes, double inv_colscale, int* emitted_i8, const int* abort_count = nullptr);
-// second-generation digit path (kernels.cu: kstar_seg_kernel)
+// second-generation K_* path (kernels.cu: kstar_seg_kernel): digit planes, or mu alone when planes is NULL (mu and
+// mu_part required)
+bool kstar_seg_applies(const dfb_handle* h, const dfb_kernel_desc& desc);
 int launch_kstar_seg(dfb_handle* h, const dfb_kernel_desc* d_desc, const dfb_kernel_desc& desc, const double* xsT,
                      const double* nrm, int64_t npad_tr, const double* alpha, int64_t n_valid, const double* Xc, int64_t m,
                      int dc, int64_t m_rows, int64_t n_write, double mean_const, double* mu, double* kss_out, void* planes,
@@ -48,7 +50,12 @@ int launch_acq(dfb_handle* h, const dfb_acq_desc& acq, const double* mu, const d
                int want_std, double* sd_out, double* score_out, bool do_argmax,
                const int64_t* idx_map = nullptr, const I8ErrModel* em = nullptr);
 int launch_collect_shortlist(dfb_handle* h, const double* score, const double* sd, int64_t mc,
-                             int64_t idx_base, const I8ErrModel& em, double pad, const double* Xc, int dc);
+                             int64_t idx_base, const int64_t* idx_map, const I8ErrModel& em, double pad, const double* Xc,
+                             int dc);
+// bound pass of dfb_score_argmax: keeps the candidates of a chunk whose acquisition at sigma = sqrt(k**) reaches
+// *best_lb - pad and appends them (x rows, global index idx_base + row) to the survivor list in row order
+int launch_prune(dfb_handle* h, const dfb_acq_desc& acq, const double* mu, const double* kss, int64_t mc, double pad,
+                 int64_t idx_base, const double* Xc, int dc);
 int launch_selfcheck(dfb_handle* h, const double* s64, int count);
 int launch_vec_max(dfb_handle* h, const double* v, int64_t n, double* out);
 int launch_reset_best(dfb_handle* h);

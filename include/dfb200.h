@@ -328,23 +328,34 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *                 digits, 32 with radix-128); 0 (default) = 8.  The kernel runs in clusters of two CTAs on adjacent
  *                 tiles that share one load of the W digits, so an odd group is rounded up by one tile; query
  *                 "last_c2_group" gives the group in effect.
+ *  "prune"      : 1 (default) = dfb_score_argmax's int8 path contracts only the candidates whose acquisition can reach
+ *                 the arg-max.  After chunk 0 is scored, every further candidate gets mu alone and is dropped when
+ *                 acq(mu, sqrt(k(x*, x*))) -- an upper bound of its score, sigma^2 <= k(x*, x*) -- lies below a certain
+ *                 lower bound of the fp64 maximum; the survivors are scored as usual.  Index and score are those of the
+ *                 full pass, bit for bit.  Applies to EI, PI and UCB with beta >= 0, plain SE / Matern kernels on <= 8
+ *                 dims, radix-256 digits, no test kernel, m > chunk, no score vector, and when the posterior's variance
+ *                 floor k** s / (n k** + s) (s = noise + jitter) exceeds the int8 error bound.  0 = contract every
+ *                 candidate.
  *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_radix256", "score_impl",
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen
  * was voided and the call redone in fp64), "last_selfcheck_ratio" (max |s_int8 - s_fp64| / allowance over the last
  * shortlist; the model's margin is its inverse), "chunk", "npad", "last_c2_group"; "i8_impl" is always 2 (bench.py
- * reports it). */
+ * reports it); "last_survivors" (candidates the bound pass of option "prune" kept; > 4 chunks = overflow, the screen
+ * was voided; 0 when it did not run), "last_pruned_candidates" (candidates contracted in no pass). */
 int dfb_query(dfb_handle* h, const char* name, double* out);
 
 /* Per-kernel-class device timing with CUDA events on the handle's stream (bench.py's roofline):
  * class 0 = K_* build (+mu), 1 = the DMMA contraction |L^-1 k_*|^2, 2 = acquisition + arg-max,
- * 3 = posterior build (whole dfb_build_posterior).  dfb_profile_read synchronises, returns the
- * accumulated milliseconds, launches and work units (candidates for 0-2, builds for 3) and resets. */
+ * 3 = posterior build (whole dfb_build_posterior), 4 = the bound pass of dfb_score_argmax (mu + upper-bound screen,
+ * option "prune").  dfb_profile_read synchronises, returns the accumulated milliseconds, launches and work units
+ * (candidates for 0-2 and 4, builds for 3) and resets.  Class 1 counts only the candidates actually contracted. */
 #define DFB_PROF_KSTAR 0
 #define DFB_PROF_GEMM  1
 #define DFB_PROF_ACQ   2
 #define DFB_PROF_BUILD 3
+#define DFB_PROF_PRUNE 4
 int dfb_profile_enable(dfb_handle* h, int on);
 int dfb_profile_read(dfb_handle* h, int cls, double* ms_total, int64_t* launches, double* units);
 

@@ -1,4 +1,7 @@
-"""Wall-clock / device-time breakdown of one bench.py step (build + fused score of 10^6 candidates)."""
+"""Wall-clock / device-time breakdown of one bench.py step (build + fused score of 10^6 candidates).
+
+The device line splits the score into the contracted chunks (kstar, gemm, acq: the seed chunk and the survivors of
+the bound pass) and the bound pass itself (mu + upper-bound screen of every other candidate)."""
 import os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,10 +25,14 @@ for prof in (False, False, False, True):
   sync(); t2 = time.perf_counter()
   line = 'build %.2f ms  score %.2f ms  total %.2f ms' % (1e3 * (t1 - t0), 1e3 * (t2 - t1), 1e3 * (t2 - t0))
   if prof:
-    r = [gp._post.profile_read(c) for c in range(3)]
-    line += ' | device: kstar %.2f (%d) gemm %.2f (%d) acq %.2f (%d) sum %.2f' % (
-        r[0][0], r[0][1], r[1][0], r[1][1], r[2][0], r[2][1], r[0][0] + r[1][0] + r[2][0])
-    line += ' | shortlist %d' % int(gp._post.query('last_shortlist'))
+    r = [gp._post.profile_read(c) for c in (0, 1, 2, 4)]
+    # kstar / gemm / acq: the chunks that were contracted (the seed chunk and the survivors of the bound pass);
+    # bound: the mu-only pass + upper-bound screen over every other candidate
+    line += ' | device: kstar %.2f (%d) gemm %.2f (%d, %d cand) acq %.2f (%d) bound %.2f (%d) sum %.2f' % (
+        r[0][0], r[0][1], r[1][0], r[1][1], r[1][2], r[2][0], r[2][1], r[3][0], r[3][1], sum(x[0] for x in r))
+    line += ' | shortlist %d survivors %d pruned %d' % (int(gp._post.query('last_shortlist')),
+                                                        int(gp._post.query('last_survivors')),
+                                                        int(gp._post.query('last_pruned_candidates')))
   print(line)
   del gp
 
