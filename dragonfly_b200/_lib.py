@@ -34,7 +34,7 @@ class FactorDesc(C.Structure):
 
 class KernelDesc(C.Structure):
   _fields_ = [('n_terms', C.c_int32), ('n_factors', C.c_int32), ('n_slots', C.c_int32),
-              ('train_dim', C.c_int32), ('cand_dim', C.c_int32), ('reserved', C.c_int32),
+              ('train_dim', C.c_int32), ('cand_dim', C.c_int32), ('esp_order', C.c_int32),
               ('post_scale', C.c_double), ('kss', C.c_double),
               ('term_first_factor', C.c_int32 * (DFB_MAX_TERMS + 1)),
               ('term_pre_scale', C.c_double * DFB_MAX_TERMS),

@@ -162,6 +162,19 @@ static int check_desc(const dfb_kernel_desc* d) {
       return -1;
     }
   }
+  if (d->esp_order < 0 || d->esp_order > d->n_terms) {
+    set_error("kernel descriptor: ESP order %d outside 0 .. n_terms = %d", d->esp_order, d->n_terms);
+    return -1;
+  }
+  if (d->esp_order > 0) {
+    for (int t = 0; t < d->n_terms; t++) {
+      const int f = d->term_first_factor[t];
+      if (d->term_first_factor[t + 1] != f + 1 || d->factors[f].n_dims != 1 || d->term_pre_scale[t] != 1.0) {
+        set_error("kernel descriptor: ESP term %d is not one 1-slot factor with pre_scale 1", t);
+        return -1;
+      }
+    }
+  }
   return 0;
 }
 
@@ -961,10 +974,10 @@ int dfb_restore_posterior(dfb_handle* h) {
 int dfb_lml_gradients(dfb_handle* h, double* out_host, int32_t n_out) {
   DFB_TRY(need(h, true, true, true, true, true));
   const dfb_kernel_desc& desc = h->desc_tr;
-  if (desc.n_terms != 1 || desc.n_factors != 1) {
-    // the reference's composite kernels inherit Kernel._child_gradient, which raises (kernel.py:123-125)
-    set_error("LML gradients are defined for plain SE / Matern kernels only (kernel has %d terms, %d factors)",
-              desc.n_terms, desc.n_factors);
+  if (desc.n_terms != 1 || desc.n_factors != 1 || desc.esp_order != 0) {
+    // the reference's composite and ESP kernels inherit Kernel._child_gradient, which raises (kernel.py:123-125)
+    set_error("LML gradients are defined for plain SE / Matern kernels only (kernel has %d terms, %d factors, "
+              "ESP order %d)", desc.n_terms, desc.n_factors, desc.esp_order);
     return -3;
   }
   const int D = desc.factors[0].n_dims;

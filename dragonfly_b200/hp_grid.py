@@ -17,19 +17,30 @@ CPU tests of the sharding logic).
 import numpy as np
 
 from . import _lib
-from .kernel import SEKernel, MaternKernel, AdditiveKernel, CoordinateProductKernel, build_descriptor
+from .kernel import SEKernel, MaternKernel, AdditiveKernel, CoordinateProductKernel, ESPKernelSE, ESPKernelMatern, \
+    build_descriptor
 from .gp_core import stable_cholesky_on_device
 
 
 class EuclideanHPLayout(object):
-  """ How a continuous hp vector maps to (mean const, noise var, kernel) for an SE / Matern GP. """
+  """ How a continuous hp vector maps to (mean const, noise var, kernel) for an SE / Matern / ESP GP.
+      ESP (kernel_type 'esp', euclidean_gp.py:283-299, 249-251, 816-892): log scale and d log bandwidths whatever
+      use_same_bandwidth says; discrete hps [nu]? (esp_kernel_type 'matern' with esp_matern_nu < 0) then [order]?
+      (esp_order == -1), handed to unpack as one tuple per sample. """
 
   def __init__(self, dim, kernel_type='matern', nu=2.5, use_same_bandwidth=False,
                mean_func_type='median', mean_func_const=0.0, noise_var_type='tune',
                noise_var_label=0.05, noise_var_value=0.1, use_additive_gp=False, add_max_group_size=6,
-               num_groups_per_group_size=-1):
-    if kernel_type not in ('se', 'matern'):
+               num_groups_per_group_size=-1, esp_kernel_type='se', esp_order=-1, esp_matern_nu=-1.0):
+    if kernel_type not in ('se', 'matern', 'esp'):
       raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kernel_type))
+    if kernel_type == 'esp':
+      if esp_kernel_type not in ('se', 'matern'):
+        raise NotImplementedError('esp_kernel_type %s is not implemented (euclidean_gp.py:285-286).'
+                                  % (esp_kernel_type))
+      if use_additive_gp:
+        raise NotImplementedError('use_additive_gp with an ESP kernel is outside the device path.')
+    self.esp_kernel_type, self.esp_order, self.esp_matern_nu = esp_kernel_type, esp_order, esp_matern_nu
     self.dim, self.kernel_type, self.nu = dim, kernel_type, nu
     self.use_same_bandwidth = use_same_bandwidth
     self.mean_func_type, self.mean_func_const = mean_func_type, mean_func_const
@@ -42,7 +53,7 @@ class EuclideanHPLayout(object):
     self.num_groups_per_group_size = num_groups_per_group_size
 
   def num_hps(self):
-    n = 1 + (1 if self.use_same_bandwidth else self.dim)
+    n = 1 + (1 if self.use_same_bandwidth and self.kernel_type != 'esp' else self.dim)
     n += 1 if self.mean_func_type == 'tune' else 0
     n += 1 if self.noise_var_type == 'tune' else 0
     return n
@@ -67,7 +78,12 @@ class EuclideanHPLayout(object):
     out.append([np.log(0.1 * Y_var), np.log(10 * Y_var)])
     X_std_norm = np.linalg.norm(X, 'fro') + 1e-4
     single = [np.log(0.01 * X_std_norm), np.log(10 * X_std_norm)]
-    out += [single] * (1 if self.use_same_bandwidth else self.dim)
+    out += [single] * (1 if self.use_same_bandwidth and self.kernel_type != 'esp' else self.dim)
+    if self.kernel_type == 'esp':
+      dscr = [[0.5, 1.5, 2.5]] if (self.esp_kernel_type == 'matern' and self.esp_matern_nu < 0) else []
+      if self.esp_order == -1:
+        dscr.append(list(range(1, max(self.dim, self.esp_order) + 1)))
+      return np.array(out), dscr
     if tune_nu is None:
       tune_nu = self.kernel_type == 'matern' and (self.nu is None or self.nu < 0)
     dscr = [[0.5, 1.5, 2.5]] if (self.kernel_type == 'matern' and tune_nu) else []
@@ -103,6 +119,8 @@ class EuclideanHPLayout(object):
     Y = np.asarray(Y, dtype=np.float64)
     mean_const, noise_var = self._mean_and_noise(hp, Y)
     scale = np.exp(hp.pop(0))
+    if self.kernel_type == 'esp':
+      return float(mean_const), float(noise_var), self._esp_kernel(scale, hp, nu)
     if self.use_same_bandwidth:
       bws = [np.exp(hp.pop(0))] * self.dim
     else:
@@ -121,6 +139,21 @@ class EuclideanHPLayout(object):
     else:
       kern = MaternKernel(self.dim, nu, scale, bws)
     return float(mean_const), float(noise_var), kern
+
+  def _esp_kernel(self, scale, hp, dscr):
+    """ get_euclidean_integral_gp_kernel_with_scale for kernel_type 'esp' (euclidean_gp.py:816-824, 841-847,
+        878-892): the order is the last discrete hp unless fixed, nu (the same for every dimension) the first. """
+    bws = [np.exp(h) for h in hp[:self.dim]]
+    assert len(hp) == self.dim
+    dscr = [] if dscr is None else list(dscr)
+    if self.esp_order > 0:
+      order = self.esp_order
+    else:
+      order, dscr = dscr[-1], dscr[:-1]
+    if self.esp_kernel_type == 'se':
+      return ESPKernelSE(self.dim, scale, int(order), bws)
+    nu = self.esp_matern_nu if self.esp_matern_nu > 0 else dscr[0]
+    return ESPKernelMatern(self.dim, [nu] * self.dim, scale, int(order), bws)
 
 
 class EuclideanMFHPLayout(EuclideanHPLayout):
@@ -278,8 +311,8 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
         'rand_exp_sampling'  random_sample_cts_dscr + exp(lml - max) weights (oper_utils.py:362-371,
                              gp_core.py:439-445): one call for all samples.
       The global NumPy RNG is consumed exactly like the reference does, so a seeded run picks the same
-      hyper-parameters.  `cts_hp_bounds` / `dscr_hp_vals` are the fitter's (euclidean_gp.py:222-320); for this layout
-      the only discrete hp is the Matern nu.  Returns what the reference returns:
+      hyper-parameters.  `cts_hp_bounds` / `dscr_hp_vals` are the fitter's (euclidean_gp.py:222-320); the discrete
+      hps are the Matern nu (and for additive models the group size), or for an ESP layout [nu]? [order]?.  Returns what the reference returns:
         ('fitted_gp', gp, (cts_hps, dscr_hps))   or   ('sample_hps_with_probs', cts, dscr, [None] * n, probs). """
   from itertools import product as itertools_product
   from .gp_core import GP, ConstantMean
@@ -289,10 +322,17 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   bounds = np.asarray(cts_hp_bounds, dtype=np.float64)
   dscr_hp_vals = [list(v) for v in dscr_hp_vals]
   additive = bool(getattr(layout, 'use_additive_gp', False))
-  if len(dscr_hp_vals) > (2 if additive else 1):
+  esp = getattr(layout, 'kernel_type', None) == 'esp'
+  if len(dscr_hp_vals) > (2 if additive or esp else 1):
     raise NotImplementedError('Discrete hyper-parameters on the device path: the Matern nu and, for additive '
                               'models, the group size.')
   has_nu = len(dscr_hp_vals) == (2 if additive else 1)       # [nu]? then [group size]? (euclidean_gp.py:226-248)
+
+  def kernel_dscr(dscr):
+    """ What unpack / lml_for_hyperparams take per sample: nu (SE / Matern), or the tuple [nu]? [order]? (ESP). """
+    if esp:
+      return tuple(dscr) if len(dscr) else None
+    return dscr[0] if has_nu else None
   dim = layout.dim
   if max_evals is None:
     max_evals = default_max_evals(method, len(bounds) + len(dscr_hp_vals))
@@ -307,7 +347,7 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   def build(cts, dscr, groupings=None):
     if build_gp is not None:                         # e.g. the reference fitter's own build_gp (fit_gp_on_fitter)
       return build_gp(cts, dscr, groupings)
-    mean_const, noise_var, kern = layout.unpack(cts, Y, dscr[0] if has_nu else None, groupings)
+    mean_const, noise_var, kern = layout.unpack(cts, Y, kernel_dscr(dscr), groupings)
     make = GP if gp_factory is None else gp_factory
     return make(list(X), list(Y), kern, ConstantMean(mean_const), noise_var)
 
@@ -335,7 +375,7 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
       return 'sample_hps_with_probs', cts, dscr, other, probs / probs.sum()
     cts = map_to_bounds(np.random.random((n_evals, len(bounds))), bounds)
     dscr = [[np.random.choice(categ) for categ in dscr_hp_vals] for _ in range(n_evals)]
-    vals = lmls_of(cts, [d[0] for d in dscr] if dscr_hp_vals else None)
+    vals = lmls_of(cts, [kernel_dscr(d) for d in dscr] if dscr_hp_vals else None)
     return 'sample_hps_with_probs', cts, dscr, [None] * n_evals, rand_exp_sampling_probs(vals)
   if method == 'direct' and _reference_fortran_direct_available():
     raise NotImplementedError('Fortran DIRECT is a sequential host optimiser; use pdoo / rand / rand_exp_sampling.')
@@ -357,7 +397,7 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
 
   best_val, best_cts, best_dscr, best_groupings = -np.inf, None, None, None
   for dscr in itertools_product(*dscr_hp_vals):
-    nu = dscr[0] if has_nu else None
+    nu = kernel_dscr(dscr)
     if not additive:
       opt_val, opt_pt, opt_groupings = optimise_cts(nu, max_evals) + (None,)
     else:
@@ -399,9 +439,16 @@ def layout_from_fitter(fitter):
         domain_use_same_bandwidth=bool(getattr(opt, 'domain_use_same_bandwidth', False)), **common)
     return None if sum(layout.tuned_nus()) > 1 else layout
   kernel_type = getattr(fitter, 'kernel_type', getattr(opt, 'kernel_type', None))
+  additive = bool(getattr(opt, 'use_additive_gp', False))
+  if kernel_type == 'esp':
+    # EuclideanGPFitter._esp_kernel_set_up (euclidean_gp.py:283-299); ESP together with use_additive_gp falls through
+    if additive or getattr(opt, 'esp_kernel_type', 'se') not in ('se', 'matern'):
+      return None
+    return EuclideanHPLayout(fitter.dim, 'esp', esp_kernel_type=getattr(opt, 'esp_kernel_type', 'se'),
+                             esp_order=int(getattr(opt, 'esp_order', -1)),
+                             esp_matern_nu=getattr(opt, 'esp_matern_nu', -1.0), **common)
   if kernel_type not in ('se', 'matern'):
     return None
-  additive = bool(getattr(opt, 'use_additive_gp', False))
   return EuclideanHPLayout(
       fitter.dim, kernel_type, nu=getattr(opt, 'matern_nu', 2.5),
       use_same_bandwidth=bool(getattr(opt, 'use_same_bandwidth', False)),

@@ -1,14 +1,15 @@
 """
 Host-side mirror of dragonfly/gp/kernel.py for the kernels on the hot path: SEKernel, MaternKernel,
-AdditiveKernel, CoordinateProductKernel (same constructor arguments, `hyperparams` dict, `dim`,
+AdditiveKernel, CoordinateProductKernel, ESPKernel (same constructor arguments, `hyperparams` dict, `dim`,
 `kernel_list` / `groupings` / `coordinate_list`, `is_guaranteed_psd`, `__call__`), plus the
 translation of such kernel objects -- these classes OR the reference's own, duck-typed by class name
 so that a patched Dragonfly install needs no changes -- into the POD `dfb_kernel_desc` that
 libdfb200's CUDA kernels evaluate (include/dfb200.h).
 
-`Kernel.__call__(X1, X2)` (kernel.py:72-83) runs on the GPU through dfb_kernel_matrix.  Kernel types
-outside the hot-path scope (Poly, ExpDecay, Hamming, ESP, NN kernels) raise NotImplementedError:
-there is no CPU fallback.
+`Kernel.__call__(X1, X2)` (kernel.py:72-83) runs on the GPU through dfb_kernel_matrix.  ESPKernel /
+ESPKernelSE / ESPKernelMatern (kernel.py:671-744) map to the descriptor's ESP form (esp_order > 0).  Kernel types
+outside the hot-path scope (Poly, ExpDecay, Hamming, NN kernels, an ESP kernel nested in another) raise
+NotImplementedError: there is no CPU fallback.
 """
 import math
 
@@ -203,6 +204,42 @@ class CoordinateProductKernel(Kernel):
         ['%s(%s)' % (g, k) for (g, k) in zip(self.coordinate_list, self.kernel_list)])
 
 
+class ESPKernel(Kernel):
+  """ kernel.py:671-726: the ESP kernel of Kandasamy & Yu (2016), scale * e_order(k_1(x_1, y_1), ..., k_d(x_d, y_d)),
+      e_order the elementary symmetric polynomial of the d one-dimensional child kernels. """
+
+  def __init__(self, scale, order, kernel_list):
+    super(ESPKernel, self).__init__()
+    self.dim = len(kernel_list)
+    self.kernel_list = kernel_list
+    self.add_hyperparams(scale=scale, order=order)
+    if self.dim < 0:
+      raise ValueError("dim cannot not be negative")
+    if order > self.dim:
+      raise ValueError("order must be less than or equal to dim")
+    if order < 1:
+      raise ValueError("order must be an integer between 1 and dim")
+
+  def is_guaranteed_psd(self):
+    return all([kern.is_guaranteed_psd() for kern in self.kernel_list])
+
+
+class ESPKernelSE(ESPKernel):
+  """ kernel.py:729-735: one 1-D SE child of scale 1 per dimension. """
+
+  def __init__(self, dim, scale, order, dim_bandwidths):
+    kernel_list = [SEKernel(1, 1.0, float(np.asarray(dim_bandwidths[i]).item())) for i in range(dim)]
+    super(ESPKernelSE, self).__init__(scale, order, kernel_list)
+
+
+class ESPKernelMatern(ESPKernel):
+  """ kernel.py:738-744: one 1-D Matern child of scale 1 per dimension, nu[i] per dimension. """
+
+  def __init__(self, dim, nu, scale, order, dim_bandwidths):
+    kernel_list = [MaternKernel(1, nu[i], 1.0, float(np.asarray(dim_bandwidths[i]).item())) for i in range(dim)]
+    super(ESPKernelMatern, self).__init__(scale, order, kernel_list)
+
+
 def kernel_from_spec(spec):
   """ Builds a kernel object from the nested-dict form used by synth_data.make_workload. """
   t = spec['type']
@@ -231,12 +268,12 @@ class _Factor(object):
 def _kind_of(kern):
   """ Duck-typed dispatch on the class name so the reference's own kernel objects work too. """
   names = [c.__name__ for c in type(kern).__mro__]
-  for n in ('SEKernel', 'MaternKernel', 'AdditiveKernel', 'CoordinateProductKernel'):
+  for n in ('SEKernel', 'MaternKernel', 'AdditiveKernel', 'CoordinateProductKernel', 'ESPKernel'):
     if n in names:
       return n
   raise NotImplementedError(
       'Kernel type %s is outside the GPU hot-path scope (supported: SEKernel, MaternKernel, '
-      'AdditiveKernel, CoordinateProductKernel); there is no CPU fallback.' % (type(kern).__name__))
+      'AdditiveKernel, CoordinateProductKernel, ESPKernel); there is no CPU fallback.' % (type(kern).__name__))
 
 
 def _expand(kern, train_coords, cand_coords):
@@ -263,6 +300,8 @@ def _expand(kern, train_coords, cand_coords):
       # K = hyperparams['scale'] * norm_constant * unnorm: the first product is formed on the host
       f.scale = float(kern.hyperparams['scale'] * consts['norm_constant'])
     return 1.0, [(1.0, [f])]
+  if kind == 'ESPKernel':
+    raise NotImplementedError('An ESP kernel inside an additive or product kernel is outside the GPU hot-path scope.')
   if kind == 'AdditiveKernel':
     terms = []
     for sub, grp in zip(kern.kernel_list, kern.groupings):
@@ -295,6 +334,37 @@ def _base_at_zero(f):
   return f.scale * u
 
 
+def esp_combine(values, order):
+  """ e_order(values) in the reference's operation order (ESPKernel._child_evaluate, kernel.py:710-726), for scalars or
+      NumPy arrays: power sums p_i = ((0 + v_1^i) + v_2^i) + ... (^1 = v, ^2 = v * v, ^i>=3 = pow), then Newton-Girard
+      e_m = (sum_{i=1..m} ((-1)^(i-1) e_{m-i}) p_i) / m. """
+  p = [None] + [0.0 * values[0] for _ in range(order)]
+  for i in range(1, order + 1):
+    for v in values:
+      p[i] = p[i] + (v if i == 1 else (v * v if i == 2 else v ** i))
+  e = [1.0 + 0.0 * values[0]] + [None] * order
+  for m in range(1, order + 1):
+    acc = 0.0 * values[0]
+    for i in range(1, m + 1):
+      acc = acc + (((-1) ** (i - 1)) * e[m - i]) * p[i]
+    e[m] = acc / m
+  return e[order]
+
+
+def _expand_esp(kern, train_coords, cand_coords):
+  """ ESPKernel -> (scale, one term per 1-D child) for the ESP form of the descriptor (esp_order > 0). """
+  if len(kern.kernel_list) != len(train_coords):
+    raise ValueError('ESP kernel has %d children for %d coordinates' % (len(kern.kernel_list), len(train_coords)))
+  terms = []
+  for t, sub in enumerate(kern.kernel_list):
+    if _kind_of(sub) not in ('SEKernel', 'MaternKernel') or int(sub.dim) != 1:
+      raise NotImplementedError('ESP children must be 1-D SE or Matern kernels on device (got %s).'
+                                % (type(sub).__name__))
+    _, sub_terms = _expand(sub, [train_coords[t]], [cand_coords[t]])
+    terms += sub_terms
+  return float(kern.hyperparams['scale']), terms
+
+
 def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, cand_dim=None):
   """ kern -> _lib.KernelDesc.  By default train and candidate matrices share the column layout
       (kernel applied to columns 0..dim-1).  Add-UCB passes train_coords = the group's columns of
@@ -308,7 +378,12 @@ def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, 
     train_dim = max(train_coords) + 1
   if cand_dim is None:
     cand_dim = max(cand_coords) + 1
-  post, terms = _expand(kern, train_coords, cand_coords)
+  esp_order = 0
+  if _kind_of(kern) == 'ESPKernel':
+    esp_order = int(kern.hyperparams['order'])
+    post, terms = _expand_esp(kern, train_coords, cand_coords)
+  else:
+    post, terms = _expand(kern, train_coords, cand_coords)
   n_factors = sum(len(facs) for _, facs in terms)
   n_slots = sum(len(f.bandwidths) for _, facs in terms for f in facs)
   if len(terms) > _lib.DFB_MAX_TERMS or n_factors > _lib.DFB_MAX_FACTORS or \
@@ -341,4 +416,22 @@ def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, 
     total = total + prod
   d.term_first_factor[len(terms)] = fi
   d.kss = float(post * total)
+  if esp_order:
+    # stationary: k(x, x) = scale * e_order(child values at distance 0)
+    d.esp_order = esp_order
+    d.kss = float(post * esp_combine([_base_at_zero(facs[0]) for _, facs in terms], esp_order))
+  check_esp_descriptor(d)
   return d
+
+
+def check_esp_descriptor(d):
+  """ The ESP rules of dfb_set_kernel's descriptor check (api.cu: check_desc), raised as ValueError before the
+      descriptor reaches the device: 0 <= esp_order <= n_terms, and for esp_order > 0 every term one 1-slot factor with
+      pre_scale 1. """
+  if d.esp_order < 0 or d.esp_order > d.n_terms:
+    raise ValueError('ESP order %d outside 0 .. n_terms = %d' % (d.esp_order, d.n_terms))
+  if d.esp_order > 0:
+    for t in range(d.n_terms):
+      f = d.term_first_factor[t]
+      if d.term_first_factor[t + 1] != f + 1 or d.factors[f].n_dims != 1 or d.term_pre_scale[t] != 1.0:
+        raise ValueError('ESP term %d is not one 1-slot factor with pre_scale 1' % (t))

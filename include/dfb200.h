@@ -59,6 +59,16 @@ extern "C" {
  * A slot is one (coordinate, bandwidth) pair of one factor; the train and candidate matrices may
  * use different column indices for the same slot (Add-UCB scores d_j-column candidates against
  * columns g_j of the training matrix, gpb_acquisitions.py:160-168).
+ *
+ * esp_order = 0 selects the sum above.  esp_order = r > 0 selects the ESP kernel (Kandasamy & Yu
+ * 2016; ESPKernel, kernel.py:671-744): every term is exactly one factor on one slot with
+ * pre_scale 1, v_t is that factor's value, and
+ *     k(x, y) = post_scale * e_r(v_1, ..., v_T)                     (1 <= r <= T = n_terms)
+ * in the reference's operation order (Newton-Girard identities):
+ *     p_i = ((0 + v_1^i) + v_2^i) + ... + v_T^i        i = 1..r   (^2 = v*v, ^i>=3 = pow(v, i))
+ *     e_0 = 1;  e_m = ((0 + (+e_{m-1}) p_1) + (-e_{m-2}) p_2 + ... ((-1)^(m-1) e_0) p_m) / m
+ * Its values may be slightly negative where the exact value is ~0 (cancellation), |k| <= k(x, x).
+ *   ESPKernelSE / ESPKernelMatern : T terms of one 1-D factor (scale 1), post_scale = outer scale
  */
 #define DFB_MAX_FACTORS   48
 #define DFB_MAX_TERMS     48
@@ -86,7 +96,7 @@ typedef struct dfb_kernel_desc {
   int32_t n_slots;
   int32_t train_dim;     /* columns of the training matrix */
   int32_t cand_dim;      /* columns of the candidate matrix */
-  int32_t reserved;
+  int32_t esp_order;     /* 0: sum of products; r > 0: ESP kernel of order r (see above) */
   double  post_scale;
   double  kss;           /* k(x, x) for any x (all supported kernels are stationary) */
   int32_t term_first_factor[DFB_MAX_TERMS + 1];
@@ -188,8 +198,8 @@ int dfb_restore_posterior(dfb_handle* h);
  *   out_host[2]     'noise_mean' = sum(alpha)                                                  gp_core.py:234-235
  *   out_host[3]     'same_dim_bandwidths'
  *   out_host[4 + j] 'dim_bandwidths', param_num = j  (j < d)
- * n_out >= 4 + d.  Needs a full posterior (DFB_BUILD_FULL).  Returns -3 for composite kernels (the reference raises
- * NotImplementedError there, kernel.py:123-125).  Uses the K_* chunk buffer as scratch. */
+ * n_out >= 4 + d.  Needs a full posterior (DFB_BUILD_FULL).  Returns -3 for composite and ESP kernels (the reference
+ * raises NotImplementedError there, kernel.py:123-125).  Uses the K_* chunk buffer as scratch. */
 int dfb_lml_gradients(dfb_handle* h, double* out_host, int32_t n_out);
 
 /* max(diag K) of the last build -- the jitter ladder's scale (general_utils.py:183-189). */
