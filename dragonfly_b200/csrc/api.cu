@@ -439,8 +439,11 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   DFB_TRY(ensure_train_scaled(h));
   DFB_CUDA_OK(cudaMemsetAsync(h->info, 0, sizeof(int) * 4, h->stream));
   // A[last, :] = K(X[last], X) + (noise + jitter) I, identity on the padding rows -> Ks scratch (128 x npad)
-  DFB_TRY(launch_kstar(h, h->d_desc_tr, h->desc_tr, 1, h->tr.xs, h->tr.nrm, npad, nullptr, h->X + m0 * h->d,
-                       n - m0, h->d, TILE, h->Ks, npad, n, npad, 0.0, nullptr, nullptr));
+  KstarArgs ka{};
+  ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
+  ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X + m0 * h->d; ka.m = n - m0; ka.dc = h->d;
+  ka.m_rows = TILE; ka.n_valid = n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
+  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
   DFB_TRY(launch_set_diag(h, h->Ks + m0, npad, 0, n - m0, h->noise_plus_jitter, 1));
   DFB_TRY(launch_set_diag(h, h->Ks + m0, npad, n - m0, TILE, 1.0, 0));
   // The four left-looking products have 1 .. nb-1 output tiles with k-depths up to m0 ~ N: each tile's k-range is
@@ -558,7 +561,6 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   const int nb = (int)(npad / TILE);
   if (do_argmax && !md.keep_best) DFB_TRY(launch_reset_best(h));
   const bool i8 = want_std && md.use_i8;
-  const bool seg_ok = i8 && h->i8_fuse && h->kstar_fast && h->kstar_seg && h->i8_radix256;
   // host candidates are staged in batches of as many whole chunks as the staging buffer holds
   // (chunk x DFB_MAX_SLOTS doubles), so a 6-column candidate matrix needs 1 copy per ~21 chunks
   const int64_t stage_rows = (Mc * DFB_MAX_SLOTS / dc) / Mc * Mc;
@@ -606,6 +608,19 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   const int* abort_count = md.collect ? h->list_count : nullptr;
   const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
                      (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
+  // K_* arguments of every chunk; the candidates, their count and mu are set per chunk
+  KstarArgs ka{};
+  ka.desc = &desc; ka.d_desc = d_desc; ka.xsT = ss.xs; ka.nrmT = ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
+  ka.dc = dc; ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad; ka.mean_const = mean_const;
+  ka.kss_out = want_std ? h->kssv : nullptr; ka.abort_count = abort_count; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
+  if (i8) {
+    ka.planes = h->Ki8; ka.plane_bytes = 2 * h->chunk * npad; ka.row_bytes = 2 * npad;
+    ka.inv_colscale = 1.0 / i8_colscale(desc);
+  }
+  const KstarWant want = md.bound_pass ? KstarWant::MU_SCREEN
+                         : !want_std   ? KstarWant::MU
+                         : i8          ? KstarWant::DIGITS
+                                       : KstarWant::ROWS;
 
   for (int64_t ci = 0; ci < n_chunks; ci++) {
     const int64_t c0 = ci * Mc;
@@ -636,14 +651,18 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
                                                          : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
 
+    ka.Xc = xc_dev; ka.m = mc; ka.m_rows = m_rows; ka.mu = mu_dev;
+    const KstarRoute route = route_kstar(h, ka, want);
+
     if (md.bound_pass) {
       // mu (bit-identical to the digit kernel's) and k(x*, x*); no K_* rows, no contraction.  Void once the seed's
       // shortlist has overflowed, like every other launch of the int8 pass.
       DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
-      int emitted = 0;
-      DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
-                               h->mu, h->kssv, nullptr, 0, 0, 0.0, h->cprep, h->mu_part, Mc, &emitted, h->list_count));
-      if (!emitted) { set_error("bound pass: the mu-only K_* kernel does not serve this kernel"); return -1; }
+      if (route.producer != KstarProducer::SEG_MU) {
+        set_error("bound pass: the mu-only K_* kernel does not serve this kernel");
+        return -1;
+      }
+      DFB_TRY(launch_kstar(h, ka, route));
       DFB_TRY(launch_prune(h, acq, h->mu, h->kssv, mc, md.pad, md.idx_base + c0, xc_dev, dc));
       DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
       DFB_TRY(release_half(c0));
@@ -652,25 +671,10 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
 
     // K stage
     DFB_TRY(prof_begin(h, DFB_PROF_KSTAR));
-    int fused_digits = 0;
-    if (seg_ok)
-      DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
-                               mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad, 1.0 / i8_colscale(desc), h->cprep,
-                               h->mu_part, Mc, &fused_digits, abort_count));
-    else if (!want_std && h->kstar_rows64)    // mu alone: the row kernel's mu without writing its rows
-      DFB_TRY(launch_kstar_seg(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, h->n, xc_dev, mc, dc, m_rows, npad, mean_const,
-                               mu_dev, nullptr, nullptr, 0, 0, 0.0, h->cprep, h->mu_part, Mc, &fused_digits, nullptr));
-    if (!fused_digits && i8 && h->i8_fuse)
-      DFB_TRY(launch_kstar_i8(h, d_desc, desc, ss.xs, ss.nrm, npad, h->alpha, xc_dev, mc, dc, m_rows, h->n, npad,
-                              mean_const, mu_dev, h->kssv, h->Ki8, 2 * h->chunk * npad, 2 * npad,
-                              1.0 / i8_colscale(desc), &fused_digits, abort_count));
-    if (!fused_digits) {
-      DFB_TRY(launch_kstar(h, d_desc, desc, 0, ss.xs, ss.nrm, npad, h->alpha, xc_dev, mc, dc, m_rows,
-                           h->Ks, npad, h->n, npad, mean_const, mu_dev, want_std ? h->kssv : nullptr));
-      if (i8)     // K_* = 2^F * digits: |K_*| <= k(x,x) for every supported (stationary, non-negative) kernel
-        DFB_TRY(launch_slice_i8(h, h->Ks, npad, m_rows, npad, nullptr, 1.0 / i8_colscale(desc), h->Ki8,
-                                2 * h->chunk * npad, 2 * npad));
-    }
+    DFB_TRY(launch_kstar(h, ka, route));
+    if (route.slice_i8)     // K_* = 2^F * digits: |K_*| <= k(x,x) for every supported (stationary, non-negative) kernel
+      DFB_TRY(launch_slice_i8(h, h->Ks, npad, m_rows, npad, nullptr, ka.inv_colscale, h->Ki8, ka.plane_bytes,
+                              ka.row_bytes));
     DFB_TRY(prof_end(h, DFB_PROF_KSTAR, (double)mc));
 
     // G stage
@@ -873,8 +877,11 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   DFB_CUDA_OK(cudaMemsetAsync(h->T, 0, sizeof(double) * (size_t)(2 * npad + TILE) * npad, h->stream));
   DFB_TRY(ensure_train_scaled(h));
   // K(X, X): GP._get_training_kernel_matrix (gp_core.py:149-153)
-  DFB_TRY(launch_kstar(h, h->d_desc_tr, h->desc_tr, 1, h->tr.xs, h->tr.nrm, npad, nullptr, h->X, n, h->d,
-                       n, h->T, npad, n, npad, 0.0, nullptr, nullptr));
+  KstarArgs ka{};
+  ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
+  ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X; ka.m = n; ka.dc = h->d; ka.m_rows = n;
+  ka.n_valid = n; ka.n_write = npad; ka.Ks = h->T; ka.ldk = npad;
+  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
   DFB_TRY(launch_init_tall(h, h->T, n, npad, noise_var + jitter, h->yc, with_bottom ? 1 : 0));
   DFB_TRY(factorise_tall(h, h->T, npad, h->Dinv, h->info, with_bottom));
   const double* Wt = h->T + (size_t)npad * npad;
@@ -1027,9 +1034,13 @@ int dfb_get_state(dfb_handle* h, double* L_dev, double* alpha_dev, double* K_dev
   DFB_CUDA_OK(cudaSetDevice(h->device));
   if (L_dev) DFB_TRY(launch_extract_lower(h, h->T, h->npad, L_dev, h->n));
   if (alpha_dev) DFB_TRY(launch_copy_pad(h, h->alpha, h->n, alpha_dev, h->n));
-  if (K_dev)
-    DFB_TRY(launch_kstar(h, h->d_desc_tr, h->desc_tr, 1, h->tr.xs, h->tr.nrm, h->npad, nullptr, h->X, h->n,
-                         h->d, h->n, K_dev, h->n, h->n, h->n, 0.0, nullptr, nullptr));
+  if (K_dev) {
+    KstarArgs ka{};
+    ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
+    ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = h->npad; ka.Xc = h->X; ka.m = h->n; ka.dc = h->d;
+    ka.m_rows = h->n; ka.n_valid = h->n; ka.n_write = h->n; ka.Ks = K_dev; ka.ldk = h->n;
+    DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  }
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -1082,7 +1093,9 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
 static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, int64_t m,
                                int32_t dc, double b2) {
   if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC) return false;
-  if (!(h->i8_fuse && h->i8_radix256 && kstar_seg_applies(h, desc))) return false;    // run_chunks' digit kernel
+  KstarArgs ka{};                     // run_chunks' digit route of a full chunk: the bound pass's mu must be SEG_DIGITS'
+  ka.desc = &desc; ka.npad_tr = ka.n_write = h->npad; ka.m_rows = h->chunk;
+  if (route_kstar(h, ka, KstarWant::DIGITS).producer != KstarProducer::SEG_DIGITS) return false;
   if (!(acq.kind == DFB_ACQ_EI || acq.kind == DFB_ACQ_PI || (acq.kind == DFB_ACQ_UCB && acq.beta >= 0.0))) return false;
   // Variance floor.  K: the noiseless training kernel matrix, s: the diagonal actually added (noise + jitter, for every
   // point, hallucinated ones included), k = K(X, x*).  The joint covariance [[K, k], [k^T, k**]] is PSD, so
@@ -1239,8 +1252,11 @@ int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* 
   DFB_CUDA_OK(cudaMemcpyAsync(h->d_desc_tmp, &h->desc_tmp, sizeof(dfb_kernel_desc), cudaMemcpyHostToDevice, h->stream));
   h->te_prepped = false;   // the test-kernel scaled set is used as scratch
   DFB_TRY(launch_prep_scaled(h, h->d_desc_tmp, 1, X2_dev, n2, d2, h->te.xs, h->te.nrm, np2));
-  DFB_TRY(launch_kstar(h, h->d_desc_tmp, h->desc_tmp, 1, h->te.xs, h->te.nrm, np2, nullptr, X1_dev, n1, d1,
-                       n1, K_dev, n2, n2, n2, 0.0, nullptr, nullptr));
+  KstarArgs ka{};
+  ka.desc = &h->desc_tmp; ka.d_desc = h->d_desc_tmp; ka.cand_uses_train_coords = 1;
+  ka.xsT = h->te.xs; ka.nrmT = h->te.nrm; ka.npad_tr = np2; ka.Xc = X1_dev; ka.m = n1; ka.dc = d1; ka.m_rows = n1;
+  ka.n_valid = n2; ka.n_write = n2; ka.Ks = K_dev; ka.ldk = n2;
+  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -1261,8 +1277,11 @@ static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, 
   const int64_t npad = h->npad;
   const int nb = (int)(npad / TILE), mbb = (int)(mbp / TILE);
   // K_* rows (zero rows beyond m) and mu
-  DFB_TRY(launch_kstar(h, d_desc, desc, 0, ss.xs, ss.nrm, npad, h->alpha, Xc_dev, m, dc, mbp, h->Ks, npad,
-                       h->n, npad, mean_const, h->ts_mu, nullptr));
+  KstarArgs ka{};
+  ka.desc = &desc; ka.d_desc = d_desc; ka.xsT = ss.xs; ka.nrmT = ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
+  ka.Xc = Xc_dev; ka.m = m; ka.dc = dc; ka.m_rows = mbp; ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
+  ka.mean_const = mean_const; ka.mu = h->ts_mu; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
+  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
   // V^T[a][i] = sum_{k <= i} K_*[a][k] W[i][k]
   GemmArgs g;
   memset(&g, 0, sizeof(g));
@@ -1271,8 +1290,9 @@ static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, 
   DFB_TRY(launch_gemm(h, g, EPI_STORE, mbb * nb));
   // K** = kernel(X_test, X_test) (gp_core.py:179) with the candidates as both sides
   DFB_TRY(launch_prep_scaled(h, d_desc, 0, Xc_dev, m, dc, h->ts_cxs, h->ts_cnrm, mbp));
-  DFB_TRY(launch_kstar(h, d_desc, desc, 0, h->ts_cxs, h->ts_cnrm, mbp, nullptr, Xc_dev, m, dc, mbp, h->ts_Cov,
-                       mbp, m, mbp, 0.0, nullptr, nullptr));
+  ka.xsT = h->ts_cxs; ka.nrmT = h->ts_cnrm; ka.npad_tr = mbp; ka.alpha = nullptr; ka.n_valid = m; ka.n_write = mbp;
+  ka.Ks = h->ts_Cov; ka.ldk = mbp; ka.mean_const = 0.0; ka.mu = nullptr;
+  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
   // Cov = K** - V^T V
   memset(&g, 0, sizeof(g));
   g.A = h->ts_Vt; g.lda = npad; g.B = h->ts_Vt; g.ldb = npad; g.C = h->ts_Cov; g.ldc = mbp;

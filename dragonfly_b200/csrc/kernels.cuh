@@ -7,24 +7,36 @@ namespace dfb {
 
 int launch_prep_scaled(dfb_handle* h, const dfb_kernel_desc* d_desc, int use_train_coords,
                        const double* X, int64_t n, int d, double* xs, double* nrm, int64_t npad);
-int launch_kstar(dfb_handle* h, const dfb_kernel_desc* d_desc, const dfb_kernel_desc& desc,
-                 int cand_uses_train_coords, const double* xsT, const double* nrmT, int64_t npad_tr,
-                 const double* alpha, const double* Xc, int64_t m, int dc, int64_t m_rows, double* Ks,
-                 int64_t ldk, int64_t n_valid, int64_t n_write, double mean_const, double* mu,
-                 double* kss_out);
-int launch_kstar_i8(dfb_handle* h, const dfb_kernel_desc* d_desc, const dfb_kernel_desc& desc,
-                    const double* xsT, const double* nrmT, int64_t npad_tr, const double* alpha,
-                    const double* Xc, int64_t m, int dc, int64_t m_rows, int64_t n_valid, int64_t n_write,
-                    double mean_const, double* mu, double* kss_out, void* planes, int64_t plane_bytes,
-                    int64_t row_bytes, double inv_colscale, int* emitted_i8, const int* abort_count = nullptr);
-// second-generation K_* path (kernels.cu: kstar_seg_kernel): digit planes, or mu alone when planes is NULL (mu and
-// mu_part required)
-bool kstar_seg_applies(const dfb_handle* h, const dfb_kernel_desc& desc);
-int launch_kstar_seg(dfb_handle* h, const dfb_kernel_desc* d_desc, const dfb_kernel_desc& desc, const double* xsT,
-                     const double* nrm, int64_t npad_tr, const double* alpha, int64_t n_valid, const double* Xc, int64_t m,
-                     int dc, int64_t m_rows, int64_t n_write, double mean_const, double* mu, double* kss_out, void* planes,
-                     int64_t plane_bytes, int64_t row_bytes, double inv_colscale, double* cprep, double* mu_part,
-                     int64_t ld_mu, int* emitted, const int* abort_count = nullptr);
+// ---- K_* stage: kernel rows k(x*, X), mu and k(x*, x*) of a block of candidates ----
+// Everything one K_* launch reads and writes.  Which of the fields a producer uses is up to the producer.
+struct KstarArgs {
+  const dfb_kernel_desc* desc;        // host copy: picks the producer and its template arguments
+  const dfb_kernel_desc* d_desc;      // the same descriptor on the device
+  int cand_uses_train_coords;         // 1: the candidates are training points (K(X, X) builds)
+  const double* xsT; const double* nrmT; int64_t npad_tr;    // scaled training set (launch_prep_scaled)
+  const double* alpha;                // NULL: no mu
+  const double* Xc; int64_t m; int dc; int64_t m_rows;       // candidates; rows m .. m_rows-1 are written as padding
+  int64_t n_valid, n_write;           // training points that count / columns written
+  double* Ks; int64_t ldk;            // fp64 rows
+  double mean_const; double* mu; double* kss_out;            // mu and k(x*, x*); either may be NULL
+  void* planes; int64_t plane_bytes, row_bytes; double inv_colscale;    // int8 digit planes
+  const int* abort_count;             // digit and mu-only producers: no-op once *abort_count > SHORTLIST_CAP; may be NULL
+  double* cprep; double* mu_part;     // segment-kernel scratch (h->cprep, h->mu_part)
+};
+enum class KstarWant {
+  ROWS,           // fp64 rows (+ mu, k(x*, x*) when asked)
+  DIGITS,         // int8 digit planes + mu + k(x*, x*)
+  MU,             // mu alone, as ROWS computes it (mean-only dfb_eval)
+  MU_SCREEN,      // mu + k(x*, x*) alone, as SEG_DIGITS computes them (bound pass of dfb_score_argmax)
+};
+enum class KstarProducer { SEG_DIGITS, SEG_ROWS64, SEG_MU, FAST_DIGITS, FAST_ROWS, ESP_DIGITS, ESP_ROWS, INTERP_ROWS };
+struct KstarRoute {
+  KstarProducer producer;
+  bool slice_i8;                      // DIGITS served by an fp64 row producer: launch_slice_i8 of a.Ks must follow
+};
+// The producer of a K_* launch (table in kernels.cu); host logic only
+KstarRoute route_kstar(const dfb_handle* h, const KstarArgs& a, KstarWant want);
+int launch_kstar(dfb_handle* h, const KstarArgs& a, KstarRoute route);
 int launch_init_tall(dfb_handle* h, double* T, int64_t n, int64_t npad, double diag_add,
                      const double* yc, int with_bottom);
 int launch_chol_diag(dfb_handle* h, double* T, int64_t ld, int step, double* Dinv, int* info);

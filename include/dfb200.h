@@ -346,7 +346,9 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *                 dims, radix-256 digits, no test kernel, m > chunk, no score vector, and when the posterior's variance
  *                 floor k** s / (n k** + s) (s = noise + jitter) exceeds the int8 error bound.  0 = contract every
  *                 candidate.
- *  "kstar_fast", "tma_cb_group": kernel-selection / scheduling knobs. */
+ *  "kstar_fast" : 1 (default) = plain SE / Matern kernels on <= 8 dims get specialised K_* kernels; 0 = they go through
+ *                 the descriptor interpreter (kstar_kernel).  Which K_* kernel runs: kernels.cu, route_kstar.
+ *  "tma_cb_group": scheduling knob of the fp64 TMA contraction. */
 int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
 /* Diagnostics: "i8_sigma2_bound", "i8_bound_limit", "i8_ready", "i8_radix256", "score_impl",
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen

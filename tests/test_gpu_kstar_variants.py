@@ -1,8 +1,8 @@
 """
 Every K_* kernel variant of the plain SE / Matern kernels, at every compiled dimension d = 1 .. 8 (-m gpu).
 
-The K_* stage is picked at run time by kernel kind and d (kernels.cu: launch_kstar, launch_kstar_i8, launch_kstar_seg,
-launch_kstar_rows64); each path below is forced through the handle's options and read back with dfb_debug_copy:
+The K_* producer is picked at run time by the options, kernel kind and d (kernels.cu: route_kstar); each path below is
+forced through the handle's options and read back with dfb_debug_copy:
   P1  kstar_kernel (the descriptor interpreter)        kstar_fast = 0
   P2  kstar_fast_kernel, fp64 rows                      kstar_rows64 = 0
   P3  cand_prep + kstar_seg_kernel<ROWS64>, fp64 rows   score_impl = 0 (the default fp64 build of dfb_eval)
