@@ -15,7 +15,7 @@ DFB_MAX_FACTORS = 48
 DFB_MAX_TERMS = 48
 DFB_MAX_SLOTS = 128
 DFB_MAX_MATERN_P = 3
-DFB_BASE_SE, DFB_BASE_MATERN = 0, 1
+DFB_BASE_SE, DFB_BASE_MATERN, DFB_BASE_POLY, DFB_BASE_EXPDECAY = 0, 1, 2, 3
 DFB_DEVICE, DFB_HOST = 0, 1
 DFB_ACQ_MEAN, DFB_ACQ_UCB, DFB_ACQ_EI, DFB_ACQ_PI, DFB_ACQ_TTEI = 0, 1, 2, 3, 4
 DFB_BUILD_FULL, DFB_BUILD_LML_ONLY, DFB_BUILD_NO_ALPHA = 0, 1, 2

@@ -147,17 +147,41 @@ static int check_desc(const dfb_kernel_desc* d) {
   }
   for (int f = 0; f < d->n_factors; f++) {
     const dfb_factor_desc& fd = d->factors[f];
-    if ((fd.kind != DFB_BASE_SE && fd.kind != DFB_BASE_MATERN) || fd.n_dims < 1 ||
+    if (fd.kind < DFB_BASE_SE || fd.kind > DFB_BASE_EXPDECAY || fd.n_dims < 1 ||
         fd.slot_off < 0 || fd.slot_off + fd.n_dims > d->n_slots || fd.p < 0 ||
-        fd.p > DFB_MAX_MATERN_P) {
+        (fd.kind == DFB_BASE_MATERN && fd.p > DFB_MAX_MATERN_P) || (fd.kind == DFB_BASE_EXPDECAY && fd.p != 0) ||
+        (fd.kind >= DFB_BASE_POLY && !(fd.scale > 0.0 && isfinite(fd.scale))) ||
+        (fd.kind == DFB_BASE_EXPDECAY && !isfinite(fd.s2))) {
       set_error("kernel descriptor: bad factor %d", f);
       return -1;
     }
+    // slot_bandwidth means a bandwidth, a scaling or a power depending on the kind (dfb200.h): a slot of a POLY or
+    // EXPDECAY factor belongs to that factor alone
+    if (fd.kind >= DFB_BASE_POLY) {
+      for (int g = 0; g < d->n_factors; g++) {
+        const dfb_factor_desc& gd = d->factors[g];
+        if (g != f && gd.slot_off < fd.slot_off + fd.n_dims && fd.slot_off < gd.slot_off + gd.n_dims) {
+          set_error("kernel descriptor: factor %d shares slots with POLY / EXPDECAY factor %d", g, f);
+          return -1;
+        }
+      }
+      for (int q = 0; q < fd.n_dims; q++) {
+        if (!isfinite(d->slot_bandwidth[fd.slot_off + q])) {
+          set_error("kernel descriptor: factor %d has a non-finite %s", f, fd.kind == DFB_BASE_POLY ? "scaling" : "power");
+          return -1;
+        }
+      }
+    }
   }
   for (int s = 0; s < d->n_slots; s++) {
+    bool bandwidth = true;              // every slot but those of POLY / EXPDECAY factors holds a bandwidth
+    for (int f = 0; f < d->n_factors; f++) {
+      const dfb_factor_desc& fd = d->factors[f];
+      if (fd.kind >= DFB_BASE_POLY && s >= fd.slot_off && s < fd.slot_off + fd.n_dims) bandwidth = false;
+    }
     if (d->slot_train_coord[s] < 0 || d->slot_train_coord[s] >= d->train_dim ||
         d->slot_cand_coord[s] < 0 || d->slot_cand_coord[s] >= d->cand_dim ||
-        !(d->slot_bandwidth[s] > 0.0)) {
+        (bandwidth && !(d->slot_bandwidth[s] > 0.0))) {
       set_error("kernel descriptor: bad slot %d", s);
       return -1;
     }
@@ -171,6 +195,10 @@ static int check_desc(const dfb_kernel_desc* d) {
       const int f = d->term_first_factor[t];
       if (d->term_first_factor[t + 1] != f + 1 || d->factors[f].n_dims != 1 || d->term_pre_scale[t] != 1.0) {
         set_error("kernel descriptor: ESP term %d is not one 1-slot factor with pre_scale 1", t);
+        return -1;
+      }
+      if (d->factors[f].kind >= DFB_BASE_POLY) {
+        set_error("kernel descriptor: ESP term %d is a POLY / EXPDECAY factor (ESP children are SE or Matern)", t);
         return -1;
       }
     }
@@ -365,8 +393,9 @@ static double i8_sigma2_bound(const dfb_handle* h, const dfb_kernel_desc& desc) 
          ldexp(1.0, h->i8_radix256 ? -40 : -43) * sqrt(desc.kss);
 }
 static const double I8_BOUND_LIMIT = 5e-9;     // absolute: half of the 1e-8 sigma^2 contract
+// The colscale and the bound rest on one k(x, x) for all candidates: non-stationary kernels are scored in fp64 only.
 static bool i8_usable(const dfb_handle* h, const dfb_kernel_desc& desc) {
-  if (!h->i8_ready || !(desc.kss > 0.0)) return false;
+  if (!h->i8_ready || !kernel_stationary(desc) || !(desc.kss > 0.0)) return false;
   if (h->i8_unguarded) return true;                 // diagnostics only (tools/sweep_i8_bound.py)
   return i8_sigma2_bound(h, desc) <= I8_BOUND_LIMIT;
 }
@@ -406,7 +435,9 @@ static int prepare_scoring(dfb_handle* h, bool i8, bool tma) {
   if (tma) h->tma_ready = false;
   if (!h->have_post || !h->have_w) return 0;
   DFB_CUDA_OK(cudaSetDevice(h->device));
-  if (i8 && (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024))) DFB_TRY(prepare_i8(h));
+  // a non-stationary training kernel never takes the int8 path (i8_usable), so its digit planes are not made
+  if (i8 && (h->score_impl == 1 || (h->score_impl == 2 && h->n >= 1024)) && kernel_stationary(h->desc_tr))
+    DFB_TRY(prepare_i8(h));
   if (tma && h->gemm_impl == 1) {
     DFB_TRY(make_tensor_map_2d_f64(&h->tmW, h->W, h->npad, h->npad, h->npad));
     DFB_TRY(make_tensor_map_2d_f64(&h->tmK, h->Ks, h->chunk, h->npad, h->npad));
@@ -444,6 +475,9 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X + m0 * h->d; ka.m = n - m0; ka.dc = h->d;
   ka.m_rows = TILE; ka.n_valid = n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
   DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  // a non-stationary kernel's max(diag K) can grow with the appended points: the block's diagonal is rebuilt here
+  const bool stationary = kernel_stationary(h->desc_tr);
+  if (!stationary) DFB_TRY(launch_diag_max(h, h->Ks + m0, npad, n - m0, h->red + 6));
   DFB_TRY(launch_set_diag(h, h->Ks + m0, npad, 0, n - m0, h->noise_plus_jitter, 1));
   DFB_TRY(launch_set_diag(h, h->Ks + m0, npad, n - m0, TILE, 1.0, 0));
   // The four left-looking products have 1 .. nb-1 output tiles with k-depths up to m0 ~ N: each tile's k-range is
@@ -494,11 +528,12 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   DFB_TRY(launch_transpose(h, Wt, h->W, npad));
   if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
   DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
-  double red[3];
+  double red[7];
   int info = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(red), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(double) * (stationary ? 3 : 7), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaMemcpyAsync(&info, h->info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  if (!stationary) h->max_diag = fmax(h->max_diag, red[6] + h->noise_var);
   if (info != 0) {
     set_error("extended matrix is not positive definite: non-positive pivot at index %d", info - 1);
     return info;
@@ -882,6 +917,9 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X; ka.m = n; ka.dc = h->d; ka.m_rows = n;
   ka.n_valid = n; ka.n_write = npad; ka.Ks = h->T; ka.ldk = npad;
   DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  // the jitter ladder's scale max(diag K) + noise: kss for a stationary kernel, else read off the diagonal just built
+  const bool stationary = kernel_stationary(h->desc_tr);
+  if (!stationary) DFB_TRY(launch_diag_max(h, h->T, npad, n, h->red + 6));
   DFB_TRY(launch_init_tall(h, h->T, n, npad, noise_var + jitter, h->yc, with_bottom ? 1 : 0));
   DFB_TRY(factorise_tall(h, h->T, npad, h->Dinv, h->info, with_bottom));
   const double* Wt = h->T + (size_t)npad * npad;
@@ -890,12 +928,13 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
   DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
   DFB_TRY(prof_end(h, DFB_PROF_BUILD, 1.0));
-  double red[3];
+  double red[7];
   int info = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(red), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(double) * (stationary ? 3 : 7), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaMemcpyAsync(&info, h->info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  h->max_diag = h->desc_tr.kss + noise_var;
+  h->max_diag = (stationary ? h->desc_tr.kss : red[6]) + noise_var;
+  h->noise_var = noise_var;
   if (info != 0) {
     set_error("matrix is not positive definite: non-positive pivot at index %d", info - 1);
     return info;
@@ -937,6 +976,7 @@ int dfb_extend_posterior(dfb_handle* h, const double* X_new_dev, int64_t q, cons
                                 cudaMemcpyDeviceToDevice, h->stream));
     DFB_CUDA_OK(cudaMemcpyAsync(s + 2 * TILE * npad + TILE, h->alpha, sizeof(double) * npad, cudaMemcpyDeviceToDevice, h->stream));
     h->ext_saved_n = n0;
+    h->ext_saved_max_diag = h->max_diag;
   }
   DFB_CUDA_OK(cudaMemcpyAsync(h->X + n0 * h->d, X_new_dev, sizeof(double) * q * h->d, cudaMemcpyDeviceToDevice, h->stream));
   DFB_CUDA_OK(cudaMemcpyAsync(h->yc + n0, y_centred_new_dev, sizeof(double) * q, cudaMemcpyDeviceToDevice, h->stream));
@@ -969,6 +1009,7 @@ int dfb_restore_posterior(dfb_handle* h) {
   DFB_CUDA_OK(cudaMemcpyAsync(h->alpha, s + 2 * TILE * npad + TILE, sizeof(double) * npad, cudaMemcpyDeviceToDevice, h->stream));
   DFB_TRY(launch_fill(h, h->yc + n0, npad - n0, 0.0));           // zero the appended targets
   h->n = n0;
+  h->max_diag = h->ext_saved_max_diag;
   h->ext_saved = false;
   h->tr_prepped = h->te_prepped = false;
   DFB_TRY(launch_transpose(h, h->T + npad * npad, h->W, npad));
@@ -981,10 +1022,12 @@ int dfb_restore_posterior(dfb_handle* h) {
 int dfb_lml_gradients(dfb_handle* h, double* out_host, int32_t n_out) {
   DFB_TRY(need(h, true, true, true, true, true));
   const dfb_kernel_desc& desc = h->desc_tr;
-  if (desc.n_terms != 1 || desc.n_factors != 1 || desc.esp_order != 0) {
-    // the reference's composite and ESP kernels inherit Kernel._child_gradient, which raises (kernel.py:123-125)
+  if (desc.n_terms != 1 || desc.n_factors != 1 || desc.esp_order != 0 ||
+      (desc.factors[0].kind != DFB_BASE_SE && desc.factors[0].kind != DFB_BASE_MATERN)) {
+    // the reference's composite, ESP, Poly and ExpDecay kernels inherit Kernel._child_gradient, which raises
+    // (kernel.py:123-125)
     set_error("LML gradients are defined for plain SE / Matern kernels only (kernel has %d terms, %d factors, "
-              "ESP order %d)", desc.n_terms, desc.n_factors, desc.esp_order);
+              "ESP order %d, first factor kind %d)", desc.n_terms, desc.n_factors, desc.esp_order, desc.factors[0].kind);
     return -3;
   }
   const int D = desc.factors[0].n_dims;
@@ -1092,7 +1135,7 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
 // chunks 1.. are then scored as today, still continuing the seed's state.
 static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, int64_t m,
                                int32_t dc, double b2) {
-  if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC) return false;
+  if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC || !kernel_stationary(desc)) return false;
   KstarArgs ka{};                     // run_chunks' digit route of a full chunk: the bound pass's mu must be SEG_DIGITS'
   ka.desc = &desc; ka.npad_tr = ka.n_write = h->npad; ka.m_rows = h->chunk;
   if (route_kstar(h, ka, KstarWant::DIGITS).producer != KstarProducer::SEG_DIGITS) return false;

@@ -31,6 +31,14 @@ void set_error(const char* fmt, ...);
 
 static inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
+// k(x, x) is the same for every x -- and the descriptor's kss means something -- unless a factor is POLY or EXPDECAY
+// (dfb200.h).  Everything that relies on a constant k(x, x) asks here: the int8 screen, the bound pass, max_diag.
+static inline bool kernel_stationary(const dfb_kernel_desc& d) {
+  for (int f = 0; f < d.n_factors; f++)
+    if (d.factors[f].kind == DFB_BASE_POLY || d.factors[f].kind == DFB_BASE_EXPDECAY) return false;
+  return true;
+}
+
 // ------------------------------------------------------------------------------------------------
 // Device-side view of the posterior state and the workspace carve-up.
 // ------------------------------------------------------------------------------------------------
@@ -184,5 +192,7 @@ struct dfb_handle {
   double* ext_save = nullptr;   // (2*TILE + 1) * npad + TILE doubles
   bool ext_saved = false;
   int64_t ext_saved_n = 0;
-  double max_diag = 0.0;
+  double ext_saved_max_diag = 0.0;
+  double max_diag = 0.0;      // max(diag K) + noise_var of the current posterior (dfb_get_max_diag)
+  double noise_var = 0.0;     // of the last dfb_build_posterior
 };

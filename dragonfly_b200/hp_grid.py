@@ -17,8 +17,8 @@ CPU tests of the sharding logic).
 import numpy as np
 
 from . import _lib
-from .kernel import SEKernel, MaternKernel, AdditiveKernel, CoordinateProductKernel, ESPKernelSE, ESPKernelMatern, \
-    build_descriptor
+from .kernel import SEKernel, MaternKernel, ExpDecayKernel, AdditiveKernel, CoordinateProductKernel, ESPKernelSE, \
+    ESPKernelMatern, build_descriptor
 from .gp_core import stable_cholesky_on_device
 
 
@@ -157,16 +157,18 @@ class EuclideanHPLayout(object):
 
 
 class EuclideanMFHPLayout(EuclideanHPLayout):
-  """ Hyper-parameter vector of the reference's EuclideanMFGPFitter (euclidean_gp.py:432-483, 680-709): [mean const]?
-      [log noise]? log scale, log fidelity bandwidth(s), log domain bandwidth(s); at most one tuned Matern nu (fidelity
-      or domain) as the discrete hp.  The GP lives on [z || x] rows with the product kernel
-      scale * k_F(z, z') * k_D(x, x') (fidelity and domain kernels with scale 1). """
+  """ Hyper-parameter vector of the reference's EuclideanMFGPFitter (euclidean_gp.py:432-483, 680-709) with SE / Matern
+      fidelity and domain kernels: [mean const]? [log noise]? log scale, log fidelity bandwidth(s), log domain
+      bandwidth(s); at most one tuned Matern nu (fidelity or domain) as the discrete hp.  The GP lives on [z || x] rows
+      with the product kernel scale * k_F(z, z') * k_D(x, x') (fidelity and domain kernels with scale 1).  An ExpDecay
+      fidelity kernel has no bandwidths: EuclideanMFExpDecayHPLayout below. """
+  FIDEL_KERNEL_TYPES = ('se', 'matern')
 
   def __init__(self, fidel_dim, domain_dim, fidel_kernel_type='se', domain_kernel_type='se', fidel_nu=2.5,
                domain_nu=2.5, fidel_use_same_bandwidth=False, domain_use_same_bandwidth=False, **kwargs):
-    for kt in (fidel_kernel_type, domain_kernel_type):
-      if kt not in ('se', 'matern'):
-        raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kt))
+    for kt, allowed in ((fidel_kernel_type, self.FIDEL_KERNEL_TYPES), (domain_kernel_type, ('se', 'matern'))):
+      if kt not in allowed:
+        raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope of %s.' % (kt, type(self).__name__))
     super(EuclideanMFHPLayout, self).__init__(fidel_dim + domain_dim, 'se', **kwargs)
     self.fidel_dim, self.domain_dim = fidel_dim, domain_dim
     self.fidel_kernel_type, self.domain_kernel_type = fidel_kernel_type, domain_kernel_type
@@ -180,8 +182,11 @@ class EuclideanMFHPLayout(EuclideanHPLayout):
     return [self.fidel_kernel_type == 'matern' and self.fidel_nu < 0,
             self.domain_kernel_type == 'matern' and self.domain_nu < 0]
 
+  def _num_fidel_hps(self):
+    return 1 if self.fidel_use_same_bandwidth else self.fidel_dim
+
   def num_hps(self):
-    n = 1 + (1 if self.fidel_use_same_bandwidth else self.fidel_dim)
+    n = 1 + self._num_fidel_hps()
     n += 1 if self.domain_use_same_bandwidth else self.domain_dim
     n += 1 if self.mean_func_type == 'tune' else 0
     n += 1 if self.noise_var_type == 'tune' else 0
@@ -190,30 +195,57 @@ class EuclideanMFHPLayout(EuclideanHPLayout):
   def bounds(self, X, Y, tune_nu=None):
     raise NotImplementedError('Use the bounds of the reference EuclideanMFGPFitter (fitter.cts_hp_bounds).')
 
+  @staticmethod
+  def _bandwidths(hp, n, same):
+    return [np.exp(hp.pop(0))] * n if same else [np.exp(hp.pop(0)) for _ in range(n)]
+
+  def _fidel_kernel(self, hp, nu):
+    """ Pops the fidelity kernel's hps from the front of `hp` (after the scale) and returns the kernel (scale 1). """
+    bws = self._bandwidths(hp, self.fidel_dim, self.fidel_use_same_bandwidth)
+    if self.fidel_kernel_type == 'se':
+      return SEKernel(self.fidel_dim, 1.0, bws)
+    return MaternKernel(self.fidel_dim, nu, 1.0, bws)
+
   def unpack(self, hp, Y, nu=None, groupings=None):
     """ gp_core.py:509-538 + euclidean_gp.py:680-709 """
     hp = list(np.asarray(hp, dtype=np.float64))
     Y = np.asarray(Y, dtype=np.float64)
     mean_const, noise_var = self._mean_and_noise(hp, Y)
     scale = np.exp(hp.pop(0))
-
-    def bandwidths(n, same):
-      return [np.exp(hp.pop(0))] * n if same else [np.exp(hp.pop(0)) for _ in range(n)]
-    f_bws = bandwidths(self.fidel_dim, self.fidel_use_same_bandwidth)
-    d_bws = bandwidths(self.domain_dim, self.domain_use_same_bandwidth)
-    assert len(hp) == 0
     f_tuned, d_tuned = self.tuned_nus()
     assert not (f_tuned and d_tuned), 'at most one tuned Matern nu on the device path'
-    f_nu = nu if f_tuned else self.fidel_nu
+    k_f = self._fidel_kernel(hp, nu if f_tuned else self.fidel_nu)
+    d_bws = self._bandwidths(hp, self.domain_dim, self.domain_use_same_bandwidth)
+    assert len(hp) == 0
     d_nu = nu if d_tuned else self.domain_nu
-    k_f = SEKernel(self.fidel_dim, 1.0, f_bws) if self.fidel_kernel_type == 'se' else \
-        MaternKernel(self.fidel_dim, f_nu, 1.0, f_bws)
     k_d = SEKernel(self.domain_dim, 1.0, d_bws) if self.domain_kernel_type == 'se' else \
         MaternKernel(self.domain_dim, d_nu, 1.0, d_bws)
     fidel_coords = list(range(self.fidel_dim))
     domain_coords = list(range(self.fidel_dim, self.fidel_dim + self.domain_dim))
     kern = CoordinateProductKernel(self.dim, scale, [k_f, k_d], [fidel_coords, domain_coords])
     return float(mean_const), float(noise_var), kern
+
+
+class EuclideanMFExpDecayHPLayout(EuclideanMFHPLayout):
+  """ EuclideanMFGPFitter with fidel_kernel_type 'expdecay' (the freeze-thaw fidelity kernel): the fidelity part of the
+      hp vector is [log offset, log power x fidel_dim] (_fidel_expdecay_kernel_setup, euclidean_gp.py:521-541), unpacked
+      into ExpDecayKernel(fidel_dim, 1.0, exp(offset), exp(powers)) (get_euclidean_integral_gp_kernel_with_scale,
+      :871-877); fidel_use_same_bandwidth plays no part, as in the reference.  The domain kernel is SE or Matern. """
+  FIDEL_KERNEL_TYPES = ('expdecay',)
+
+  def __init__(self, fidel_dim, domain_dim, domain_kernel_type='se', domain_nu=2.5, domain_use_same_bandwidth=False,
+               **kwargs):
+    super(EuclideanMFExpDecayHPLayout, self).__init__(fidel_dim, domain_dim, 'expdecay', domain_kernel_type,
+                                                      domain_nu=domain_nu,
+                                                      domain_use_same_bandwidth=domain_use_same_bandwidth, **kwargs)
+
+  def _num_fidel_hps(self):
+    return 1 + self.fidel_dim
+
+  def _fidel_kernel(self, hp, nu):
+    offset = np.exp(hp.pop(0))
+    powers = np.exp(np.array([hp.pop(0) for _ in range(self.fidel_dim)]))
+    return ExpDecayKernel(self.fidel_dim, 1.0, offset, powers)
 
 
 # One LML-only build at N = 5000 is a 40-step dependency chain (chol_diag -> panel -> next column) that leaves most
@@ -428,15 +460,19 @@ def layout_from_fitter(fitter):
                 noise_var_type=opt.noise_var_type, noise_var_label=getattr(opt, 'noise_var_label', 0.05),
                 noise_var_value=getattr(opt, 'noise_var_value', 0.1))
   if hasattr(fitter, 'fidel_dim') and hasattr(opt, 'fidel_kernel_type'):
-    # EuclideanMFGPFitter (euclidean_gp.py:418-716)
-    if (opt.fidel_kernel_type not in ('se', 'matern') or opt.domain_kernel_type not in ('se', 'matern') or
+    # EuclideanMFGPFitter (euclidean_gp.py:418-716); a 'poly' fidelity or domain kernel stays with the reference,
+    # whose fitter raises NotImplementedError for it (:515-519, 587-591, 619-621)
+    if (opt.fidel_kernel_type not in ('se', 'matern', 'expdecay') or opt.domain_kernel_type not in ('se', 'matern') or
         getattr(opt, 'domain_use_additive_gp', False)):
       return None
+    domain = dict(domain_nu=getattr(opt, 'domain_matern_nu', 2.5),
+                  domain_use_same_bandwidth=bool(getattr(opt, 'domain_use_same_bandwidth', False)), **common)
+    if opt.fidel_kernel_type == 'expdecay':
+      return EuclideanMFExpDecayHPLayout(fitter.fidel_dim, fitter.domain_dim, opt.domain_kernel_type, **domain)
     layout = EuclideanMFHPLayout(
         fitter.fidel_dim, fitter.domain_dim, opt.fidel_kernel_type, opt.domain_kernel_type,
-        fidel_nu=getattr(opt, 'fidel_matern_nu', 2.5), domain_nu=getattr(opt, 'domain_matern_nu', 2.5),
-        fidel_use_same_bandwidth=bool(getattr(opt, 'fidel_use_same_bandwidth', False)),
-        domain_use_same_bandwidth=bool(getattr(opt, 'domain_use_same_bandwidth', False)), **common)
+        fidel_nu=getattr(opt, 'fidel_matern_nu', 2.5),
+        fidel_use_same_bandwidth=bool(getattr(opt, 'fidel_use_same_bandwidth', False)), **domain)
     return None if sum(layout.tuned_nus()) > 1 else layout
   kernel_type = getattr(fitter, 'kernel_type', getattr(opt, 'kernel_type', None))
   additive = bool(getattr(opt, 'use_additive_gp', False))

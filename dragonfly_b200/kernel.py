@@ -1,14 +1,16 @@
 """
 Host-side mirror of dragonfly/gp/kernel.py for the kernels on the hot path: SEKernel, MaternKernel,
-AdditiveKernel, CoordinateProductKernel, ESPKernel (same constructor arguments, `hyperparams` dict, `dim`,
-`kernel_list` / `groupings` / `coordinate_list`, `is_guaranteed_psd`, `__call__`), plus the
+PolyKernel, ExpDecayKernel, AdditiveKernel, CoordinateProductKernel, ESPKernel (same constructor arguments,
+`hyperparams` dict, `dim`, `kernel_list` / `groupings` / `coordinate_list`, `is_guaranteed_psd`, `__call__`), plus the
 translation of such kernel objects -- these classes OR the reference's own, duck-typed by class name
 so that a patched Dragonfly install needs no changes -- into the POD `dfb_kernel_desc` that
 libdfb200's CUDA kernels evaluate (include/dfb200.h).
 
 `Kernel.__call__(X1, X2)` (kernel.py:72-83) runs on the GPU through dfb_kernel_matrix.  ESPKernel /
-ESPKernelSE / ESPKernelMatern (kernel.py:671-744) map to the descriptor's ESP form (esp_order > 0).  Kernel types
-outside the hot-path scope (Poly, ExpDecay, Hamming, NN kernels, an ESP kernel nested in another) raise
+ESPKernelSE / ESPKernelMatern (kernel.py:671-744) map to the descriptor's ESP form (esp_order > 0).  PolyKernel and
+ExpDecayKernel (kernel.py:331-433) map to the non-stationary factor kinds POLY and EXPDECAY; a descriptor with one of
+them carries kss = NaN, because k(x, x) depends on x.  Kernel types outside the hot-path scope (Hamming, NN kernels, an
+ESP kernel nested in another, Poly / ExpDecay as ESP children, a Poly kernel of non-integer order) raise
 NotImplementedError: there is no CPU fallback.
 """
 import math
@@ -156,6 +158,65 @@ class MaternKernel(Kernel):
         np.mean(self.hyperparams['dim_bandwidths']))
 
 
+class PolyKernel(Kernel):
+  """ kernel.py:331-392: scale * ((x * dim_scalings) . (y * dim_scalings) + 1) ** order. """
+
+  def __init__(self, dim, order, scale, dim_scalings=None):
+    super(PolyKernel, self).__init__()
+    self.dim = dim
+    self.set_poly_hyperparams(order, scale, dim_scalings)
+
+  def is_guaranteed_psd(self):
+    return True
+
+  def set_order(self, order):
+    self.add_hyperparams(order=order)
+
+  def set_scale(self, scale):
+    self.add_hyperparams(scale=scale)
+
+  def set_dim_scalings(self, dim_scalings):
+    if dim_scalings is not None:
+      if len(dim_scalings) != self.dim:
+        raise ValueError('Dimension of dim_scalings should be dim.')
+      dim_scalings = np.array(dim_scalings)
+    self.add_hyperparams(dim_scalings=dim_scalings)
+
+  def set_single_scaling(self, scaling):
+    self.set_dim_scalings(None if scaling is None else [scaling] * self.dim)
+
+  def set_poly_hyperparams(self, order, scale, dim_scalings):
+    self.set_order(order)
+    self.set_scale(scale)
+    if hasattr(dim_scalings, '__len__'):
+      self.set_dim_scalings(dim_scalings)
+    else:
+      self.set_single_scaling(dim_scalings)
+
+  def __str__(self):
+    return 'Poly: d=%d, scale=%0.2f, %s' % (self.hyperparams['order'], self.hyperparams['scale'],
+                                            ','.join(['%0.2f' % (e) for e in self.hyperparams['dim_scalings']]))
+
+
+class ExpDecayKernel(Kernel):
+  """ kernel.py:395-433: the freeze-thaw kernel of Swersky et al.,
+      scale * prod_i 1 / (1 + x_i + y_i) ** powers[i] + offset, on raw coordinates. """
+
+  def __init__(self, dim, scale=None, offset=None, powers=None):
+    super(ExpDecayKernel, self).__init__()
+    self.dim = dim
+    if not hasattr(powers, '__iter__'):
+      powers = [powers] * dim
+    self.set_hyperparams(scale=scale, offset=offset, powers=powers)
+
+  def is_guaranteed_psd(self):
+    return True
+
+  def __str__(self):
+    return 'ExpDec: sc=%0.3f, offset=%0.3f, pow=%s' % (self.hyperparams['scale'], self.hyperparams['offset'],
+                                                       str(list(self.hyperparams['powers'])))
+
+
 class AdditiveKernel(Kernel):
   """ kernel.py:461-500: scale * sum_g k_g(x[g], y[g]) over non-overlapping groups. """
 
@@ -268,12 +329,44 @@ class _Factor(object):
 def _kind_of(kern):
   """ Duck-typed dispatch on the class name so the reference's own kernel objects work too. """
   names = [c.__name__ for c in type(kern).__mro__]
-  for n in ('SEKernel', 'MaternKernel', 'AdditiveKernel', 'CoordinateProductKernel', 'ESPKernel'):
+  for n in ('SEKernel', 'MaternKernel', 'PolyKernel', 'ExpDecayKernel', 'AdditiveKernel', 'CoordinateProductKernel',
+            'ESPKernel'):
     if n in names:
       return n
   raise NotImplementedError(
-      'Kernel type %s is outside the GPU hot-path scope (supported: SEKernel, MaternKernel, '
+      'Kernel type %s is outside the GPU hot-path scope (supported: SEKernel, MaternKernel, PolyKernel, ExpDecayKernel, '
       'AdditiveKernel, CoordinateProductKernel, ESPKernel); there is no CPU fallback.' % (type(kern).__name__))
+
+
+def _nonstationary_factor(kern, kind, train_coords, cand_coords):
+  """ PolyKernel -> one POLY factor (p = order, slot values = dim_scalings); ExpDecayKernel -> one EXPDECAY factor
+      (s2 = offset, slot values = powers).  include/dfb200.h, "kernel descriptor". """
+  need = ('order', 'scale', 'dim_scalings') if kind == 'PolyKernel' else ('scale', 'offset', 'powers')
+  missing = [key for key in need if key not in getattr(kern, 'hyperparams', {})]
+  if missing:
+    # not the reference's object: a duck-typed class name without the hyper-parameters that define the kernel
+    raise NotImplementedError('%s object without hyper-parameter(s) %s has no device form; there is no CPU fallback.'
+                              % (kind, ', '.join(missing)))
+  f = _Factor()
+  f.train_coords = [int(c) for c in train_coords]
+  f.cand_coords = [int(c) for c in cand_coords]
+  f.s8, f.gamma_ratio, f.coeffs = 0.0, 0.0, []
+  f.scale = float(kern.hyperparams['scale'])
+  if kind == 'PolyKernel':
+    order = kern.hyperparams['order']
+    if float(order) != int(order) or int(order) < 0:
+      raise NotImplementedError('PolyKernel of order %s: only non-negative integer orders run on the device.' % (order,))
+    if kern.hyperparams['dim_scalings'] is None:
+      raise ValueError('PolyKernel needs dim_scalings.')
+    vals = np.asarray(kern.hyperparams['dim_scalings'], dtype=np.float64).reshape(-1)
+    f.kind, f.p, f.s2 = _lib.DFB_BASE_POLY, int(order), 0.0
+  else:
+    vals = np.asarray(kern.hyperparams['powers'], dtype=np.float64).reshape(-1)
+    f.kind, f.p, f.s2 = _lib.DFB_BASE_EXPDECAY, 0, float(kern.hyperparams['offset'])
+  if len(vals) != len(train_coords):
+    raise ValueError('%s has %d dim_scalings / powers for %d coordinates' % (kind, len(vals), len(train_coords)))
+  f.bandwidths = [float(v) for v in vals]
+  return f
 
 
 def _expand(kern, train_coords, cand_coords):
@@ -300,6 +393,10 @@ def _expand(kern, train_coords, cand_coords):
       # K = hyperparams['scale'] * norm_constant * unnorm: the first product is formed on the host
       f.scale = float(kern.hyperparams['scale'] * consts['norm_constant'])
     return 1.0, [(1.0, [f])]
+  if kind in ('PolyKernel', 'ExpDecayKernel'):
+    # one factor value each: ExpDecay's offset stays inside its factor, so a product multiplies ((scale k_F) k_D)
+    # in CoordinateProductKernel._child_evaluate's order (kernel.py:573-584)
+    return 1.0, [(1.0, [_nonstationary_factor(kern, kind, train_coords, cand_coords)])]
   if kind == 'ESPKernel':
     raise NotImplementedError('An ESP kernel inside an additive or product kernel is outside the GPU hot-path scope.')
   if kind == 'AdditiveKernel':
@@ -411,17 +508,24 @@ def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, 
         d.slot_cand_coord[si] = f.cand_coords[q]
         d.slot_bandwidth[si] = f.bandwidths[q]
         si += 1
-      prod = prod * _base_at_zero(f)
+      prod = prod * (_base_at_zero(f) if f.kind in (_lib.DFB_BASE_SE, _lib.DFB_BASE_MATERN) else np.nan)
       fi += 1
     total = total + prod
   d.term_first_factor[len(terms)] = fi
-  d.kss = float(post * total)
+  # NaN for a non-stationary kernel (a POLY or EXPDECAY factor): no k(x, x) holds for every x
+  d.kss = float(post * total) if is_stationary(d) else float('nan')
   if esp_order:
     # stationary: k(x, x) = scale * e_order(child values at distance 0)
     d.esp_order = esp_order
     d.kss = float(post * esp_combine([_base_at_zero(facs[0]) for _, facs in terms], esp_order))
   check_esp_descriptor(d)
   return d
+
+
+def is_stationary(d):
+  """ Whether k(x, x) is the same for every x: no factor of the descriptor is POLY or EXPDECAY (api.cu and common.cuh:
+      kernel_stationary). """
+  return all(d.factors[f].kind in (_lib.DFB_BASE_SE, _lib.DFB_BASE_MATERN) for f in range(d.n_factors))
 
 
 def check_esp_descriptor(d):

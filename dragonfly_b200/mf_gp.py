@@ -11,7 +11,7 @@ from .gp_core import GP
 
 
 class EuclideanGP(GP):
-  """ euclidean_gp.py:134-150: kernel may be an object or one of 'se' / 'matern' / 'esp'. """
+  """ euclidean_gp.py:134-150: kernel may be an object or one of 'se' / 'matern' / 'poly' / 'esp'. """
 
   def __init__(self, X, Y, kernel, mean_func, noise_var, kernel_hyperparams=None,
                build_posterior=True, reporter=None, **kwargs):
@@ -29,6 +29,9 @@ class EuclideanGP(GP):
       return gp_kernel.MaternKernel(kernel_hyperparams['dim'], kernel_hyperparams['nu'],
                                     kernel_hyperparams['scale'],
                                     kernel_hyperparams['dim_bandwidths'])
+    elif kernel_type in ['poly']:         # euclidean_gp.py:160-163
+      return gp_kernel.PolyKernel(kernel_hyperparams['dim'], kernel_hyperparams['order'],
+                                  kernel_hyperparams['scale'], kernel_hyperparams['dim_scalings'])
     elif kernel_type in ['esp']:          # euclidean_gp.py:168-171
       return gp_kernel.ESPKernelSE(kernel_hyperparams['dim'], kernel_hyperparams['scale'],
                                    kernel_hyperparams['order'], kernel_hyperparams['dim_bandwidths'])

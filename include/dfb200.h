@@ -69,23 +69,38 @@ extern "C" {
  *     e_0 = 1;  e_m = ((0 + (+e_{m-1}) p_1) + (-e_{m-2}) p_2 + ... ((-1)^(m-1) e_0) p_m) / m
  * Its values may be slightly negative where the exact value is ~0 (cancellation), |k| <= k(x, x).
  *   ESPKernelSE / ESPKernelMatern : T terms of one 1-D factor (scale 1), post_scale = outer scale
+ *
+ * Two non-stationary factor kinds (k(x, x) depends on x) reuse the same fields:
+ *     POLY      x~ = x[coords] * slot_bandwidth (a MULTIPLY: dim_scalings)             kernel.py:381-386
+ *               b = scale * (x~.y~ + 1)^p          p = order (>= 0)
+ *     EXPDECAY  z = x[coords] (raw), slot_bandwidth = the per-coordinate power p_q      kernel.py:415-426
+ *               b = ((scale * k_1) * k_2 ...) + s2,   k_q = 1 / (1 + (z_q + z'_q))^p_q,   s2 = offset
+ *   v^p follows NumPy's scalar-power fast paths: ^1 = v, ^2 = v * v, ^0.5 = sqrt(v), ^-1 = 1 / v, ^0 = 1,
+ *   else pow(v, p).  Both kinds are evaluated by the descriptor interpreter only (no specialised K_* kernel).
+ *   PolyKernel                   : 1 term, 1 factor (kernel_type 'poly')
+ *   ExpDecayKernel               : 1 factor; the MF fidelity kernel of a CoordinateProductKernel
+ * A descriptor is stationary when none of its factors is POLY or EXPDECAY; only then is kss meaningful.  The host
+ * writes kss = NaN for non-stationary descriptors, and the library never runs the int8 screen or the bound pass of
+ * dfb_score_argmax on them (their error model and variance floor rest on a constant k(x, x)).
  */
 #define DFB_MAX_FACTORS   48
 #define DFB_MAX_TERMS     48
 #define DFB_MAX_SLOTS     128
 #define DFB_MAX_MATERN_P  3
 
-#define DFB_BASE_SE      0
-#define DFB_BASE_MATERN  1
+#define DFB_BASE_SE        0
+#define DFB_BASE_MATERN    1
+#define DFB_BASE_POLY      2
+#define DFB_BASE_EXPDECAY  3
 
 typedef struct dfb_factor_desc {
-  int32_t kind;          /* DFB_BASE_SE | DFB_BASE_MATERN */
-  int32_t p;             /* Matern: nu = p + 1/2 (0 <= p <= DFB_MAX_MATERN_P) */
+  int32_t kind;          /* DFB_BASE_SE | DFB_BASE_MATERN | DFB_BASE_POLY | DFB_BASE_EXPDECAY */
+  int32_t p;             /* Matern: nu = p + 1/2 (0 <= p <= DFB_MAX_MATERN_P);  POLY: order;  EXPDECAY: 0 */
   int32_t n_dims;        /* number of slots of this factor */
   int32_t slot_off;      /* first slot */
-  double  scale;         /* SE: scale;  Matern: scale * norm_constant */
+  double  scale;         /* SE, POLY, EXPDECAY: scale;  Matern: scale * norm_constant */
   double  s8;            /* sqrt(8 nu) */
-  double  s2;            /* sqrt(2 nu) */
+  double  s2;            /* Matern: sqrt(2 nu);  EXPDECAY: offset */
   double  gamma_ratio;   /* Gamma(p+1) / Gamma(2p+1) */
   double  coeffs[DFB_MAX_MATERN_P + 1];  /* (p+i)! / (i! (p-i)!) */
 } dfb_factor_desc;
@@ -98,13 +113,13 @@ typedef struct dfb_kernel_desc {
   int32_t cand_dim;      /* columns of the candidate matrix */
   int32_t esp_order;     /* 0: sum of products; r > 0: ESP kernel of order r (see above) */
   double  post_scale;
-  double  kss;           /* k(x, x) for any x (all supported kernels are stationary) */
+  double  kss;           /* k(x, x) for any x if the kernel is stationary, else NaN (see above) */
   int32_t term_first_factor[DFB_MAX_TERMS + 1];
   double  term_pre_scale[DFB_MAX_TERMS];
   dfb_factor_desc factors[DFB_MAX_FACTORS];
   int32_t slot_train_coord[DFB_MAX_SLOTS];
   int32_t slot_cand_coord[DFB_MAX_SLOTS];
-  double  slot_bandwidth[DFB_MAX_SLOTS];
+  double  slot_bandwidth[DFB_MAX_SLOTS];   /* SE / Matern: bandwidth;  POLY: scaling;  EXPDECAY: power */
 } dfb_kernel_desc;
 
 /* ---- acquisition descriptor --------------------------------- dragonfly/opt/gpb_acquisitions.py */
@@ -198,11 +213,12 @@ int dfb_restore_posterior(dfb_handle* h);
  *   out_host[2]     'noise_mean' = sum(alpha)                                                  gp_core.py:234-235
  *   out_host[3]     'same_dim_bandwidths'
  *   out_host[4 + j] 'dim_bandwidths', param_num = j  (j < d)
- * n_out >= 4 + d.  Needs a full posterior (DFB_BUILD_FULL).  Returns -3 for composite and ESP kernels (the reference
- * raises NotImplementedError there, kernel.py:123-125).  Uses the K_* chunk buffer as scratch. */
+ * n_out >= 4 + d.  Needs a full posterior (DFB_BUILD_FULL).  Returns -3 for composite, ESP, POLY and EXPDECAY kernels (the
+ * reference raises NotImplementedError there, kernel.py:123-125).  Uses the K_* chunk buffer as scratch. */
 int dfb_lml_gradients(dfb_handle* h, double* out_host, int32_t n_out);
 
-/* max(diag K) of the last build -- the jitter ladder's scale (general_utils.py:183-189). */
+/* max(diag K) + noise_var of the current posterior -- the jitter ladder's scale (general_utils.py:183-189): kss + noise_var
+ * for a stationary kernel, else the largest diagonal entry actually built (kept current by dfb_extend_posterior). */
 int dfb_get_max_diag(dfb_handle* h, double* out_host);
 /* Copies of gp.L (n x n lower), gp.alpha (n), gp.K_trtr_wo_noise (n x n); any may be NULL.
  * Read directly by _add_ucb (gpb_acquisitions.py:169-171) and gp_core.py:203.  */
@@ -308,7 +324,8 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *                 on the pure fp64 DMMA path:
  *                 0 = fp64 DMMA everywhere (no reduced-precision arithmetic anywhere);
  *                 1 = int8-slice wgmma path everywhere, sigma vectors included (exact digit expansion of both fp64
- *                     operands, exact int32 accumulation; a-priori bound: query "i8_sigma2_bound");
+ *                     operands, exact int32 accumulation; a-priori bound: query "i8_sigma2_bound"), except for
+ *                     non-stationary kernels (POLY / EXPDECAY factors), which always score in fp64;
  *                 2 = auto: dfb_eval stays fp64; dfb_score_argmax screens with the int8 path, re-scores in fp64
  *                     every candidate whose int8 score -- widened by the error allowance that follows from the
  *                     bound -- could reach the fp64 maximum, returns the fp64 arg-max (index and score) of those,
