@@ -78,6 +78,7 @@ PROTOTYPES = {
   'dfb_get_state': (C.c_int, [_P, _P, _P, _P]),
   'dfb_set_alpha': (C.c_int, [_P, _P, _I64]),
   'dfb_eval': (C.c_int, [_P, _P, _I64, _I32, _I32, _D, _P, _P]),
+  'dfb_mu_upper_bound': (C.c_int, [_P, _P, _I64, _I32, _I32, _D, _P]),
   'dfb_eval_covar': (C.c_int, [_P, _P, _I64, _I32, _D, _P, _P]),
   'dfb_score_argmax': (C.c_int, [_P, C.POINTER(AcqDesc), _P, _I64, _I32, _I32, _D, _P,
                                  C.POINTER(_D), C.POINTER(_I64)]),
@@ -94,6 +95,7 @@ PROTOTYPES = {
   'dfb_launch_count': (_I64, [_P]),
   'dfb_debug_score_i8': (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _P, _D, _P, _P, _I64]),
   'dfb_debug_copy': (C.c_int, [_P, C.c_char_p, _P, _I64]),
+  'dfb_debug_approx_error': (C.c_int, [_P, _I32, C.POINTER(_D)]),
   'dfb_set_option': (C.c_int, [_P, C.c_char_p, _I64]),
   'dfb_query': (C.c_int, [_P, C.c_char_p, C.POINTER(_D)]),
   'dfb_profile_enable': (C.c_int, [_P, C.c_int]),

@@ -85,7 +85,9 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   int64_t* surv_idx = c.take<int64_t>((size_t)surv_cap);
   double* surv_X = c.take<double>((size_t)surv_cap * PRUNE_MAX_DC);
   int* surv_count = c.take<int>(4);
-  uint32_t* keep_words = c.take<uint32_t>((size_t)chunk / 32 + 1);
+  // one screen launch covers a host staging batch (up to chunk x DFB_MAX_SLOTS rows) or ~10^6 device rows
+  const int64_t keep_cap = round_up(chunk * DFB_MAX_SLOTS > ((int64_t)1 << 20) ? chunk * DFB_MAX_SLOTS : (int64_t)1 << 20, 32);
+  uint32_t* keep_words = c.take<uint32_t>((size_t)keep_cap / 32);
   double* best_score = c.take<double>(1);
   int64_t* best_index = c.take<int64_t>(1);
   double* red = c.take<double>(8);
@@ -104,7 +106,7 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
     h->Ks = Ks; h->Wi8 = Wi8; h->Ki8 = Ki8; h->rowscale = rowscale; h->rowinv = rowinv; h->list_idx = list_idx; h->list_X = list_X; h->list_count = list_count; h->list_s8 = list_s8; h->list_err = list_err; h->blk_lb = blk_lb; h->best_lb = best_lb; h->partial = partial; h->mu = mu; h->sd = sd; h->score = score; h->kssv = kssv; h->stage = stage;
     h->blk_score = blk_score; h->blk_index = blk_index; h->best_score = best_score;
     h->surv_cap = surv_cap; h->surv_idx = surv_idx; h->surv_X = surv_X; h->surv_count = surv_count;
-    h->keep_words = keep_words;
+    h->keep_words = keep_words; h->keep_cap = keep_cap;
     h->best_index = best_index; h->red = red; h->info = info;
     h->d_desc_tr = d0; h->d_desc_te = d1; h->d_desc_tmp = d2;
     h->n_max = n_max; h->npad_max = npad; h->chunk = chunk;
@@ -564,7 +566,7 @@ struct ChunkMode {
   bool allow_small;            // dfb_eval of <= SMALL_EVAL_M points: row-streaming kernel instead of the tile GEMM
   bool keep_scores;            // leave the scores of a single-chunk pass in h->score (self-check of the shortlist)
   bool keep_best;              // continue the running arg-max and best_lb of an earlier pass instead of resetting them
-  bool bound_pass;             // mu only + the upper-bound screen into the survivor list (dfb_score_argmax)
+  bool bound_pass;             // the upper-bound screen into the survivor list (dfb_score_argmax); with out.mu: mu_bar
 };
 static ChunkMode chunk_mode(bool want_std, bool do_argmax, bool use_i8, const int64_t* idx_map = nullptr) {
   ChunkMode md;
@@ -577,8 +579,9 @@ constexpr int64_t SMALL_EVAL_M = 32;      // up to four 8-wide passes over W's r
 // Per chunk two stages, back to back on the handle's stream:
 //   K: (host candidates: staging copy) K_* rows / digit planes + mu + k(x*,x*)      fp64 pipe
 //   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
-// The bound pass (md.bound_pass) replaces both by mu + k(x*,x*) alone and the screen that appends the candidates whose
-// acquisition bound reaches best_lb to the survivor list.
+// The bound pass (md.bound_pass) replaces both by one launch of the screen per staging batch (host candidates) or per
+// keep_cap rows (device candidates), which appends the candidates whose acquisition bound reaches best_lb to the
+// survivor list; with out.mu it writes mu_bar instead, chunk by chunk (dfb_mu_upper_bound).
 static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
                       int32_t space, double mean_const, ChunkOut out, const ChunkMode& md) {
   const bool want_std = md.want_std, do_argmax = md.do_argmax;
@@ -623,6 +626,9 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     DFB_CUDA_OK(cudaEventRecord(h->cp_fork, h->stream));  // the copy stream starts after everything already on the caller's stream
     DFB_CUDA_OK(cudaStreamWaitEvent(h->cp_stream, h->cp_fork, 0));
   }
+  // rows per step: a chunk, or for the screen a whole staging batch / keep_cap device rows
+  int64_t step = Mc;
+  if (md.bound_pass && out.mu == nullptr) step = space != DFB_HOST ? h->keep_cap : dbuf ? half_rows : stage_rows;
   auto issue_copy = [&](int64_t bi) -> int {               // batch bi -> half bi % 2, on the copy stream
     const int64_t lo = bi * half_rows;
     const int64_t hi = (m - lo < half_rows) ? m : lo + half_rows;
@@ -636,10 +642,9 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     if (!dbuf) return 0;
     const int64_t bi = c0 / half_rows;
     const int64_t b_hi = (m - bi * half_rows < half_rows) ? m : (bi + 1) * half_rows;
-    if (c0 + Mc >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
+    if (c0 + step >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
     return 0;
   };
-  const int64_t n_chunks = (m + Mc - 1) / Mc;
   const int* abort_count = md.collect ? h->list_count : nullptr;
   const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
                      (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
@@ -652,14 +657,10 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     ka.planes = h->Ki8; ka.plane_bytes = 2 * h->chunk * npad; ka.row_bytes = 2 * npad;
     ka.inv_colscale = 1.0 / i8_colscale(desc);
   }
-  const KstarWant want = md.bound_pass ? KstarWant::MU_SCREEN
-                         : !want_std   ? KstarWant::MU
-                         : i8          ? KstarWant::DIGITS
-                                       : KstarWant::ROWS;
+  const KstarWant want = !want_std ? KstarWant::MU : i8 ? KstarWant::DIGITS : KstarWant::ROWS;
 
-  for (int64_t ci = 0; ci < n_chunks; ci++) {
-    const int64_t c0 = ci * Mc;
-    const int64_t mc = (m - c0 < Mc) ? (m - c0) : Mc;
+  for (int64_t c0 = 0; c0 < m; c0 += step) {
+    const int64_t mc = (m - c0 < step) ? (m - c0) : step;
     const int64_t m_rows = round_up(mc, TILE);
     const double* xc_dev;
     if (space == DFB_HOST && dbuf) {
@@ -686,23 +687,21 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
                                                          : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
 
-    ka.Xc = xc_dev; ka.m = mc; ka.m_rows = m_rows; ka.mu = mu_dev;
-    const KstarRoute route = route_kstar(h, ka, want);
-
     if (md.bound_pass) {
-      // mu (bit-identical to the digit kernel's) and k(x*, x*); no K_* rows, no contraction.  Void once the seed's
-      // shortlist has overflowed, like every other launch of the int8 pass.
+      // mu_bar and the screen; no K_* rows, no contraction.  Void once the seed's shortlist has overflowed, like every
+      // other launch of the int8 pass.
       DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
-      if (route.producer != KstarProducer::SEG_MU) {
-        set_error("bound pass: the mu-only K_* kernel does not serve this kernel");
-        return -1;
-      }
-      DFB_TRY(launch_kstar(h, ka, route));
-      DFB_TRY(launch_prune(h, acq, h->mu, h->kssv, mc, md.pad, md.idx_base + c0, xc_dev, dc));
+      DFB_TRY(launch_prune(h, acq, desc, d_desc, ss.xs, xc_dev, mc, dc, mean_const, md.pad, md.idx_base + c0, abort_count,
+                           out.mu != nullptr ? mu_dev : nullptr));
       DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
+      if (space == DFB_HOST && out.mu)
+        DFB_CUDA_OK(cudaMemcpyAsync(out.mu + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
       DFB_TRY(release_half(c0));
       continue;
     }
+
+    ka.Xc = xc_dev; ka.m = mc; ka.m_rows = m_rows; ka.mu = mu_dev;
+    const KstarRoute route = route_kstar(h, ka, want);
 
     // K stage
     DFB_TRY(prof_begin(h, DFB_PROF_KSTAR));
@@ -1116,12 +1115,47 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
   return 0;
 }
 
+int dfb_mu_upper_bound(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t space, double mean_const,
+                       double* mu_ub_out) {
+  DFB_TRY(need(h, true, true, true, true, false));
+  if (m < 0 || (m > 0 && (Xc == nullptr || mu_ub_out == nullptr))) { set_error("bad mu_upper_bound arguments"); return -1; }
+  if (h->have_test_kernel || !kstar_plain(h->desc_tr)) {
+    set_error("dfb_mu_upper_bound: the bound pass serves plain SE / Matern kernels on <= 8 dims without a test kernel");
+    return -1;
+  }
+  if (m == 0) return 0;
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  dfb_acq_desc acq;
+  memset(&acq, 0, sizeof(acq));
+  ChunkOut out = {mu_ub_out, nullptr, nullptr};
+  ChunkMode md = chunk_mode(false, false, false);
+  md.bound_pass = true;
+  DFB_TRY(run_chunks(h, acq, Xc, m, dc, space, mean_const, out, md));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if ((which != 0 && which != 1) || out_host == nullptr) { set_error("bad approx_error arguments"); return -1; }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  unsigned long long* bits = reinterpret_cast<unsigned long long*>(h->red);
+  DFB_TRY(launch_approx_err(h, which, bits));
+  unsigned long long v = 0;
+  DFB_CUDA_OK(cudaMemcpyAsync(&v, bits, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  memcpy(out_host, &v, sizeof(double));
+  return 0;
+}
+
 // ---- bound pass of dfb_score_argmax ---------------------------------------------------------------------------------
-// Most candidates of a large random batch cannot reach the arg-max, and proving so needs mu alone:
-//   (1) ub = acq(mu, sqrt(k**)) >= the fp64 score of the exact pass.  EI (d/d sigma = phi(z) > 0), UCB with beta >= 0
-//       and PI for mu < the incumbent (z < 0) are non-decreasing in sigma, and the device's fp64 variance
-//       fl(k** - sum of partials) with every partial >= 0 is at most k** in floating point as well.  The ulp-level
-//       non-monotonicity of the ndtr / erfc formulas is dwarfed by the shortlist's pad (1e-9 of the score scale).
+// Most candidates of a large random batch cannot reach the arg-max, and proving so needs an upper bound of mu alone:
+//   (1) ub = acq(mu_bar, sqrt(k**)) >= the fp64 score of the exact pass.  mu_bar (kernels.cu: prune_bound_kernel, in
+//       single precision) is at least the fp64 mu of every K_* producer.  EI and UCB with beta >= 0 are
+//       non-decreasing in mu and in sigma, PI is non-decreasing in mu and, for mu_bar < the incumbent (z < 0), in
+//       sigma; the device's fp64 variance fl(k** - sum of partials) with every partial >= 0 is at most k** in floating
+//       point as well.  The ulp-level non-monotonicity of the ndtr / erfc formulas is dwarfed by the shortlist's pad
+//       (1e-9 of the score scale).
 //   (2) best_lb <= the final fp64 maximum (argmax_merge_kernel: a maximum of certain lower bounds).
 // So a candidate with ub < best_lb - pad has an fp64 score below the maximum: every candidate whose fp64 score equals
 // the maximum, ties included, survives, the shortlist of the passes that follow contains all of them, and the fp64
@@ -1129,16 +1163,14 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
 // (3) No dropped candidate can be a NaN winner (a negative fp64 variance gives a NaN score, and np.argmax takes the
 //     first NaN): see bound_pass_applies.
 // Order: (a) chunk 0 scored as today (collect mode) seeds best, best_lb and the shortlist; (b) the bound pass over
-// chunks 1.. fills the survivor list; (c) one read-back of the survivor count; (d) the survivors are scored like any
+// rows chunk.. (one screen + gather per launch of run_chunks' bound-pass step) fills the survivor list; (c) one
+// read-back of the survivor count; (d) the survivors are scored like any
 // other chunk (collect mode, indices mapped back), continuing the arg-max of (a); the caller then re-scores the
 // shortlist in fp64 and runs the self-check unchanged.  A survivor list that overflows (4 chunks) voids the screen:
 // chunks 1.. are then scored as today, still continuing the seed's state.
 static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, int64_t m,
                                int32_t dc, double b2) {
-  if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC || !kernel_stationary(desc)) return false;
-  KstarArgs ka{};                     // run_chunks' digit route of a full chunk: the bound pass's mu must be SEG_DIGITS'
-  ka.desc = &desc; ka.npad_tr = ka.n_write = h->npad; ka.m_rows = h->chunk;
-  if (route_kstar(h, ka, KstarWant::DIGITS).producer != KstarProducer::SEG_DIGITS) return false;
+  if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC || !kstar_plain(desc)) return false;
   if (!(acq.kind == DFB_ACQ_EI || acq.kind == DFB_ACQ_PI || (acq.kind == DFB_ACQ_UCB && acq.beta >= 0.0))) return false;
   // Variance floor.  K: the noiseless training kernel matrix, s: the diagonal actually added (noise + jitter, for every
   // point, hallucinated ones included), k = K(X, x*).  The joint covariance [[K, k], [k^T, k**]] is PSD, so

@@ -149,7 +149,8 @@ struct dfb_handle {
   int64_t* surv_idx = nullptr;    // surv_cap global indices
   double* surv_X = nullptr;       // surv_cap x PRUNE_MAX_DC candidate rows
   int* surv_count = nullptr;      // [0] survivors wanted (> surv_cap = overflow)
-  uint32_t* keep_words = nullptr; // chunk / 32 ballot words of one chunk
+  uint32_t* keep_words = nullptr; // keep_cap / 32 ballot words of one screen launch
+  int64_t keep_cap = 0;           // rows one screen launch may cover
   int64_t last_survivors = 0, last_pruned = 0;
   int64_t last_selfcheck_violations = 0;
   double last_selfcheck_ratio = 0.0;   // max |s_int8 - s_fp64| / E_i over the last shortlist

@@ -27,8 +27,10 @@ enum class KstarWant {
   ROWS,           // fp64 rows (+ mu, k(x*, x*) when asked)
   DIGITS,         // int8 digit planes + mu + k(x*, x*)
   MU,             // mu alone, as ROWS computes it (mean-only dfb_eval)
-  MU_SCREEN,      // mu + k(x*, x*) alone, as SEG_DIGITS computes them (bound pass of dfb_score_argmax)
 };
+// "plain" of the route table: one term, one SE or Matern (p <= 2) factor on slots 0 .. d-1, d <= 8, no ESP -- the
+// kernels specialised on (kind, p, d)
+bool kstar_plain(const dfb_kernel_desc& desc);
 enum class KstarProducer { SEG_DIGITS, SEG_ROWS64, SEG_MU, FAST_DIGITS, FAST_ROWS, ESP_DIGITS, ESP_ROWS, INTERP_ROWS };
 struct KstarRoute {
   KstarProducer producer;
@@ -64,10 +66,16 @@ int launch_acq(dfb_handle* h, const dfb_acq_desc& acq, const double* mu, const d
 int launch_collect_shortlist(dfb_handle* h, const double* score, const double* sd, int64_t mc,
                              int64_t idx_base, const int64_t* idx_map, const I8ErrModel& em, double pad, const double* Xc,
                              int dc);
-// bound pass of dfb_score_argmax: keeps the candidates of a chunk whose acquisition at sigma = sqrt(k**) reaches
-// *best_lb - pad and appends them (x rows, global index idx_base + row) to the survivor list in row order
-int launch_prune(dfb_handle* h, const dfb_acq_desc& acq, const double* mu, const double* kss, int64_t mc, double pad,
-                 int64_t idx_base, const double* Xc, int dc);
+// bound pass of dfb_score_argmax (plain kernels): keeps the m candidates Xc (device) whose acquisition at
+// (mu_bar, sqrt(k**)) reaches *best_lb - pad, mu_bar a certified upper bound of mu, and appends them (x rows, global
+// index idx_base + row) to the survivor list in row order; m <= h->keep_cap.  mu_ub non-NULL: writes mu_bar instead
+// (no screen).  No-op once *abort_count > SHORTLIST_CAP (abort_count may be NULL).
+int launch_prune(dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, const dfb_kernel_desc* d_desc,
+                 const double* xsT, const double* Xc, int64_t m, int dc, double mean_const, double pad, int64_t idx_base,
+                 const int* abort_count, double* mu_ub);
+// largest relative error of ex2.approx.ftz.f32 (which = 0) or rsqrt.approx.ftz.f32 (1) over the inputs the bound pass
+// gives them, as the bit pattern of a double in *out_bits (device)
+int launch_approx_err(dfb_handle* h, int which, unsigned long long* out_bits);
 int launch_selfcheck(dfb_handle* h, const double* s64, int count);
 int launch_vec_max(dfb_handle* h, const double* v, int64_t n, double* out);
 int launch_reset_best(dfb_handle* h);

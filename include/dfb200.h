@@ -234,6 +234,13 @@ int dfb_set_alpha(dfb_handle* h, const double* alpha_dev, int64_t n);
  * Never materialises the M x M covariance.  sd may be NULL (uncert_form 'none').  */
 int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t space,
              double mean_const, double* mu, double* sd);
+/* A certified upper bound mu_ub >= the mu of GP.eval(X_test, 'none') (gp_core.py:165-190, mean) -- at least the fp64
+ * mu of dfb_eval by any of its K_* producers -- computed in single precision by the screen of dfb_score_argmax's bound
+ * pass (option "prune").  +inf where the bound's analysis does not hold (coordinates beyond 2^60 after scaling), NaN
+ * for rows with NaN.  Plain SE / Matern (p <= 2) kernels on <= 8 dims, no test kernel.  mu_ub_out in the space of
+ * Xc.  */
+int dfb_mu_upper_bound(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t space, double mean_const,
+                       double* mu_ub_out);
 /* Optional second workspace for the block-exact joint posterior (covariance / Thompson sampling)
  * of up to `mb` candidates at a time (mb <= the scoring chunk).  */
 size_t dfb_ts_workspace_bytes(int64_t n_max, int64_t mb);
@@ -315,6 +322,10 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
  * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk).
  * Synchronises. */
 int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
+/* Diagnostics (tests/test_gpu_prune_f32.py): the largest relative error of ex2.approx.ftz.f32 (which = 0) over every
+ * float in [-126, 0], or of rsqrt.approx.ftz.f32 (which = 1) over every float in [2^-120, 2^126), against fp64
+ * references -- the inputs the bound pass of dfb_score_argmax gives them.  Synchronises. */
+int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host);
 
 /* Tuning switches.
  *  "gemm_impl"  : 0 = cp.async-ring DMMA kernel, 1 = TMA + mbarrier warp-specialised DMMA kernel for the
@@ -356,11 +367,12 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  *                 tiles that share one load of the W digits, so an odd group is rounded up by one tile; query
  *                 "last_c2_group" gives the group in effect.
  *  "prune"      : 1 (default) = dfb_score_argmax's int8 path contracts only the candidates whose acquisition can reach
- *                 the arg-max.  After chunk 0 is scored, every further candidate gets mu alone and is dropped when
- *                 acq(mu, sqrt(k(x*, x*))) -- an upper bound of its score, sigma^2 <= k(x*, x*) -- lies below a certain
- *                 lower bound of the fp64 maximum; the survivors are scored as usual.  Index and score are those of the
- *                 full pass, bit for bit.  Applies to EI, PI and UCB with beta >= 0, plain SE / Matern kernels on <= 8
- *                 dims, radix-256 digits, no test kernel, m > chunk, no score vector, and when the posterior's variance
+ *                 the arg-max.  After chunk 0 is scored, every further candidate gets a certified upper bound mu_ub of
+ *                 its mean (single precision, dfb_mu_upper_bound) and is dropped when acq(mu_ub, sqrt(k(x*, x*))) -- an
+ *                 upper bound of its score, sigma^2 <= k(x*, x*) -- lies below a certain lower bound of the fp64
+ *                 maximum; the survivors are scored as usual.  Index and score are those of the full pass, bit for
+ *                 bit.  Applies to EI, PI and UCB with beta >= 0, plain SE / Matern (p <= 2) kernels on <= 8 dims, no
+ *                 test kernel, m > chunk, no score vector, and when the posterior's variance
  *                 floor k** s / (n k** + s) (s = noise + jitter) exceeds the int8 error bound.  0 = contract every
  *                 candidate.
  *  "kstar_fast" : 1 (default) = plain SE / Matern kernels on <= 8 dims get specialised K_* kernels; 0 = they go through
@@ -377,7 +389,7 @@ int dfb_query(dfb_handle* h, const char* name, double* out);
 
 /* Per-kernel-class device timing with CUDA events on the handle's stream (bench.py's roofline):
  * class 0 = K_* build (+mu), 1 = the DMMA contraction |L^-1 k_*|^2, 2 = acquisition + arg-max,
- * 3 = posterior build (whole dfb_build_posterior), 4 = the bound pass of dfb_score_argmax (mu + upper-bound screen,
+ * 3 = posterior build (whole dfb_build_posterior), 4 = the bound pass of dfb_score_argmax (upper bound of mu + screen,
  * option "prune").  dfb_profile_read synchronises, returns the accumulated milliseconds, launches and work units
  * (candidates for 0-2 and 4, builds for 3) and resets.  Class 1 counts only the candidates actually contracted. */
 #define DFB_PROF_KSTAR 0

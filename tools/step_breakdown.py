@@ -1,7 +1,7 @@
 """Wall-clock / device-time breakdown of one bench.py step (build + fused score of 10^6 candidates).
 
 The device line splits the score into the contracted chunks (kstar, gemm, acq: the seed chunk and the survivors of
-the bound pass) and the bound pass itself (mu + upper-bound screen of every other candidate)."""
+the bound pass) and the bound pass itself (a certified upper bound of mu and the screen, for every other candidate)."""
 import os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -27,7 +27,7 @@ for prof in (False, False, False, True):
   if prof:
     r = [gp._post.profile_read(c) for c in (0, 1, 2, 4)]
     # kstar / gemm / acq: the chunks that were contracted (the seed chunk and the survivors of the bound pass);
-    # bound: the mu-only pass + upper-bound screen over every other candidate
+    # bound: the upper bound of mu + screen over every other candidate
     line += ' | device: kstar %.2f (%d) gemm %.2f (%d, %d cand) acq %.2f (%d) bound %.2f (%d) sum %.2f' % (
         r[0][0], r[0][1], r[1][0], r[1][1], r[1][2], r[2][0], r[2][1], r[3][0], r[3][1], sum(x[0] for x in r))
     line += ' | shortlist %d survivors %d pruned %d' % (int(gp._post.query('last_shortlist')),
