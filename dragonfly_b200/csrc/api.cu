@@ -4,6 +4,8 @@
 #include <new>
 #include <stdlib.h>
 #include <float.h>
+#include <algorithm>
+#include <vector>
 #include "kernels.cuh"
 #include "gemm_tma.h"
 
@@ -945,6 +947,81 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   if (lml_out_host != nullptr) {
     const double quad = (flags == DFB_BUILD_FULL) ? red[1] : red[2];
     *lml_out_host = -0.5 * quad - red[0] - 0.5 * (double)n * log(2.0 * M_PI);
+  }
+  return 0;
+}
+
+int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
+                  int32_t B, double* lml_out, int32_t* info_out) {
+  DFB_TRY(need(h, true, false, true, false, false));
+  if (B < 0 || (B > 0 && (descs == nullptr || noise_var == nullptr || mean_const == nullptr || lml_out == nullptr ||
+                          info_out == nullptr))) {
+    set_error("lml_batch: bad arguments");
+    return -1;
+  }
+  if (h->npad > LML_BATCH_MAX_NPAD) {
+    set_error("lml_batch: n = %lld above the batch kernel's %d", (long long)h->n, LML_BATCH_MAX_NPAD);
+    return -1;
+  }
+  int ns_max = 1, nf_max = 1;
+  for (int b = 0; b < B; b++) {
+    DFB_TRY(check_desc(&descs[b]));
+    if (descs[b].esp_order != 0) { set_error("lml_batch: item %d is an ESP kernel", b); return -1; }
+    if (descs[b].train_dim != h->d) {
+      set_error("lml_batch: item %d has train_dim %d != data dim %d", b, descs[b].train_dim, h->d);
+      return -1;
+    }
+    ns_max = std::max(ns_max, (int)descs[b].n_slots);
+    nf_max = std::max(nf_max, (int)descs[b].n_factors);
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  // The K_* chunk buffer is idle outside scoring: it holds the items' parameters, results and factorisation scratch.
+  // A batch larger than it holds runs as consecutive launches of what fits.
+  const int64_t npad = h->npad;
+  const int64_t item = lml_batch_item_doubles(npad, ns_max, nf_max);
+  const size_t per_item_bytes = sizeof(dfb_kernel_desc) + 4 * sizeof(double) + sizeof(int) + item * sizeof(double);
+  const size_t ks_bytes = (size_t)h->chunk * h->npad_max * sizeof(double);
+  const int64_t cap = std::min<int64_t>((int64_t)((ks_bytes - 4096) / per_item_bytes), 65535);
+  if (cap < 1) { set_error("lml_batch: workspace too small for one item"); return -1; }
+  std::vector<char> up, down;
+  for (int b0 = 0; b0 < B; b0 += (int)cap) {
+    const int nb_items = (int)std::min<int64_t>(cap, B - b0);
+    Carver c(reinterpret_cast<char*>(h->Ks));
+    dfb_kernel_desc* d_descs = c.take<dfb_kernel_desc>(nb_items);
+    double* d_noise = c.take<double>(nb_items);
+    double* d_mean = c.take<double>(nb_items);
+    const size_t up_bytes = c.off;
+    double* d_red = c.take<double>(2 * (size_t)nb_items);
+    const size_t down_off = (reinterpret_cast<char*>(d_red) - reinterpret_cast<char*>(h->Ks));
+    int* d_info = c.take<int>(nb_items);
+    const size_t down_bytes = c.off - down_off;
+    double* scratch = c.take<double>((size_t)item * nb_items);
+    up.assign(up_bytes, 0);
+    memcpy(up.data() + (reinterpret_cast<char*>(d_descs) - reinterpret_cast<char*>(h->Ks)), descs + b0,
+           sizeof(dfb_kernel_desc) * nb_items);
+    memcpy(up.data() + (reinterpret_cast<char*>(d_noise) - reinterpret_cast<char*>(h->Ks)), noise_var + b0,
+           sizeof(double) * nb_items);
+    memcpy(up.data() + (reinterpret_cast<char*>(d_mean) - reinterpret_cast<char*>(h->Ks)), mean_const + b0,
+           sizeof(double) * nb_items);
+    DFB_CUDA_OK(cudaMemcpyAsync(h->Ks, up.data(), up_bytes, cudaMemcpyHostToDevice, h->stream));
+    LmlBatchArgs g;
+    g.descs = d_descs; g.noise = d_noise; g.mean = d_mean;
+    g.X = h->X; g.y = h->yc; g.n = h->n; g.d = h->d; g.npad = npad;
+    g.ns_max = ns_max; g.nf_max = nf_max;
+    g.scratch = scratch; g.item_doubles = item;
+    g.red = d_red; g.info = d_info;
+    DFB_TRY(launch_lml_batch(h, g, nb_items));
+    down.resize(down_bytes);
+    DFB_CUDA_OK(cudaMemcpyAsync(down.data(), d_red, down_bytes, cudaMemcpyDeviceToHost, h->stream));
+    DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+    const double* red = reinterpret_cast<const double*>(down.data());
+    const int* info = reinterpret_cast<const int*>(down.data() + (reinterpret_cast<char*>(d_info) -
+                                                                   reinterpret_cast<char*>(d_red)));
+    for (int b = 0; b < nb_items; b++) {
+      info_out[b0 + b] = info[b];
+      // dfb_build_posterior's LML-only formula
+      lml_out[b0 + b] = info[b] != 0 ? NAN : -0.5 * red[2 * b + 1] - red[2 * b] - 0.5 * (double)h->n * log(2.0 * M_PI);
+    }
   }
   return 0;
 }

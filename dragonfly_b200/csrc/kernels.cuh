@@ -100,4 +100,17 @@ int launch_lml_grad_tiles(dfb_handle* h, const dfb_kernel_desc* d_desc, const do
 int launch_lml_grad_reduce(dfb_handle* h, const double* partial, int64_t n_tiles, int pstride, int n_out,
                            const double* alpha, int64_t n, double* out);
 
+// dfb_lml_batch: B LML-only builds on the handle's training set, one CTA per item (kernels.cu, lml_batch_kernel)
+constexpr int LML_BATCH_MAX_NPAD = 4 * TILE;
+struct LmlBatchArgs {
+  const dfb_kernel_desc* descs; const double* noise; const double* mean;    // B of each (device)
+  const double* X; const double* y; int64_t n; int d; int64_t npad;         // training set; y = Y (uncentred), padded
+  int ns_max, nf_max;                 // largest n_slots / n_factors in the batch: the staged coordinates per item
+  double* scratch; int64_t item_doubles;
+  double* red;                        // [B][2]: sum log L_ii, |L^-1 y_c|^2
+  int* info;                          // [B]: 0, or 1 + the index of the first non-positive pivot
+};
+int64_t lml_batch_item_doubles(int64_t npad, int ns, int nf);
+int launch_lml_batch(dfb_handle* h, const LmlBatchArgs& g, int B);
+
 }  // namespace dfb

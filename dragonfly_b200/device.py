@@ -132,6 +132,22 @@ class DevicePosterior(object):
     self.lml = lml.value if info == 0 else None
     return info, self.lml
 
+  def lml_batch(self, descs, noise_vars, mean_consts):
+    """ dfb_lml_batch on the training set of set_train (pass the raw Y, mean 0): one LML-only build per item, all in one
+        launch.  Returns (lmls, infos); an item with info > 0 is not positive definite and its lml is NaN. """
+    B = len(descs)
+    arr = (_lib.KernelDesc * B)(*descs)
+    noise = np.ascontiguousarray(noise_vars, dtype=np.float64)
+    mean = np.ascontiguousarray(mean_consts, dtype=np.float64)
+    assert len(noise) == B and len(mean) == B
+    lmls = np.empty(B)
+    infos = np.empty(B, dtype=np.int32)
+    _lib.check(self.lib.dfb_lml_batch(self.h, arr, noise.ctypes.data_as(C.POINTER(C.c_double)),
+                                      mean.ctypes.data_as(C.POINTER(C.c_double)), B,
+                                      lmls.ctypes.data_as(C.POINTER(C.c_double)),
+                                      infos.ctypes.data_as(C.POINTER(C.c_int32))), 'dfb_lml_batch')
+    return lmls, infos
+
   def capacity(self):
     """ Training points this posterior can hold without a rebuild: its padded size (a multiple of 128). """
     return (self.n + 127) // 128 * 128

@@ -319,6 +319,46 @@ def lml_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=None, lan
   return lmls, post
 
 
+# Largest training set dfb_lml_batch serves (DESIGN.md 4.3, 10): one CTA factorises a whole item, so its time grows
+# as N^3 on one SM while lml_for_hyperparams spreads each build over the GPU.
+LML_BATCH_MAX_N = 512
+
+
+def lml_batch_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=None):
+  """ What lml_for_hyperparams returns, with every LML of a plain (not ESP, not additive) layout on N <= LML_BATCH_MAX_N
+      points from ONE dfb_lml_batch call.  Items that are not positive definite are rebuilt one at a time through
+      stable_cholesky_on_device (its jitter ladder), as lml_for_hyperparams builds them.  Returns (lmls, post). """
+  from .device import DevicePosterior
+  X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
+  Y = np.asarray(Y, dtype=np.float64)
+  if (len(X) > LML_BATCH_MAX_N or getattr(layout, 'kernel_type', None) == 'esp' or
+      getattr(layout, 'use_additive_gp', False)):
+    return lml_for_hyperparams(X, Y, hps, layout, nus=nus, post=post, device=device)
+  if post is None or post.n_max < len(X):
+    post = DevicePosterior(len(X), device=device)
+  key = (X.shape, X.tobytes(), Y.tobytes())
+  if getattr(post, '_lml_batch_train', None) != key:
+    post.set_train(X, Y)                          # raw Y: the kernel forms Y - mean_const per item
+    post._lml_batch_train = key
+  descs, noise, means = [], [], []
+  for i, hp in enumerate(hps):
+    mean_const, noise_var, kern = layout.unpack(hp, Y, None if nus is None else nus[i])
+    descs.append(build_descriptor(kern, train_dim=X.shape[1], cand_dim=X.shape[1]))
+    noise.append(noise_var)
+    means.append(mean_const)
+  if not descs:
+    return np.empty(0), post
+  lmls, infos = post.lml_batch(descs, noise, means)
+  bad = np.nonzero(infos != 0)[0]
+  for i in bad:
+    post.set_train(X, Y - means[i])
+    post.set_kernel(descs[i])
+    lmls[i], _ = stable_cholesky_on_device(post, noise[i], flags=_lib.DFB_BUILD_LML_ONLY)
+  if len(bad):
+    post._lml_batch_train = None
+  return lmls, post
+
+
 def default_max_evals(method, num_hps):
   """ gp_core.py:456-462 """
   if method in ('direct', 'pdoo'):
@@ -495,26 +535,48 @@ def layout_from_fitter(fitter):
       num_groups_per_group_size=getattr(opt, 'num_groups_per_group_size', -1))
 
 
+def post_sampling_covers(layout):
+  """ The layouts whose 'post_sampling' fits run on the device (post_sampling.post_sample_hps): SE / Matern, not
+      additive; the MF product of SE / Matern fidelity and domain kernels.  ESP and ExpDecay stay with the reference. """
+  if type(layout) is EuclideanHPLayout:
+    return layout.kernel_type in ('se', 'matern') and not layout.use_additive_gp
+  return type(layout) is EuclideanMFHPLayout
+
+
+def _fitter_data(fitter, layout):
+  """ The rows the fitter's GPs are built on: [z || x] for an MF fitter. """
+  if isinstance(layout, EuclideanMFHPLayout):
+    X_mat = np.concatenate((np.asarray(fitter.ZZ, dtype=np.float64).reshape(len(fitter.YY), -1),
+                            np.asarray(fitter.XX, dtype=np.float64).reshape(len(fitter.YY), -1)), axis=1)
+    return X_mat, np.array(fitter.YY)
+  return np.array(fitter.X), np.array(fitter.Y)
+
+
 def fit_gp_on_fitter(fitter, reference_fit_gp, num_samples=1, hp_tune_criterion=None):
   """ GPFitter.fit_gp (gp_core.py:783-821) for a reference EuclideanGPFitter instance: hp_tune_criterion 'ml' with
       ml_hp_tune_opt rand / rand_exp_sampling / pdoo / direct-without-Fortran runs fit_gp above (every batch of
       _tuning_objective evaluations as one lml_for_hyperparams call; same global-RNG consumption, same selection,
-      the final GP built by the fitter's own build_gp); everything else is handed to `reference_fit_gp`. """
+      the final GP built by the fitter's own build_gp); 'post_sampling' with the slice sampler on a layout that
+      post_sampling_covers runs post_sampling.post_sample_hps; everything else is handed to `reference_fit_gp`. """
   from argparse import Namespace
   from .gpb_acquisitions import _reference_fortran_direct_available
   crit = fitter.options.hp_tune_criterion if hp_tune_criterion is None else hp_tune_criterion
   method = getattr(fitter, 'ml_hp_tune_opt_method', None)
+  if crit == 'post_sampling':
+    layout = layout_from_fitter(fitter)
+    if getattr(fitter.options, 'post_hp_tune_method', None) != 'slice' or not post_sampling_covers(layout):
+      return reference_fit_gp(fitter, num_samples, hp_tune_criterion)
+    from .post_sampling import post_sample_hps
+    X_mat, Y_vec = _fitter_data(fitter, layout)
+    return post_sample_hps(X_mat, Y_vec, layout, fitter.cts_hp_bounds, fitter.dscr_hp_vals, num_samples=num_samples,
+                           offset=fitter.options.post_hp_tune_offset, burn=fitter.options.post_hp_tune_burn,
+                           build_gp=lambda cts, dscr: fitter.build_gp(cts, dscr, other_gp_params=None))
   layout = layout_from_fitter(fitter) if crit == 'ml' else None
   if (layout is None or method not in ('rand', 'rand_exp_sampling', 'pdoo', 'direct') or
       (method == 'direct' and _reference_fortran_direct_available())):
     return reference_fit_gp(fitter, num_samples, hp_tune_criterion)
   other = lambda grp: None if grp is None else Namespace(add_gp_groupings=grp)
-  if isinstance(layout, EuclideanMFHPLayout):
-    X_mat = np.concatenate((np.asarray(fitter.ZZ, dtype=np.float64).reshape(len(fitter.YY), -1),
-                            np.asarray(fitter.XX, dtype=np.float64).reshape(len(fitter.YY), -1)), axis=1)
-    Y_vec = np.array(fitter.YY)
-  else:
-    X_mat, Y_vec = np.array(fitter.X), np.array(fitter.Y)
+  X_mat, Y_vec = _fitter_data(fitter, layout)
   return fit_gp(X_mat, Y_vec, layout, fitter.cts_hp_bounds, fitter.dscr_hp_vals,
                 method=method, max_evals=fitter.hp_tune_max_evals,
                 build_gp=lambda cts, dscr, grp: fitter.build_gp(cts, dscr, other_gp_params=other(grp)))

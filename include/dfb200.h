@@ -189,6 +189,14 @@ int dfb_set_train(dfb_handle* h, const double* X_dev, int64_t n, int32_t d,
  * positive definite (np.linalg.LinAlgError in stable_cholesky, general_utils.py:176-192).  */
 int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t flags,
                         double* lml_out_host);
+/* The LML of B hyper-parameter settings on the training set of dfb_set_train -- B x GPFitter._tuning_objective
+ * (gp_core.py:565-574) in one launch, one CTA per item.  Pass the raw Y to dfb_set_train (mean 0): item b uses the
+ * kernel descs[b] (esp_order == 0), noise_var[b] and y_c = Y - mean_const[b].  n <= 512.  lml_out[b] and info_out[b]
+ * are what dfb_build_posterior(descs[b], noise_var[b], 0, DFB_BUILD_LML_ONLY) returns on the same data, bit for bit:
+ * info_out[b] = 1 + index of the first non-positive pivot (lml_out[b] = NaN) or 0.  Does not touch the posterior.  One
+ * host copy in, one launch, one copy out per batch that fits the scoring chunk buffer; larger B runs as several. */
+int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
+                  int32_t B, double* lml_out, int32_t* info_out);
 /* GP.add_data_multiple (gp_core.py:139-146) and the (N + q)-point factorisation of
  * eval_with_hallucinated_observations (gp_core.py:200-206) WITHOUT the reference's full rebuild: appends q
  * training points (X_new: q x d, y_centred_new: q) to a built posterior and re-derives only the last row block
