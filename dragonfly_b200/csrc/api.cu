@@ -242,6 +242,23 @@ static int ensure_test_scaled(dfb_handle* h) {
   return 0;
 }
 
+// The kernel candidates are scored with: the test kernel (Add-UCB) when one is set, else the training kernel.
+struct ActiveKernel { const dfb_kernel_desc& desc; const dfb_kernel_desc* d_desc; const ScaledSet& ss; };
+static ActiveKernel active_kernel(const dfb_handle* h) {
+  if (h->have_test_kernel) return {h->desc_te, h->d_desc_te, h->te};
+  return {h->desc_tr, h->d_desc_tr, h->tr};
+}
+
+// K(X[row0 : row0 + m_rows], X) of the training kernel into Ks (n_write columns), rows beyond n as padding: the
+// posterior build (GP._get_training_kernel_matrix, gp_core.py:149-153), its replay and dfb_get_state.
+static int launch_train_kstar(dfb_handle* h, int64_t row0, int64_t m_rows, double* Ks, int64_t ldk, int64_t n_write) {
+  KstarArgs ka{};
+  ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
+  ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = h->npad; ka.Xc = h->X + row0 * h->d; ka.m = h->n - row0;
+  ka.dc = h->d; ka.m_rows = m_rows; ka.n_valid = h->n; ka.n_write = n_write; ka.Ks = Ks; ka.ldk = ldk;
+  return launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS));
+}
+
 // The blocked right-looking factorisation of the tall matrix [A ; I ; y^T] (see gemm.cuh):
 // top -> L, bottom -> L^-T, y row -> (L^-1 y)^T.
 //
@@ -450,6 +467,26 @@ static int prepare_scoring(dfb_handle* h, bool i8, bool tma) {
   return 0;
 }
 
+// The LML from lml_reduce's sums: quad = |L^-1 y|^2 or y^T alpha, log_det_half = sum log L_ii
+static double lml(double quad, double log_det_half, int64_t n) { return -0.5 * quad - log_det_half - 0.5 * (double)n * log(2.0 * M_PI); }
+
+// The tail of a factorisation of [A ; I ; y^T]: W = L^-1 from L^-T (unless LML-only), alpha (DFB_BUILD_FULL), the LML
+// sums, then the read-back of the sums and the pivot status.  A non-stationary training kernel reads back 7 sums: red[6]
+// is the max(diag K) launch_diag_max left.  end_build closes the DFB_PROF_BUILD interval before the read-back.
+static int posterior_tail(dfb_handle* h, int32_t flags, bool end_build, double red[7], int* info) {
+  const int64_t n = h->n, npad = h->npad;
+  const double* Wt = h->T + (size_t)npad * npad;
+  const double* v = h->T + (size_t)2 * npad * npad;
+  if (flags != DFB_BUILD_LML_ONLY) DFB_TRY(launch_transpose(h, Wt, h->W, npad));
+  if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
+  DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
+  if (end_build) DFB_TRY(prof_end(h, DFB_PROF_BUILD, 1.0));
+  const size_t red_bytes = sizeof(double) * (kernel_stationary(h->desc_tr) ? 3 : 7);
+  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, red_bytes, cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(info, h->info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
 
 // ---- incremental posterior update (SURVEY 8f rank 1) ------------------------------------------------------
 // Appending q training points changes only the LAST row block of L (as long as n + q stays inside the same
@@ -474,11 +511,7 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   DFB_TRY(ensure_train_scaled(h));
   DFB_CUDA_OK(cudaMemsetAsync(h->info, 0, sizeof(int) * 4, h->stream));
   // A[last, :] = K(X[last], X) + (noise + jitter) I, identity on the padding rows -> Ks scratch (128 x npad)
-  KstarArgs ka{};
-  ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
-  ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X + m0 * h->d; ka.m = n - m0; ka.dc = h->d;
-  ka.m_rows = TILE; ka.n_valid = n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
-  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  DFB_TRY(launch_train_kstar(h, m0, TILE, h->Ks, npad, npad));
   // a non-stationary kernel's max(diag K) can grow with the appended points: the block's diagonal is rebuilt here
   const bool stationary = kernel_stationary(h->desc_tr);
   if (!stationary) DFB_TRY(launch_diag_max(h, h->Ks + m0, npad, n - m0, h->red + 6));
@@ -527,16 +560,9 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   g.A = h->T; g.lda = npad; g.B = h->Dinv; g.ldb = TILE; g.D = h->T; g.ldd = npad;
   g.alpha = 1.0; g.mode = MODE_PANEL; g.K = TILE; g.step = step; g.nb = nb; g.info = h->info;
   DFB_TRY(launch_gemm(h, g, EPI_STORE, 2 * nb + 1 - (step + 1)));
-  const double* Wt = mid;
-  const double* v = yrow;
-  DFB_TRY(launch_transpose(h, Wt, h->W, npad));
-  if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
-  DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
   double red[7];
   int info = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(double) * (stationary ? 3 : 7), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaMemcpyAsync(&info, h->info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  DFB_TRY(posterior_tail(h, flags, false, red, &info));
   if (!stationary) h->max_diag = fmax(h->max_diag, red[6] + h->noise_var);
   if (info != 0) {
     set_error("extended matrix is not positive definite: non-positive pivot at index %d", info - 1);
@@ -545,10 +571,7 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   h->have_post = true;
   h->have_w = true;
   DFB_TRY(prepare_scoring(h, true, false));     // npad is unchanged: the fp64 TMA maps stay valid
-  if (lml_out_host != nullptr) {
-    const double quad = (flags == DFB_BUILD_FULL) ? red[1] : red[2];
-    *lml_out_host = -0.5 * quad - red[0] - 0.5 * (double)n * log(2.0 * M_PI);
-  }
+  if (lml_out_host != nullptr) *lml_out_host = lml((flags == DFB_BUILD_FULL) ? red[1] : red[2], red[0], n);
   return 0;
 }
 
@@ -558,150 +581,131 @@ struct ChunkOut {
 
 // Scores m candidates chunk by chunk: K_* rows + mu -> |L^-1 k_*|^2 -> sd / acquisition / arg-max.
 struct ChunkMode {
-  bool want_std, do_argmax;
-  bool use_i8;                 // int8-slice wgmma contraction instead of fp64 DMMA
-  bool collect;                // gather the shortlist for the exact re-score
-  I8ErrModel em;               // int8 error model (collect): bound on |d sigma^2|, score sensitivity
-  double pad;                  // extra slack of the shortlist test
-  const int64_t* idx_map;      // global index of each row (re-score passes), NULL = idx_base + row
-  int64_t idx_base;            // global index of row 0 when idx_map is NULL
-  bool allow_small;            // dfb_eval of <= SMALL_EVAL_M points: row-streaming kernel instead of the tile GEMM
-  bool keep_scores;            // leave the scores of a single-chunk pass in h->score (self-check of the shortlist)
-  bool keep_best;              // continue the running arg-max and best_lb of an earlier pass instead of resetting them
-  bool bound_pass;             // the upper-bound screen into the survivor list (dfb_score_argmax); with out.mu: mu_bar
+  bool want_std = false, do_argmax = false;
+  bool use_i8 = false;                 // int8-slice wgmma contraction instead of fp64 DMMA
+  bool collect = false;                // gather the shortlist for the exact re-score
+  I8ErrModel em{};                     // int8 error model (collect): bound on |d sigma^2|, score sensitivity
+  double pad = 0.0;                    // extra slack of the shortlist test
+  const int64_t* idx_map = nullptr;    // global index of each row (re-score passes), NULL = idx_base + row
+  int64_t idx_base = 0;                // global index of row 0 when idx_map is NULL
+  bool allow_small = false;            // dfb_eval of <= SMALL_EVAL_M points: row-streaming kernel instead of the tile GEMM
+  bool keep_scores = false;            // leave the scores of a single-chunk pass in h->score (self-check of the shortlist)
+  bool keep_best = false;              // continue the running arg-max and best_lb of an earlier pass instead of resetting them
 };
-static ChunkMode chunk_mode(bool want_std, bool do_argmax, bool use_i8, const int64_t* idx_map = nullptr) {
-  ChunkMode md;
-  memset(&md, 0, sizeof(md));
-  md.want_std = want_std; md.do_argmax = do_argmax; md.use_i8 = use_i8; md.idx_map = idx_map;
-  return md;
-}
 constexpr int64_t SMALL_EVAL_M = 32;      // up to four 8-wide passes over W's rows (105 MB each at N = 5000): still ~10x cheaper than one 128-wide tile pass
 
-// Per chunk two stages, back to back on the handle's stream:
-//   K: (host candidates: staging copy) K_* rows / digit planes + mu + k(x*,x*)      fp64 pipe
-//   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
-// The bound pass (md.bound_pass) replaces both by one launch of the screen per staging batch (host candidates) or per
-// keep_cap rows (device candidates), which appends the candidates whose acquisition bound reaches best_lb to the
-// survivor list; with out.mu it writes mu_bar instead, chunk by chunk (dfb_mu_upper_bound).
-static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
-                      int32_t space, double mean_const, ChunkOut out, const ChunkMode& md) {
-  const bool want_std = md.want_std, do_argmax = md.do_argmax;
-  const dfb_kernel_desc& desc = h->have_test_kernel ? h->desc_te : h->desc_tr;
-  const dfb_kernel_desc* d_desc = h->have_test_kernel ? h->d_desc_te : h->d_desc_tr;
-  const ScaledSet& ss = h->have_test_kernel ? h->te : h->tr;
-  if (dc != desc.cand_dim) {
-    set_error("candidates have %d columns, the kernel descriptor expects %d", dc, desc.cand_dim);
-    return -1;
-  }
+// Checks the candidates' column count against the active kernel and brings the scaled training sets up to date.
+static int prepare_candidates(dfb_handle* h, const ActiveKernel& k, int32_t dc, int32_t space) {
+  if (dc != k.desc.cand_dim) { set_error("candidates have %d columns, the kernel descriptor expects %d", dc, k.desc.cand_dim); return -1; }
   if (space == DFB_HOST && dc > DFB_MAX_SLOTS) { set_error("host candidates: dc > %d", DFB_MAX_SLOTS); return -1; }
   DFB_TRY(ensure_train_scaled(h));
   DFB_TRY(ensure_test_scaled(h));
+  return 0;
+}
+
+// How the rows of the caller's candidate matrix reach the device, step by step.  Steps cover the rows in order and
+// never straddle a batch.  Device rows are used in place, as one batch.  Host rows are staged in batches of as many
+// whole chunks as h->stage holds (chunk x DFB_MAX_SLOTS doubles), so a 6-column matrix needs one copy per ~21 chunks.
+// Page-locked host rows (what the streamed `rand` maximiser hands over) use the buffer as two halves, and the copy of
+// batch b+1 runs on h->cp_stream while batch b is scored (cp_done: copy done, cp_free: every step that reads the half
+// is done).  Pageable memory keeps the single-buffer copy on the compute stream: its cudaMemcpyAsync would block the
+// host on the half's cp_free and stall the launches of the batch in flight.
+struct CandidateStage {
+  dfb_handle* h = nullptr;
+  const double* Xc = nullptr; // the caller's rows
+  int64_t m = 0, batch = 0;   // batch: rows per batch
+  int32_t dc = 0;
+  bool host = false;          // the rows, and so the results, are in host memory
+  bool dbuf = false;          // page-locked host rows: two halves, copies one batch ahead on h->cp_stream
+
+  int open(dfb_handle* hh, const double* X, int64_t mm, int32_t d, int32_t space) {
+    h = hh; Xc = X; m = batch = mm; dc = d; host = space == DFB_HOST;
+    if (!host) return 0;
+    const int64_t Mc = h->chunk;
+    const int64_t stage_rows = (Mc * DFB_MAX_SLOTS / dc) / Mc * Mc;
+    const int64_t half_rows = (stage_rows / Mc / 2) * Mc;
+    if (half_rows >= Mc && m > half_rows) {
+      cudaPointerAttributes pa;
+      if (cudaPointerGetAttributes(&pa, Xc) == cudaSuccess && pa.type == cudaMemoryTypeHost) dbuf = true;
+      cudaGetLastError();                                   // an unregistered pointer may leave a sticky-free error behind
+    }
+    batch = dbuf ? half_rows : stage_rows;
+    if (!dbuf) return 0;
+    if (h->cp_stream == nullptr) {
+      DFB_CUDA_OK(cudaStreamCreateWithFlags(&h->cp_stream, cudaStreamNonBlocking));
+      cudaEvent_t* evs[5] = {&h->cp_done[0], &h->cp_free[0], &h->cp_done[1], &h->cp_free[1], &h->cp_fork};
+      for (int i = 0; i < 5; i++) DFB_CUDA_OK(cudaEventCreateWithFlags(evs[i], cudaEventDisableTiming));
+    }
+    DFB_CUDA_OK(cudaEventRecord(h->cp_fork, h->stream));  // the copy stream starts after everything already on the caller's stream
+    DFB_CUDA_OK(cudaStreamWaitEvent(h->cp_stream, h->cp_fork, 0));
+    return 0;
+  }
+  // *xc: the device rows of the step that starts at row c0
+  int rows(int64_t c0, const double** xc) {
+    if (!host) { *xc = Xc + c0 * dc; return 0; }
+    const int64_t bi = c0 / batch;
+    if (c0 % batch == 0) {                                  // first step of batch bi
+      if (bi == 0 || !dbuf) DFB_TRY(copy(bi));
+      if (dbuf && (bi + 1) * batch < m) DFB_TRY(copy(bi + 1));
+      if (dbuf) DFB_CUDA_OK(cudaStreamWaitEvent(h->stream, h->cp_done[bi & 1], 0));
+    }
+    *xc = buffer(bi) + (c0 - bi * batch) * dc;
+    return 0;
+  }
+  // Every launch that reads rows c0 .. c0 + mc - 1 is enqueued: after the last step of a batch its half may be refilled.
+  int done(int64_t c0, int64_t mc) {
+    if (dbuf && (c0 + mc == m || (c0 + mc) % batch == 0))
+      DFB_CUDA_OK(cudaEventRecord(h->cp_free[(c0 / batch) & 1], h->stream));
+    return 0;
+  }
+  double* buffer(int64_t bi) const { return h->stage + (dbuf ? (bi & 1) * batch * dc : 0); }
+  int copy(int64_t bi) {      // batch bi into its buffer: on the compute stream, or one batch ahead on the copy stream
+    const int64_t lo = bi * batch, hi = std::min(m, lo + batch);
+    const cudaStream_t s = dbuf ? h->cp_stream : h->stream;
+    if (dbuf && bi >= 2) DFB_CUDA_OK(cudaStreamWaitEvent(s, h->cp_free[bi & 1], 0));
+    DFB_CUDA_OK(cudaMemcpyAsync(buffer(bi), Xc + lo * dc, sizeof(double) * (hi - lo) * dc, cudaMemcpyHostToDevice, s));
+    if (dbuf) DFB_CUDA_OK(cudaEventRecord(h->cp_done[bi & 1], s));
+    return 0;
+  }
+};
+
+// Per chunk two stages, back to back on the handle's stream:
+//   K: K_* rows / digit planes + mu + k(x*,x*)                                      fp64 pipe
+//   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
+static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
+                      int32_t space, double mean_const, ChunkOut out, const ChunkMode& md) {
+  const bool want_std = md.want_std, do_argmax = md.do_argmax;
+  const ActiveKernel k = active_kernel(h);
+  DFB_TRY(prepare_candidates(h, k, dc, space));
   const int64_t npad = h->npad, Mc = h->chunk;
   const int nb = (int)(npad / TILE);
   if (do_argmax && !md.keep_best) DFB_TRY(launch_reset_best(h));
   const bool i8 = want_std && md.use_i8;
-  // host candidates are staged in batches of as many whole chunks as the staging buffer holds
-  // (chunk x DFB_MAX_SLOTS doubles), so a 6-column candidate matrix needs 1 copy per ~21 chunks
-  const int64_t stage_rows = (Mc * DFB_MAX_SLOTS / dc) / Mc * Mc;
-  int64_t staged_lo = 0, staged_hi = 0;
-  // Page-locked host candidates (what the streamed `rand` maximiser hands over): the staging buffer is used as two halves
-  // and the copy of batch b+1 runs on a copy stream while batch b is scored (ev_cp: copy done, ev_free: every stage
-  // that reads the half is done).  Pageable memory keeps the single-buffer copy on the compute stream: its
-  // cudaMemcpyAsync would block the host on the half's ev_free and stall the launches of the batch in flight.
-  const int64_t half_rows = (stage_rows / Mc / 2) * Mc;
-  bool dbuf = false;
-  if (space == DFB_HOST && half_rows >= Mc && m > half_rows) {
-    cudaPointerAttributes pa;
-    if (cudaPointerGetAttributes(&pa, Xc) == cudaSuccess && pa.type == cudaMemoryTypeHost) dbuf = true;
-    cudaGetLastError();                                   // an unregistered pointer may leave a sticky-free error behind
-  }
-  if (dbuf) {
-    if (h->cp_stream == nullptr) {
-      DFB_CUDA_OK(cudaStreamCreateWithFlags(&h->cp_stream, cudaStreamNonBlocking));
-      for (int i = 0; i < 2; i++) {
-        DFB_CUDA_OK(cudaEventCreateWithFlags(&h->cp_done[i], cudaEventDisableTiming));
-        DFB_CUDA_OK(cudaEventCreateWithFlags(&h->cp_free[i], cudaEventDisableTiming));
-      }
-      DFB_CUDA_OK(cudaEventCreateWithFlags(&h->cp_fork, cudaEventDisableTiming));
-    }
-    DFB_CUDA_OK(cudaEventRecord(h->cp_fork, h->stream));  // the copy stream starts after everything already on the caller's stream
-    DFB_CUDA_OK(cudaStreamWaitEvent(h->cp_stream, h->cp_fork, 0));
-  }
-  // rows per step: a chunk, or for the screen a whole staging batch / keep_cap device rows
-  int64_t step = Mc;
-  if (md.bound_pass && out.mu == nullptr) step = space != DFB_HOST ? h->keep_cap : dbuf ? half_rows : stage_rows;
-  auto issue_copy = [&](int64_t bi) -> int {               // batch bi -> half bi % 2, on the copy stream
-    const int64_t lo = bi * half_rows;
-    const int64_t hi = (m - lo < half_rows) ? m : lo + half_rows;
-    if (bi >= 2) DFB_CUDA_OK(cudaStreamWaitEvent(h->cp_stream, h->cp_free[bi & 1], 0));
-    DFB_CUDA_OK(cudaMemcpyAsync(h->stage + (bi & 1) * half_rows * dc, Xc + lo * dc, sizeof(double) * (hi - lo) * dc,
-                                cudaMemcpyHostToDevice, h->cp_stream));
-    DFB_CUDA_OK(cudaEventRecord(h->cp_done[bi & 1], h->cp_stream));
-    return 0;
-  };
-  auto release_half = [&](int64_t c0) -> int {             // last chunk of its batch: the half may be overwritten
-    if (!dbuf) return 0;
-    const int64_t bi = c0 / half_rows;
-    const int64_t b_hi = (m - bi * half_rows < half_rows) ? m : (bi + 1) * half_rows;
-    if (c0 + step >= b_hi) DFB_CUDA_OK(cudaEventRecord(h->cp_free[bi & 1], h->stream));
-    return 0;
-  };
+  CandidateStage st;
+  DFB_TRY(st.open(h, Xc, m, dc, space));
   const int* abort_count = md.collect ? h->list_count : nullptr;
   const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
                      (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
   // K_* arguments of every chunk; the candidates, their count and mu are set per chunk
   KstarArgs ka{};
-  ka.desc = &desc; ka.d_desc = d_desc; ka.xsT = ss.xs; ka.nrmT = ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
+  ka.desc = &k.desc; ka.d_desc = k.d_desc; ka.xsT = k.ss.xs; ka.nrmT = k.ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
   ka.dc = dc; ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad; ka.mean_const = mean_const;
   ka.kss_out = want_std ? h->kssv : nullptr; ka.abort_count = abort_count; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
   if (i8) {
     ka.planes = h->Ki8; ka.plane_bytes = 2 * h->chunk * npad; ka.row_bytes = 2 * npad;
-    ka.inv_colscale = 1.0 / i8_colscale(desc);
+    ka.inv_colscale = 1.0 / i8_colscale(k.desc);
   }
   const KstarWant want = !want_std ? KstarWant::MU : i8 ? KstarWant::DIGITS : KstarWant::ROWS;
 
-  for (int64_t c0 = 0; c0 < m; c0 += step) {
-    const int64_t mc = (m - c0 < step) ? (m - c0) : step;
+  for (int64_t c0 = 0; c0 < m; c0 += Mc) {
+    const int64_t mc = std::min(m - c0, Mc);
     const int64_t m_rows = round_up(mc, TILE);
     const double* xc_dev;
-    if (space == DFB_HOST && dbuf) {
-      const int64_t bi = c0 / half_rows;
-      if (c0 % half_rows == 0) {                           // first chunk of a batch
-        if (bi == 0) DFB_TRY(issue_copy(0));
-        if ((bi + 1) * half_rows < m) DFB_TRY(issue_copy(bi + 1));
-        DFB_CUDA_OK(cudaStreamWaitEvent(h->stream, h->cp_done[bi & 1], 0));
-      }
-      xc_dev = h->stage + (bi & 1) * half_rows * dc + (c0 - bi * half_rows) * dc;
-    } else if (space == DFB_HOST) {
-      if (c0 >= staged_hi) {
-        staged_lo = c0;
-        staged_hi = (m - c0 < stage_rows) ? m : c0 + stage_rows;
-        DFB_CUDA_OK(cudaMemcpyAsync(h->stage, Xc + staged_lo * dc, sizeof(double) * (staged_hi - staged_lo) * dc,
-                                    cudaMemcpyHostToDevice, h->stream));
-      }
-      xc_dev = h->stage + (c0 - staged_lo) * dc;
-    } else {
-      xc_dev = Xc + c0 * dc;
-    }
+    DFB_TRY(st.rows(c0, &xc_dev));
     double* mu_dev = (space == DFB_DEVICE && out.mu) ? out.mu + c0 : h->mu;
     double* sd_dev = (space == DFB_DEVICE && out.sd) ? out.sd + c0 : h->sd;
     double* sc_dev = (space == DFB_DEVICE && out.score) ? out.score + c0
                                                          : ((out.score || md.collect || md.keep_scores) ? h->score : nullptr);
-
-    if (md.bound_pass) {
-      // mu_bar and the screen; no K_* rows, no contraction.  Void once the seed's shortlist has overflowed, like every
-      // other launch of the int8 pass.
-      DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
-      DFB_TRY(launch_prune(h, acq, desc, d_desc, ss.xs, xc_dev, mc, dc, mean_const, md.pad, md.idx_base + c0, abort_count,
-                           out.mu != nullptr ? mu_dev : nullptr));
-      DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
-      if (space == DFB_HOST && out.mu)
-        DFB_CUDA_OK(cudaMemcpyAsync(out.mu + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
-      DFB_TRY(release_half(c0));
-      continue;
-    }
-
     ka.Xc = xc_dev; ka.m = mc; ka.m_rows = m_rows; ka.mu = mu_dev;
     const KstarRoute route = route_kstar(h, ka, want);
 
@@ -728,7 +732,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       g.partial = h->partial; g.ld_partial = Mc;
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
-        const double colscale = i8_colscale(desc);
+        const double colscale = i8_colscale(k.desc);
         DFB_TRY(launch_score_i8_args(h, h->i8_radix256 != 0, h->tmWi8, h->tmKi8, nb,
                                      (int)(m_rows / i8_tile_n(h->i8_radix256)), (int)npad, h->partial, Mc,
                                      h->rowscale, colscale, abort_count));
@@ -752,7 +756,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
         DFB_TRY(launch_collect_shortlist(h, sc_dev, sd_dev, mc, md.idx_base + c0, idx_map, md.em, md.pad, xc_dev, dc));
       DFB_TRY(prof_end(h, DFB_PROF_ACQ, (double)mc));
     }
-    if (space == DFB_HOST) {
+    if (st.host) {
       if (out.mu)
         DFB_CUDA_OK(cudaMemcpyAsync(out.mu + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
       if (out.sd && want_std)
@@ -760,7 +764,34 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       if (out.score)
         DFB_CUDA_OK(cudaMemcpyAsync(out.score + c0, sc_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
     }
-    DFB_TRY(release_half(c0));
+    DFB_TRY(st.done(c0, mc));
+  }
+  return 0;
+}
+
+// The bound pass of dfb_score_argmax (see bound_pass_applies): no K_* rows, no contraction, but one screen per step of
+// keep_cap device rows or one staging batch of host rows, which appends the candidates whose acquisition bound reaches
+// best_lb - pad to the survivor list (global index idx_base + row).  With mu_out it writes mu_bar there instead, a chunk
+// per step (dfb_mu_upper_bound).  Void once *abort_count (the seed's shortlist; may be NULL) has overflowed.
+static int run_bound_pass(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc, int32_t space,
+                          double mean_const, double pad, int64_t idx_base, const int* abort_count, double* mu_out) {
+  const ActiveKernel k = active_kernel(h);
+  DFB_TRY(prepare_candidates(h, k, dc, space));
+  CandidateStage st;
+  DFB_TRY(st.open(h, Xc, m, dc, space));
+  const int64_t step = mu_out != nullptr ? h->chunk : std::min(h->keep_cap, st.batch);    // keep_cap >= a host batch
+  for (int64_t c0 = 0; c0 < m; c0 += step) {
+    const int64_t mc = std::min(m - c0, step);
+    const double* xc_dev;
+    DFB_TRY(st.rows(c0, &xc_dev));
+    double* mu_dev = mu_out == nullptr ? nullptr : space == DFB_DEVICE ? mu_out + c0 : h->mu;
+    DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
+    DFB_TRY(launch_prune(h, acq, k.desc, k.d_desc, k.ss.xs, xc_dev, mc, dc, mean_const, pad, idx_base + c0, abort_count,
+                         mu_dev));
+    DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
+    if (st.host && mu_out != nullptr)
+      DFB_CUDA_OK(cudaMemcpyAsync(mu_out + c0, mu_dev, sizeof(double) * mc, cudaMemcpyDeviceToHost, h->stream));
+    DFB_TRY(st.done(c0, mc));
   }
   return 0;
 }
@@ -912,28 +943,15 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   DFB_CUDA_OK(cudaMemsetAsync(h->info, 0, sizeof(int) * 4, h->stream));
   DFB_CUDA_OK(cudaMemsetAsync(h->T, 0, sizeof(double) * (size_t)(2 * npad + TILE) * npad, h->stream));
   DFB_TRY(ensure_train_scaled(h));
-  // K(X, X): GP._get_training_kernel_matrix (gp_core.py:149-153)
-  KstarArgs ka{};
-  ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
-  ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = npad; ka.Xc = h->X; ka.m = n; ka.dc = h->d; ka.m_rows = n;
-  ka.n_valid = n; ka.n_write = npad; ka.Ks = h->T; ka.ldk = npad;
-  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  DFB_TRY(launch_train_kstar(h, 0, n, h->T, npad, npad));
   // the jitter ladder's scale max(diag K) + noise: kss for a stationary kernel, else read off the diagonal just built
   const bool stationary = kernel_stationary(h->desc_tr);
   if (!stationary) DFB_TRY(launch_diag_max(h, h->T, npad, n, h->red + 6));
   DFB_TRY(launch_init_tall(h, h->T, n, npad, noise_var + jitter, h->yc, with_bottom ? 1 : 0));
   DFB_TRY(factorise_tall(h, h->T, npad, h->Dinv, h->info, with_bottom));
-  const double* Wt = h->T + (size_t)npad * npad;
-  const double* v = h->T + (size_t)2 * npad * npad;
-  if (with_bottom) DFB_TRY(launch_transpose(h, Wt, h->W, npad));
-  if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
-  DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
-  DFB_TRY(prof_end(h, DFB_PROF_BUILD, 1.0));
   double red[7];
   int info = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, sizeof(double) * (stationary ? 3 : 7), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaMemcpyAsync(&info, h->info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  DFB_TRY(posterior_tail(h, flags, true, red, &info));
   h->max_diag = (stationary ? h->desc_tr.kss : red[6]) + noise_var;
   h->noise_var = noise_var;
   if (info != 0) {
@@ -944,10 +962,7 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   h->have_post = true;
   h->have_w = with_bottom;
   DFB_TRY(prepare_scoring(h, true, true));
-  if (lml_out_host != nullptr) {
-    const double quad = (flags == DFB_BUILD_FULL) ? red[1] : red[2];
-    *lml_out_host = -0.5 * quad - red[0] - 0.5 * (double)n * log(2.0 * M_PI);
-  }
+  if (lml_out_host != nullptr) *lml_out_host = lml((flags == DFB_BUILD_FULL) ? red[1] : red[2], red[0], n);
   return 0;
 }
 
@@ -1019,8 +1034,7 @@ int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noi
                                                                    reinterpret_cast<char*>(d_red)));
     for (int b = 0; b < nb_items; b++) {
       info_out[b0 + b] = info[b];
-      // dfb_build_posterior's LML-only formula
-      lml_out[b0 + b] = info[b] != 0 ? NAN : -0.5 * red[2 * b + 1] - red[2 * b] - 0.5 * (double)h->n * log(2.0 * M_PI);
+      lml_out[b0 + b] = info[b] != 0 ? NAN : lml(red[2 * b + 1], red[2 * b], h->n);
     }
   }
   return 0;
@@ -1153,13 +1167,7 @@ int dfb_get_state(dfb_handle* h, double* L_dev, double* alpha_dev, double* K_dev
   DFB_CUDA_OK(cudaSetDevice(h->device));
   if (L_dev) DFB_TRY(launch_extract_lower(h, h->T, h->npad, L_dev, h->n));
   if (alpha_dev) DFB_TRY(launch_copy_pad(h, h->alpha, h->n, alpha_dev, h->n));
-  if (K_dev) {
-    KstarArgs ka{};
-    ka.desc = &h->desc_tr; ka.d_desc = h->d_desc_tr; ka.cand_uses_train_coords = 1;
-    ka.xsT = h->tr.xs; ka.nrmT = h->tr.nrm; ka.npad_tr = h->npad; ka.Xc = h->X; ka.m = h->n; ka.dc = h->d;
-    ka.m_rows = h->n; ka.n_valid = h->n; ka.n_write = h->n; ka.Ks = K_dev; ka.ldk = h->n;
-    DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
-  }
+  if (K_dev) DFB_TRY(launch_train_kstar(h, 0, h->n, K_dev, h->n, h->n));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -1182,9 +1190,9 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
   memset(&acq, 0, sizeof(acq));
   acq.kind = DFB_ACQ_MEAN;
   ChunkOut out = {mu, sd, nullptr};
-  const dfb_kernel_desc& desc = h->have_test_kernel ? h->desc_te : h->desc_tr;
-  ChunkMode md = chunk_mode(sd != nullptr, false, false);
-  md.use_i8 = (sd != nullptr) && (h->score_impl == 1) && i8_usable(h, desc);
+  ChunkMode md;
+  md.want_std = sd != nullptr;
+  md.use_i8 = (sd != nullptr) && (h->score_impl == 1) && i8_usable(h, active_kernel(h).desc);
   md.allow_small = h->small_eval != 0;
   h->last_used_i8 = md.use_i8 ? 1 : 0;
   DFB_TRY(run_chunks(h, acq, Xc, m, dc, space, mean_const, out, md));
@@ -1204,10 +1212,7 @@ int dfb_mu_upper_bound(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, i
   DFB_CUDA_OK(cudaSetDevice(h->device));
   dfb_acq_desc acq;
   memset(&acq, 0, sizeof(acq));
-  ChunkOut out = {mu_ub_out, nullptr, nullptr};
-  ChunkMode md = chunk_mode(false, false, false);
-  md.bound_pass = true;
-  DFB_TRY(run_chunks(h, acq, Xc, m, dc, space, mean_const, out, md));
+  DFB_TRY(run_bound_pass(h, acq, Xc, m, dc, space, mean_const, 0.0, 0, nullptr, mu_ub_out));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   return 0;
 }
@@ -1240,8 +1245,8 @@ int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host) {
 // (3) No dropped candidate can be a NaN winner (a negative fp64 variance gives a NaN score, and np.argmax takes the
 //     first NaN): see bound_pass_applies.
 // Order: (a) chunk 0 scored as today (collect mode) seeds best, best_lb and the shortlist; (b) the bound pass over
-// rows chunk.. (one screen + gather per launch of run_chunks' bound-pass step) fills the survivor list; (c) one
-// read-back of the survivor count; (d) the survivors are scored like any
+// rows chunk.. (run_bound_pass: one screen + gather per step) fills the survivor list; (c) one read-back of the
+// survivor count; (d) the survivors are scored like any
 // other chunk (collect mode, indices mapped back), continuing the arg-max of (a); the caller then re-scores the
 // shortlist in fp64 and runs the self-check unchanged.  A survivor list that overflows (4 chunks) voids the screen:
 // chunks 1.. are then scored as today, still continuing the seed's state.
@@ -1268,10 +1273,8 @@ static int run_chunks_pruned(dfb_handle* h, const dfb_acq_desc& acq, const doubl
   const ChunkOut none = {nullptr, nullptr, nullptr};
   const double* rest = Xc + Mc * dc;
   DFB_TRY(run_chunks(h, acq, Xc, Mc, dc, space, mean_const, none, md));                 // (a)
-  ChunkMode bp = md;
-  bp.bound_pass = true; bp.keep_best = true; bp.idx_base = Mc;
   DFB_CUDA_OK(cudaMemsetAsync(h->surv_count, 0, sizeof(int), h->stream));
-  DFB_TRY(run_chunks(h, acq, rest, m - Mc, dc, space, mean_const, none, bp));            // (b)
+  DFB_TRY(run_bound_pass(h, acq, rest, m - Mc, dc, space, mean_const, md.pad, Mc, h->list_count, nullptr));  // (b)
   int surv = 0;
   DFB_CUDA_OK(cudaMemcpyAsync(&surv, h->surv_count, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));                                        // (c)
@@ -1289,6 +1292,17 @@ static int run_chunks_pruned(dfb_handle* h, const dfb_acq_desc& acq, const doubl
   return run_chunks(h, acq, h->surv_X, surv, dc, DFB_DEVICE, mean_const, none, cont);   // (d)
 }
 
+// The running arg-max (score, index) of the handle, read back
+static int read_best(dfb_handle* h, double* best_score_host, int64_t* best_index_host) {
+  double bs = 0.0; int64_t bi = -1;
+  DFB_CUDA_OK(cudaMemcpyAsync(&bs, h->best_score, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(&bi, h->best_index, sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  if (best_score_host) *best_score_host = bs;
+  if (best_index_host) *best_index_host = bi;
+  return 0;
+}
+
 int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m, int32_t dc,
                      int32_t space, double mean_const, double* scores, double* best_score_host,
                      int64_t* best_index_host) {
@@ -1299,20 +1313,21 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
   if (acq->kind < DFB_ACQ_MEAN || acq->kind > DFB_ACQ_TTEI) { set_error("unknown acquisition kind %d", acq->kind); return -1; }
   DFB_CUDA_OK(cudaSetDevice(h->device));
   ChunkOut out = {nullptr, nullptr, scores};
-  const dfb_kernel_desc& desc = h->have_test_kernel ? h->desc_te : h->desc_tr;
+  const dfb_kernel_desc& desc = active_kernel(h).desc;
   // A caller that asks for the full score vector gets fp64 scores (parity use); the shortlist scheme
   // only guarantees the arg-max, so the int8 pass is reserved for arg-max-only calls unless forced.
   const bool fast = want_std && h->score_impl != 0 && i8_usable(h, desc) &&
                     (scores == nullptr || h->score_impl == 1);
-  ChunkMode md = chunk_mode(want_std, true, fast);
+  ChunkMode exact;                       // the fp64 arg-max
+  exact.want_std = want_std; exact.do_argmax = true;
+  ChunkMode md = exact;
+  md.use_i8 = fast;
   h->last_used_i8 = fast ? 1 : 0;
   h->last_shortlist = 0;
   h->last_selfcheck_violations = 0;
   h->last_selfcheck_ratio = 0.0;
   h->last_survivors = 0;
   h->last_pruned = 0;
-  double bs = 0.0;
-  int64_t bi = -1;
   bool need_exact_pass = !fast;
   if (fast) {
     // Pass 1: int8-slice scoring of everything, collecting the shortlist of candidates whose fp64 score could be
@@ -1342,8 +1357,8 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
       // Pass 2: exact fp64 (DMMA) re-score of the shortlist; indices map back to the caller's rows.  Then the
       // self-check: int8 vs fp64 score of every listed candidate against its allowance.
       h->last_shortlist = count;
-      ChunkMode ex = chunk_mode(want_std, true, false, h->list_idx);
-      ex.keep_scores = true;
+      ChunkMode ex = exact;
+      ex.idx_map = h->list_idx; ex.keep_scores = true;
       ChunkOut none = {nullptr, nullptr, nullptr};
       DFB_TRY(run_chunks(h, *acq, h->list_X, count, dc, DFB_DEVICE, mean_const, none, ex));
       DFB_TRY(launch_selfcheck(h, h->score, count));
@@ -1355,16 +1370,8 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
       if (chk[0] > 0) need_exact_pass = true;      // the error model failed on a candidate that matters: fp64
     }
   }
-  if (need_exact_pass) {
-    ChunkMode ex = chunk_mode(want_std, true, false);
-    DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, ex));
-  }
-  DFB_CUDA_OK(cudaMemcpyAsync(&bs, h->best_score, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaMemcpyAsync(&bi, h->best_index, sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  if (best_score_host) *best_score_host = bs;
-  if (best_index_host) *best_index_host = bi;
-  return 0;
+  if (need_exact_pass) DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, exact));
+  return read_best(h, best_score_host, best_index_host);
 }
 
 int dfb_moo_score_argmax(dfb_handle* h, const dfb_moo_desc* desc, const double* const* a_dev,
@@ -1380,14 +1387,7 @@ int dfb_moo_score_argmax(dfb_handle* h, const dfb_moo_desc* desc, const double* 
   DFB_CUDA_OK(cudaSetDevice(h->device));
   DFB_TRY(launch_reset_best(h));
   DFB_TRY(launch_moo(h, *desc, a_dev, ucb ? b_dev : nullptr, m, scores_dev));
-  double bs = 0.0;
-  int64_t bi = -1;
-  DFB_CUDA_OK(cudaMemcpyAsync(&bs, h->best_score, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaMemcpyAsync(&bi, h->best_index, sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
-  if (best_score_host) *best_score_host = bs;
-  if (best_index_host) *best_index_host = bi;
-  return 0;
+  return read_best(h, best_score_host, best_index_host);
 }
 
 int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* X1_dev, int64_t n1,
@@ -1417,11 +1417,9 @@ int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* 
 // K_* -> V^T = K_* W^T -> Cov = K** - V^T V    (gp_core.py:173-181)
 static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc,
                                 double mean_const, int64_t* mbp_out, bool lower_only) {
-  const dfb_kernel_desc& desc = h->have_test_kernel ? h->desc_te : h->desc_tr;
-  const dfb_kernel_desc* d_desc = h->have_test_kernel ? h->d_desc_te : h->d_desc_tr;
-  const ScaledSet& ss = h->have_test_kernel ? h->te : h->tr;
+  const ActiveKernel k = active_kernel(h);
   if (h->ts_ws == nullptr) { set_error("no Thompson-sampling workspace: call dfb_set_ts_workspace first"); return -1; }
-  if (dc != desc.cand_dim) { set_error("candidates have %d columns, the kernel descriptor expects %d", dc, desc.cand_dim); return -1; }
+  if (dc != k.desc.cand_dim) { set_error("candidates have %d columns, the kernel descriptor expects %d", dc, k.desc.cand_dim); return -1; }
   const int64_t mbp = round_up(m, TILE);
   if (m < 1 || mbp > h->ts_mb || mbp > h->chunk) { set_error("block of %lld candidates exceeds the TS workspace (%lld) / chunk (%lld)", (long long)m, (long long)h->ts_mb, (long long)h->chunk); return -1; }
   DFB_TRY(ensure_train_scaled(h));
@@ -1430,7 +1428,7 @@ static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, 
   const int nb = (int)(npad / TILE), mbb = (int)(mbp / TILE);
   // K_* rows (zero rows beyond m) and mu
   KstarArgs ka{};
-  ka.desc = &desc; ka.d_desc = d_desc; ka.xsT = ss.xs; ka.nrmT = ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
+  ka.desc = &k.desc; ka.d_desc = k.d_desc; ka.xsT = k.ss.xs; ka.nrmT = k.ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
   ka.Xc = Xc_dev; ka.m = m; ka.dc = dc; ka.m_rows = mbp; ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
   ka.mean_const = mean_const; ka.mu = h->ts_mu; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
   DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
@@ -1441,7 +1439,7 @@ static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, 
   g.mode = MODE_GENERIC; g.n_rb = mbb; g.n_cb = nb; g.K = (int)npad; g.tri = 2;
   DFB_TRY(launch_gemm(h, g, EPI_STORE, mbb * nb));
   // K** = kernel(X_test, X_test) (gp_core.py:179) with the candidates as both sides
-  DFB_TRY(launch_prep_scaled(h, d_desc, 0, Xc_dev, m, dc, h->ts_cxs, h->ts_cnrm, mbp));
+  DFB_TRY(launch_prep_scaled(h, k.d_desc, 0, Xc_dev, m, dc, h->ts_cxs, h->ts_cnrm, mbp));
   ka.xsT = h->ts_cxs; ka.nrmT = h->ts_cnrm; ka.npad_tr = mbp; ka.alpha = nullptr; ka.n_valid = m; ka.n_write = mbp;
   ka.Ks = h->ts_Cov; ka.ldk = mbp; ka.mean_const = 0.0; ka.mu = nullptr;
   DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
@@ -1604,7 +1602,7 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
 int dfb_query(dfb_handle* h, const char* name, double* out) {
   DFB_TRY(need(h, false, false, false, false, false));
   if (name == nullptr || out == nullptr) { set_error("bad query arguments"); return -1; }
-  const dfb_kernel_desc& desc = h->have_test_kernel ? h->desc_te : h->desc_tr;
+  const dfb_kernel_desc& desc = active_kernel(h).desc;
   if (strcmp(name, "i8_sigma2_bound") == 0) { *out = h->i8_ready ? i8_sigma2_bound(h, desc) : -1.0; return 0; }
   if (strcmp(name, "last_used_i8") == 0) { *out = (double)h->last_used_i8; return 0; }
   if (strcmp(name, "last_shortlist") == 0) { *out = (double)h->last_shortlist; return 0; }

@@ -165,7 +165,7 @@ struct dfb_handle {
   int8_t* Ki8 = nullptr;      // the same for the K_* chunk
   double* cprep = nullptr;    // chunk x 10 scaled candidate rows (cand_prep_kernel)
   double* mu_part = nullptr;  // (npad / 64 + 2) x chunk
-  cudaStream_t cp_stream = nullptr;   // H2D copies of page-locked host candidates, one batch ahead (api.cu: run_chunks)
+  cudaStream_t cp_stream = nullptr;   // H2D copies of page-locked host candidates, one batch ahead (api.cu: CandidateStage)
   cudaEvent_t cp_fork = nullptr, cp_done[2] = {nullptr, nullptr}, cp_free[2] = {nullptr, nullptr};
   double* rowscale = nullptr; // npad  2^E_i
   double* rowinv = nullptr;   // npad  2^-E_i

@@ -1,5 +1,5 @@
 """
-The bound pass of dfb_score_argmax (option "prune", api.cu: run_chunks_pruned) (-m gpu).
+The bound pass of dfb_score_argmax (option "prune", api.cu: run_chunks_pruned, run_bound_pass) (-m gpu).
 
 After chunk 0 is scored, the candidates of the later chunks get mu alone and are dropped when acq(mu, sqrt(k**)) lies
 below a certain lower bound of the fp64 maximum.  The arg-max must not notice: prune = 1 returns the same (score,
@@ -178,9 +178,14 @@ def test_m_around_the_chunk(B, small, m):
       assert surv + pruned == 1
 
 
-@pytest.mark.parametrize('space', ['pageable', 'pinned', 'device'])
-def test_candidate_memory_spaces(B, small, space):
-  m = 12 * CHUNK + 5           # > half the staging buffer: the double-buffered copy of page-locked candidates
+SPACES = ['pageable', 'pinned', 'device']
+
+
+# 12 chunks: > half the staging buffer, the double-buffered copy of page-locked candidates.  45 chunks: at d = 6 a staging
+# batch is 21 chunks, so the bound pass of pageable candidates crosses three batches, page-locked ones five halves.
+@pytest.mark.parametrize('space,m', [(s, 12 * CHUNK + 5) for s in SPACES] + [(s, 45 * CHUNK + 5) for s in SPACES],
+                         ids=SPACES + [s + '-45chunks' for s in SPACES])
+def test_candidate_memory_spaces(B, small, space, m):
   host = small.rs.random_sample((m, 6))
   if space == 'pageable':
     C = host

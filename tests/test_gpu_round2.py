@@ -174,7 +174,7 @@ def test_cartesian_product_gp_against_the_reference(B):
 
 
 def test_page_locked_host_candidates_match_device_and_pageable_bit_for_bit(B, gp1500):
-  """ Host candidates in page-locked memory take the double-buffered staging path of run_chunks (copy of batch b+1 on a
+  """ Host candidates in page-locked memory take the double-buffered path of CandidateStage (copy of batch b+1 on a
       copy stream while batch b is scored): same results as device-resident and as pageable candidates, bit for bit,
       over several batches, for the fused arg-max and for eval. """
   w, gp = gp1500

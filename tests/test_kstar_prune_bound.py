@@ -1,5 +1,5 @@
 """
-The two facts the bound pass of dfb_score_argmax rests on (api.cu: bound_pass_applies, run_chunks_pruned), on the CPU.
+The two facts the bound pass of dfb_score_argmax (api.cu: bound_pass_applies, run_bound_pass) rests on, on the CPU.
 
 Variance floor: for K = k(X, X) of a stationary kernel, s > 0 the diagonal added to it and any x*,
     sigma^2(x*) = k** - k^T (K + s I)^-1 k >= k** s / (tr K + s),
