@@ -1582,6 +1582,8 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
   const void* src = nullptr;
   int64_t size = 0;
   if (strcmp(name, "W") == 0) { src = h->W; size = (int64_t)sizeof(double) * npad * npad; }
+  else if (strcmp(name, "T") == 0) { src = h->T; size = (int64_t)sizeof(double) * (2 * npad + TILE) * npad; }
+  else if (strcmp(name, "alpha") == 0) { src = h->alpha; size = (int64_t)sizeof(double) * npad; }
   else if (strcmp(name, "Wi8") == 0) { src = h->Wi8; size = 3 * 2 * npad * npad; }
   else if (strcmp(name, "rowscale") == 0) { src = h->rowscale; size = (int64_t)sizeof(double) * npad; }
   else if (strcmp(name, "Ki8") == 0) { src = h->Ki8; size = 3 * 2 * chunk * npad; }

@@ -327,7 +327,9 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
 /* Diagnostics: device-to-device copy of one internal buffer of the current state; bytes must equal its size (query
  * "npad" and "chunk"): "W" (fp64 L^-1, npad^2), "Wi8" (its three digit planes, 6 npad^2 bytes), "rowscale" (npad
  * doubles), "Ki8" (the three K_* digit planes of the chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
- * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk).
+ * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk),
+ * "T" (the factorised tall matrix [L ; L^-T ; (L^-1 y_c)^T], (2 npad + 128) x npad: its padding, the y row), "alpha"
+ * (npad doubles, padding included).
  * Synchronises. */
 int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
 /* Diagnostics (tests/test_gpu_prune_f32.py): the largest relative error of ex2.approx.ftz.f32 (which = 0) over every
