@@ -15,7 +15,8 @@ DFB_MAX_FACTORS = 48
 DFB_MAX_TERMS = 48
 DFB_MAX_SLOTS = 128
 DFB_MAX_MATERN_P = 3
-DFB_BASE_SE, DFB_BASE_MATERN, DFB_BASE_POLY, DFB_BASE_EXPDECAY = 0, 1, 2, 3
+DFB_BASE_SE, DFB_BASE_MATERN, DFB_BASE_POLY, DFB_BASE_EXPDECAY, DFB_BASE_HAMMING = 0, 1, 2, 3, 4
+DFB_CAND_REAL, DFB_CAND_INTEGER, DFB_CAND_CATEGORICAL = 0, 1, 2
 DFB_DEVICE, DFB_HOST = 0, 1
 DFB_ACQ_MEAN, DFB_ACQ_UCB, DFB_ACQ_EI, DFB_ACQ_PI, DFB_ACQ_TTEI = 0, 1, 2, 3, 4
 DFB_BUILD_FULL, DFB_BUILD_LML_ONLY, DFB_BUILD_NO_ALPHA = 0, 1, 2
@@ -93,6 +94,8 @@ PROTOTYPES = {
   'dfb_fill_rng': (C.c_int, [_P, C.c_uint64, _I64, _I32, _I64, _I32, _P]),
   'dfb_ts_argmax': (C.c_int, [_P, _P, _I64, _I32, _I64, _I64, _I32, _P, _P]),
   'dfb_fill_candidates': (C.c_int, [_P, C.c_uint64, _I64, _I64, _I32, C.POINTER(_D), C.POINTER(_D), _P]),
+  'dfb_fill_mixed_candidates': (C.c_int, [_P, C.c_uint64, _I64, _I64, _I32, C.POINTER(_I32), C.POINTER(_D),
+                                          C.POINTER(_D), C.POINTER(_I64), _P]),
   'dfb_measure_peak': (C.c_int, [C.c_int, C.c_int, C.POINTER(_D)]),
   'dfb_launch_count': (_I64, [_P]),
   'dfb_debug_score_i8': (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _P, _D, _P, _P, _I64]),

@@ -151,27 +151,30 @@ static int check_desc(const dfb_kernel_desc* d) {
   }
   for (int f = 0; f < d->n_factors; f++) {
     const dfb_factor_desc& fd = d->factors[f];
-    if (fd.kind < DFB_BASE_SE || fd.kind > DFB_BASE_EXPDECAY || fd.n_dims < 1 ||
+    if (fd.kind < DFB_BASE_SE || fd.kind > DFB_BASE_HAMMING || fd.n_dims < 1 ||
         fd.slot_off < 0 || fd.slot_off + fd.n_dims > d->n_slots || fd.p < 0 ||
-        (fd.kind == DFB_BASE_MATERN && fd.p > DFB_MAX_MATERN_P) || (fd.kind == DFB_BASE_EXPDECAY && fd.p != 0) ||
+        (fd.kind == DFB_BASE_MATERN && fd.p > DFB_MAX_MATERN_P) ||
+        ((fd.kind == DFB_BASE_EXPDECAY || fd.kind == DFB_BASE_HAMMING) && fd.p != 0) ||
         (fd.kind >= DFB_BASE_POLY && !(fd.scale > 0.0 && isfinite(fd.scale))) ||
         (fd.kind == DFB_BASE_EXPDECAY && !isfinite(fd.s2))) {
       set_error("kernel descriptor: bad factor %d", f);
       return -1;
     }
-    // slot_bandwidth means a bandwidth, a scaling or a power depending on the kind (dfb200.h): a slot of a POLY or
-    // EXPDECAY factor belongs to that factor alone
+    // slot_bandwidth means a bandwidth, a scaling, a power or a weight depending on the kind (dfb200.h): a slot of a
+    // POLY, EXPDECAY or HAMMING factor belongs to that factor alone
     if (fd.kind >= DFB_BASE_POLY) {
       for (int g = 0; g < d->n_factors; g++) {
         const dfb_factor_desc& gd = d->factors[g];
         if (g != f && gd.slot_off < fd.slot_off + fd.n_dims && fd.slot_off < gd.slot_off + gd.n_dims) {
-          set_error("kernel descriptor: factor %d shares slots with POLY / EXPDECAY factor %d", g, f);
+          set_error("kernel descriptor: factor %d shares slots with POLY / EXPDECAY / HAMMING factor %d", g, f);
           return -1;
         }
       }
       for (int q = 0; q < fd.n_dims; q++) {
-        if (!isfinite(d->slot_bandwidth[fd.slot_off + q])) {
-          set_error("kernel descriptor: factor %d has a non-finite %s", f, fd.kind == DFB_BASE_POLY ? "scaling" : "power");
+        const double w = d->slot_bandwidth[fd.slot_off + q];
+        if (!isfinite(w) || (fd.kind == DFB_BASE_HAMMING && !(w >= 0.0))) {
+          set_error("kernel descriptor: factor %d has a %s %s", f, fd.kind == DFB_BASE_HAMMING ? "negative or non-finite" :
+                    "non-finite", fd.kind == DFB_BASE_POLY ? "scaling" : fd.kind == DFB_BASE_HAMMING ? "weight" : "power");
           return -1;
         }
       }
@@ -202,7 +205,8 @@ static int check_desc(const dfb_kernel_desc* d) {
         return -1;
       }
       if (d->factors[f].kind >= DFB_BASE_POLY) {
-        set_error("kernel descriptor: ESP term %d is a POLY / EXPDECAY factor (ESP children are SE or Matern)", t);
+        set_error("kernel descriptor: ESP term %d is a POLY / EXPDECAY / HAMMING factor (ESP children are SE or Matern)",
+                  t);
         return -1;
       }
     }
@@ -982,6 +986,12 @@ int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noi
   for (int b = 0; b < B; b++) {
     DFB_TRY(check_desc(&descs[b]));
     if (descs[b].esp_order != 0) { set_error("lml_batch: item %d is an ESP kernel", b); return -1; }
+    for (int f = 0; f < descs[b].n_factors; f++) {
+      if (descs[b].factors[f].kind == DFB_BASE_HAMMING) {
+        set_error("lml_batch: item %d has a HAMMING factor (batched fitting covers Euclidean kernels only)", b);
+        return -1;
+      }
+    }
     if (descs[b].train_dim != h->d) {
       set_error("lml_batch: item %d has train_dim %d != data dim %d", b, descs[b].train_dim, h->d);
       return -1;
@@ -1114,7 +1124,7 @@ int dfb_lml_gradients(dfb_handle* h, double* out_host, int32_t n_out) {
   const dfb_kernel_desc& desc = h->desc_tr;
   if (desc.n_terms != 1 || desc.n_factors != 1 || desc.esp_order != 0 ||
       (desc.factors[0].kind != DFB_BASE_SE && desc.factors[0].kind != DFB_BASE_MATERN)) {
-    // the reference's composite, ESP, Poly and ExpDecay kernels inherit Kernel._child_gradient, which raises
+    // the reference's composite, ESP, Poly, ExpDecay and Hamming kernels inherit Kernel._child_gradient, which raises
     // (kernel.py:123-125)
     set_error("LML gradients are defined for plain SE / Matern kernels only (kernel has %d terms, %d factors, "
               "ESP order %d, first factor kind %d)", desc.n_terms, desc.n_factors, desc.esp_order, desc.factors[0].kind);
@@ -1535,6 +1545,27 @@ int dfb_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, i
   }
   DFB_CUDA_OK(cudaSetDevice(h->device));
   return launch_fill_candidates(h, seed, row0, m, d, lo_host, hi_host, out_dev);
+}
+
+int dfb_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int32_t d, const int32_t* kinds_host,
+                              const double* lo_host, const double* hi_host, const int64_t* n_levels_host, double* out_dev) {
+  DFB_TRY(need(h, false, false, false, false, false));
+  if (out_dev == nullptr || kinds_host == nullptr || lo_host == nullptr || hi_host == nullptr || m < 1 || row0 < 0 ||
+      d < 1 || d > DFB_MAX_SLOTS) {
+    set_error("bad fill_mixed_candidates arguments (m = %lld, d = %d)", (long long)m, d);
+    return -1;
+  }
+  for (int s = 0; s < d; s++) {
+    const int k = kinds_host[s];
+    if (k < DFB_CAND_REAL || k > DFB_CAND_CATEGORICAL ||
+        (k == DFB_CAND_CATEGORICAL && (n_levels_host == nullptr || n_levels_host[s] < 1 ||
+                                       n_levels_host[s] > ((int64_t)1 << 52)))) {
+      set_error("fill_mixed_candidates: bad column %d (kind %d)", s, k);
+      return -1;
+    }
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  return launch_fill_mixed_candidates(h, seed, row0, m, d, kinds_host, lo_host, hi_host, n_levels_host, out_dev);
 }
 
 int dfb_ts_argmax(dfb_handle* h, const double* samples_dev, int64_t ld, int32_t S, int64_t m, int64_t idx_base,

@@ -82,6 +82,8 @@ int launch_reset_best(dfb_handle* h);
 int launch_fill_rng(dfb_handle* h, uint64_t seed, int64_t col0, int S, int64_t m, int what, double* out);
 int launch_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int d, const double* lo,
                            const double* hi, double* out);
+int launch_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int d, const int32_t* kinds,
+                                 const double* lo, const double* hi, const int64_t* n_levels, double* out);
 int launch_ts_argmax(dfb_handle* h, const double* samples, int64_t ld, int S, int64_t m, int64_t idx_base, int reset,
                      double* best, int64_t* index);
 int launch_small_sumsq(dfb_handle* h, const double* W, int64_t ldw, const double* Ks, int64_t ldk, int64_t n_rows,

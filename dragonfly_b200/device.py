@@ -336,6 +336,24 @@ class DevicePosterior(object):
                                             C.c_void_p(out.data_ptr())), 'dfb_fill_candidates')
     return out
 
+  def fill_mixed_candidates(self, seed, row0, m, kinds, bounds, n_levels, out=None):
+    """ dfb_fill_mixed_candidates: rows row0 .. row0+m-1 of the device-generated candidate matrix of a Cartesian-product
+        domain; kinds: per column DFB_CAND_*; bounds: (d, 2) [lo, hi] (read for real / integer columns); n_levels: per
+        column number of categories (read for categorical columns). """
+    k = np.ascontiguousarray(np.asarray(kinds, dtype=np.int32))
+    b = np.ascontiguousarray(np.asarray(bounds, dtype=np.float64)).reshape(-1, 2)
+    lv = np.ascontiguousarray(np.asarray(n_levels, dtype=np.int64))
+    d = int(k.shape[0])
+    lo = np.ascontiguousarray(b[:, 0]); hi = np.ascontiguousarray(b[:, 1])
+    if out is None:
+      out = torch.empty((int(m), d), dtype=torch.float64, device=self.device)
+    _lib.check(self.lib.dfb_fill_mixed_candidates(
+        self.h, C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), int(row0), int(m), d,
+        k.ctypes.data_as(C.POINTER(C.c_int32)), lo.ctypes.data_as(C.POINTER(C.c_double)),
+        hi.ctypes.data_as(C.POINTER(C.c_double)), lv.ctypes.data_as(C.POINTER(C.c_int64)),
+        C.c_void_p(out.data_ptr())), 'dfb_fill_mixed_candidates')
+    return out
+
   def ts_argmax(self, samples, idx_base, best, index, reset):
     """ dfb_ts_argmax: fold one block of draws (S x m CUDA tensor) into the running per-draw arg-max. """
     S, m = int(samples.shape[0]), int(samples.shape[1])

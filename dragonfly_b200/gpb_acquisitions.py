@@ -44,6 +44,225 @@ def _check_rand_euclidean(anc_data):
   return anc_data.acq_opt_method in ['rand']
 
 
+def _is_cp_domain(anc_data):
+  return anc_data.domain.get_type() == 'cartesian_product'
+
+
+# ---------------------------------------------------------------------------------------------
+# Cartesian-product domains (maximise_acquisition's CP branch, :35-37; exd_utils.py:219-289)
+# ---------------------------------------------------------------------------------------------
+_CP_NUMERIC = ('euclidean', 'integral')
+_CP_DISCRETE = ('prod_discrete', 'prod_discrete_numeric')
+
+
+class _CPPart(object):
+  """ One part of a CP domain as candidate columns: its type, column count, bounds (numeric parts), the lists of levels
+      (discrete parts) and, for a part under a Hamming factor, that factor's CategoryCodes table. """
+  __slots__ = ('type', 'dim', 'bounds', 'levels', 'codes')
+
+
+def _cp_parts(domain, kernel):
+  """ The parts of a CP domain in domain order; raises for what the device does not serve (constraints, NN and
+      discrete-Euclidean parts, nested CP domains). """
+  from .kernel import category_codes, _kind_of
+  has_constraints = getattr(domain, 'has_constraints', None)
+  if has_constraints is not None and has_constraints():
+    raise NotImplementedError('Constrained Cartesian-product domains are outside the GPU hot-path scope.')
+  kernel_list = getattr(kernel, 'kernel_list', None)
+  if kernel_list is None or len(kernel_list) != len(domain.list_of_domains):
+    raise NotImplementedError('A Cartesian-product domain needs a CPGP whose kernel has one factor per part.')
+  parts = []
+  for dom, kern in zip(domain.list_of_domains, kernel_list):
+    p = _CPPart()
+    p.type = dom.get_type()
+    p.bounds, p.levels, p.codes = None, None, None
+    if p.type in _CP_NUMERIC:
+      p.bounds = np.asarray(dom.bounds)
+      p.dim = len(p.bounds)
+    elif p.type in _CP_DISCRETE:
+      p.levels = [list(loi) for loi in dom.list_of_list_of_items]
+      p.dim = len(p.levels)
+      if _kind_of(kern) == 'HammingKernel':
+        p.codes = category_codes(kern)
+      elif p.type != 'prod_discrete_numeric':
+        raise NotImplementedError('A prod_discrete part needs a HammingKernel factor.')
+    else:
+      raise NotImplementedError("Domain parts of type '%s' are outside the GPU hot-path scope." % (p.type))
+    parts.append(p)
+  return parts
+
+
+def _level_columns(p, level_values):
+  """ The candidate column values of one discrete coordinate's levels: Hamming codes, or the numeric values. """
+  if p.codes is not None:
+    return np.array([p.codes.encode(v) for v in level_values], dtype=np.float64)
+  return np.asarray(level_values, dtype=np.float64)
+
+
+def draw_cp_candidates(parts, max_evals):
+  """ sample_from_cp_domain_without_constraints (cp_domain_utils.py:448-489) for M = max_evals points, part by part in
+      domain order, consuming the global MT19937 stream exactly as the reference does:
+        euclidean  map_to_bounds(np.random.random((M, d_j)), bounds)                    oper_utils.py:318-326
+        integral   the same, then .astype(int)                                           oper_utils.py:337-340
+        discrete   one np.random.choice(levels_q) per point and coordinate, point-major  oper_utils.py:342-360
+      The last is drawn as ONE np.random.randint(0, n_q) over the (M, d_j) grid of level counts: the legacy generator
+      draws a broadcast randint element by element in C order with the same bounded-integer routine as choice's scalar
+      randint(0, n_q) (n_q = 1 draws nothing in both), so the stream advances identically.  The drawn value is
+      np.array(levels_q)[idx] -- NumPy's promotion applies ([1, 'a'] draws '1') -- and that value is what gets encoded.
+      Returns (rows, draws): the (M, sum d_j) float64 candidate matrix and per part what point_from_draws needs. """
+  M = int(max_evals)
+  cols, draws = [], []
+  for p in parts:
+    if p.type in _CP_NUMERIC:
+      vals = map_to_bounds(np.random.random((M, p.dim)), p.bounds)
+      if p.type == 'integral':
+        vals = vals.astype(int)
+      cols.append(np.asarray(vals, dtype=np.float64))
+      draws.append(vals)
+    else:
+      n_levels = np.array([len(loi) for loi in p.levels], dtype=np.int64)
+      idx = np.random.randint(0, np.broadcast_to(n_levels, (M, p.dim))) if M > 0 else np.zeros((0, p.dim), np.int64)
+      c = np.empty((M, p.dim), dtype=np.float64)
+      for q in range(p.dim):
+        arr = np.array(p.levels[q])
+        c[:, q] = _level_columns(p, [arr[k] for k in range(len(arr))])[idx[:, q]]
+      cols.append(c)
+      draws.append(idx)
+  rows = np.ascontiguousarray(np.concatenate(cols, axis=1)) if cols else np.zeros((M, 0))
+  return rows, draws
+
+
+def point_from_draws(parts, draws, i):
+  """ Point i of draw_cp_candidates in the reference's list-of-parts form: ndarray rows for Euclidean parts, int arrays
+      for integral parts, lists of NumPy scalars (np.array(levels_q)[idx]) for discrete parts. """
+  pt = []
+  for p, d in zip(parts, draws):
+    if p.type in _CP_NUMERIC:
+      pt.append(d[i])
+    else:
+      pt.append([np.array(p.levels[q])[int(d[i, q])] for q in range(p.dim)])
+  return pt
+
+
+def _cp_device_layout(parts):
+  """ Column kinds, bounds and level counts of dfb_fill_mixed_candidates for the parts, plus per discrete part the
+      level -> column value tables (the device draws level indices). """
+  from . import _lib
+  kinds, bounds, n_levels, luts = [], [], [], []
+  for p in parts:
+    for q in range(p.dim):
+      if p.type in _CP_NUMERIC:
+        kinds.append(_lib.DFB_CAND_REAL if p.type == 'euclidean' else _lib.DFB_CAND_INTEGER)
+        bounds.append([float(p.bounds[q][0]), float(p.bounds[q][1])])
+        n_levels.append(0)
+        luts.append(None)
+      else:
+        arr = np.array(p.levels[q])
+        kinds.append(_lib.DFB_CAND_CATEGORICAL)
+        bounds.append([0.0, 0.0])
+        n_levels.append(len(arr))
+        luts.append(_level_columns(p, [arr[k] for k in range(len(arr))]))
+  return kinds, bounds, n_levels, luts
+
+
+def _cp_device_rows(sess, seed, r0, m, layout, out=None):
+  """ Rows r0 .. r0+m-1 of the device-generated CP candidates, category columns mapped from level index to their column
+      value (a Hamming code or the level's number) on the device. """
+  import torch
+  kinds, bounds, n_levels, luts = layout
+  pts = sess.post.fill_mixed_candidates(seed, r0, m, kinds, bounds, n_levels, out=out)
+  for c, lut in enumerate(luts):
+    if lut is not None and not np.array_equal(lut, np.arange(len(lut), dtype=np.float64)):
+      lut_d = torch.as_tensor(lut, device=pts.device)
+      pts[:, c] = lut_d[pts[:, c].long()]
+  return pts
+
+
+def _cp_point_from_device_row(parts, row):
+  """ The list-of-parts point of one row of dfb_fill_mixed_candidates (categorical columns as level indices). """
+  pt, c = [], 0
+  for p in parts:
+    vals = row[c:c + p.dim]
+    if p.type == 'euclidean':
+      pt.append(np.array(vals, dtype=np.float64))
+    elif p.type == 'integral':
+      pt.append(np.array(vals).astype(int))
+    else:
+      pt.append([np.array(p.levels[q])[int(vals[q])] for q in range(p.dim)])
+    c += p.dim
+  return pt
+
+
+def _cp_fused_maximise(gp, anc_data, acq):
+  """ maximise_acquisition on a CP domain with acq_opt_method 'rand' (_rand_maximise_vectorised_objective_in_cp_domain,
+      exd_utils.py:247-274): the reference scores its sampled points one gp.eval at a time; here every candidate is
+      scored in fused device slabs and the arg-max follows np.argmax over the per-point values (first index on ties).
+      candidate_rng 'numpy' draws the reference's points (draw_cp_candidates), 'device' draws them with
+      dfb_fill_mixed_candidates keyed by (seed, global row, column). """
+  from . import dist as dfb_dist
+  parts = _cp_parts(anc_data.domain, gp.kernel)
+  if _shard_info()[1] > 1:
+    raise NotImplementedError('Cartesian-product candidate draws are not sharded across ranks.')
+  mode = getattr(anc_data, 'candidate_rng', None) or CANDIDATE_RNG
+  if mode not in ('numpy', 'device'):
+    raise ValueError("candidate_rng should be 'numpy' or 'device'.")
+  M = int(anc_data.max_evals)
+  if mode == 'device':
+    seed = (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
+  else:
+    rows, draws = draw_cp_candidates(parts, M)
+  with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
+    slab = sess.slab_rows(2 * STREAM_SLAB_ROWS if mode == 'device' else STREAM_SLAB_ROWS)
+    layout = _cp_device_layout(parts) if mode == 'device' else None
+    best_s, best_i, buf = 0.0, -1, None
+    for r0 in range(0, M, slab):
+      m = min(slab, M - r0)
+      if mode == 'device':
+        buf = _cp_device_rows(sess, seed, r0, m, layout, out=None if buf is None else buf[:m])
+        pts = buf
+      else:
+        pts = rows[r0:r0 + m]
+      res = sess.score(pts)
+      s, gi = float(res[0]), r0 + int(res[1])
+      if dfb_dist.better(s, gi, best_s, best_i):
+        best_s, best_i = s, gi
+    if mode == 'device':
+      kinds, bounds, n_levels, _ = layout
+      row = sess.post.fill_mixed_candidates(seed, best_i, 1, kinds, bounds, n_levels).cpu().numpy()[0]
+      return _cp_point_from_device_row(parts, row)
+  return point_from_draws(parts, draws, best_i)
+
+
+def _cp_other_maximiser(acq_fn, anc_data):
+  """ The non-'rand' maximisers on a CP domain.  'direct' / 'pdoo' on a domain of Euclidean parts only: PDOO over the
+      flattened bounds, the point regrouped into parts (maximise_with_method_on_product_euclidean_spaces,
+      exd_utils.py:219-244).  'ga' is the reference's own (a Dragonfly install is needed) with a one-point device
+      objective.  acq_fn takes a list of list-of-parts points. """
+  method = str(anc_data.acq_opt_method).lower()
+  if method.startswith(('direct', 'pdoo')):
+    doms = anc_data.domain.list_of_domains
+    if any(d.get_type() != 'euclidean' for d in doms):
+      raise NotImplementedError("'%s' on a Cartesian-product domain needs Euclidean parts only; use 'rand'." % (method))
+    dims = [int(d.get_dim()) for d in doms]
+    starts = np.concatenate(([0], np.cumsum(dims))).astype(int)
+    regroup = lambda x: [np.asarray(x)[starts[j]:starts[j + 1]] for j in range(len(dims))]
+    flat = copy(anc_data)
+    flat.domain = EuclideanDomain(np.concatenate([np.asarray(d.bounds, dtype=np.float64) for d in doms]))
+    flat_fn = lambda X: acq_fn([regroup(x) for x in np.asarray(X, dtype=np.float64)])
+    return regroup(_delegate_to_reference_maximiser(flat_fn, flat))
+  if method.startswith('ga'):
+    try:
+      from dragonfly.exd.exd_utils import maximise_with_method  # pylint: disable=import-error
+    except ImportError:
+      raise NotImplementedError("acq_opt_method '%s' on a Cartesian-product domain is the reference's GA and needs a "
+                                "Dragonfly install; 'rand' runs on the device." % (anc_data.acq_opt_method))
+    _, opt_pt = maximise_with_method(anc_data.acq_opt_method, lambda x: acq_fn([x]), anc_data.domain,
+                                     anc_data.max_evals)
+    return opt_pt
+  raise NotImplementedError("acq_opt_method '%s' is not served on Cartesian-product domains; use 'rand'."
+                            % (anc_data.acq_opt_method))
+
+
 # Multi-GPU (SURVEY.md 8e): when torch.distributed is initialised with more than one rank, every rank runs
 # the same acquisition call in lock-step -- same seed, hence the same candidate matrix -- scores only its
 # contiguous shard of the rows on its own GPU and joins with ONE 16-byte all-gather (dist.all_reduce_argmax).
@@ -349,9 +568,18 @@ def _get_gp_ucb_dim(gp):
   """ transcribed from the reference's :202-209 """
   if hasattr(gp, 'ucb_dim') and gp.ucb_dim is not None:
     return gp.ucb_dim
-  elif hasattr(gp.kernel, 'dim'):
+  elif hasattr(gp.kernel, 'dim') and type(gp.kernel).__name__ != 'CartesianProductKernel':
+    # the reference's CartesianProductKernel has no `dim` (kernel.py:504-518); ours carries one for the descriptor
     return gp.kernel.dim
   return 3.0
+
+
+def _acq_on_cp_domain(gp, anc_data, acq, acq_fn):
+  """ CP-domain dispatch of the acquisitions below: the fused 'rand' maximiser, else _cp_other_maximiser with the
+      host objective acq_fn(list of points). """
+  if anc_data.acq_opt_method in ['rand']:
+    return _cp_fused_maximise(gp, anc_data, acq)
+  return _cp_other_maximiser(acq_fn, anc_data)
 
 
 def _get_ucb_beta_th(dim, time_step):
@@ -361,13 +589,15 @@ def _get_ucb_beta_th(dim, time_step):
 
 def asy_ucb(gp, anc_data):
   beta_th = _get_ucb_beta_th(_get_gp_ucb_dim(gp), anc_data.t)
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ucb', beta=beta_th)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
   gp_eval = _get_gp_eval_for_parallel_strategy(gp, anc_data, 'std')
   def _ucb_acq(x):
     mu, sigma = gp_eval(x)
     return mu + beta_th * sigma
+  if _is_cp_domain(anc_data):
+    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ucb', beta=beta_th), _ucb_acq)
+  if _check_rand_euclidean(anc_data):
+    acq = make_acq_desc('ucb', beta=beta_th)
+    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
   return _delegate_to_reference_maximiser(_ucb_acq, anc_data)
 
 
@@ -380,14 +610,16 @@ def syn_ucb(num_workers, list_of_gps, anc_datas):
 # ---------------------------------------------------------------------------------------------
 def asy_pi(gp, anc_data):
   curr_best = anc_data.curr_max_val
+  gp_eval = _get_gp_eval_for_parallel_strategy(gp, anc_data, 'std')
+  def _pi_acq(x):
+    from scipy.stats import norm as normal_distro
+    mu, sigma = gp_eval(x)
+    return normal_distro.cdf((mu - curr_best) / sigma)
+  if _is_cp_domain(anc_data):
+    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('pi', best=curr_best), _pi_acq)
   if _check_rand_euclidean(anc_data):
     acq = make_acq_desc('pi', best=curr_best)
     return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  from scipy.stats import norm as normal_distro
-  gp_eval = _get_gp_eval_for_parallel_strategy(gp, anc_data, 'std')
-  def _pi_acq(x):
-    mu, sigma = gp_eval(x)
-    return normal_distro.cdf((mu - curr_best) / sigma)
   return _delegate_to_reference_maximiser(_pi_acq, anc_data)
 
 
@@ -397,15 +629,17 @@ def syn_pi(num_workers, list_of_gps, anc_datas):
 
 def asy_ei(gp, anc_data):
   curr_best = anc_data.curr_max_val
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ei', best=curr_best)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  from scipy.stats import norm as normal_distro
   gp_eval = _get_gp_eval_for_parallel_strategy(gp, anc_data, 'std')
   def _ei_acq(x):
+    from scipy.stats import norm as normal_distro
     mu, sigma = gp_eval(x)
     z = (mu - curr_best) / sigma
     return sigma * (z * normal_distro.cdf(z) + normal_distro.pdf(z))
+  if _is_cp_domain(anc_data):
+    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ei', best=curr_best), _ei_acq)
+  if _check_rand_euclidean(anc_data):
+    acq = make_acq_desc('ei', best=curr_best)
+    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
   return _delegate_to_reference_maximiser(_ei_acq, anc_data)
 
 
@@ -419,15 +653,17 @@ def _ttei(gp, anc_data, ref_point):
   ref_mean, ref_std = gp_eval([ref_point])
   ref_mean = float(ref_mean[0])
   ref_std = float(ref_std[0])
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  from scipy.stats import norm as normal_distro
   def _tt_ei_acq(x):
+    from scipy.stats import norm as normal_distro
     mu, sigma = gp_eval(x)
     comb_std = np.sqrt(ref_std ** 2 + sigma ** 2)
     z = (mu - ref_mean) / comb_std
     return comb_std * (z * normal_distro.cdf(z) + normal_distro.pdf(z))
+  if _is_cp_domain(anc_data):
+    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std), _tt_ei_acq)
+  if _check_rand_euclidean(anc_data):
+    acq = make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std)
+    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
   return _delegate_to_reference_maximiser(_tt_ei_acq, anc_data)
 
 

@@ -9,8 +9,9 @@ libdfb200's CUDA kernels evaluate (include/dfb200.h).
 `Kernel.__call__(X1, X2)` (kernel.py:72-83) runs on the GPU through dfb_kernel_matrix.  ESPKernel /
 ESPKernelSE / ESPKernelMatern (kernel.py:671-744) map to the descriptor's ESP form (esp_order > 0).  PolyKernel and
 ExpDecayKernel (kernel.py:331-433) map to the non-stationary factor kinds POLY and EXPDECAY; a descriptor with one of
-them carries kss = NaN, because k(x, x) depends on x.  Kernel types outside the hot-path scope (Hamming, NN kernels, an
-ESP kernel nested in another, Poly / ExpDecay as ESP children, a Poly kernel of non-integer order) raise
+them carries kss = NaN, because k(x, x) depends on x.  HammingKernel (kernel.py:436-457) maps to the HAMMING factor on
+category codes (CategoryCodes); it keeps a descriptor stationary.  Kernel types outside the hot-path scope (NN kernels,
+an ESP kernel nested in another, Poly / ExpDecay / Hamming as ESP children, a Poly kernel of non-integer order) raise
 NotImplementedError: there is no CPU fallback.
 """
 import math
@@ -217,6 +218,87 @@ class ExpDecayKernel(Kernel):
                                                        str(list(self.hyperparams['powers'])))
 
 
+class CategoryCodes(object):
+  """ The value -> code table of one Hamming kernel: categories are compared on the device as small non-negative integer
+      codes (fp64 columns).  Two values get the same code exactly when Python's == calls them equal -- what the
+      reference's np.equal on object arrays does (general_utils.py:139-142) -- so a dict keyed by the value is the
+      table.  It only grows: training rows, candidates and hallucinations all use one table.  NaN is refused (NaN != NaN
+      would make k(x, x) depend on x), and so is an unhashable category. """
+
+  def __init__(self):
+    self.codes = {}
+
+  def encode(self, value):
+    try:
+      is_nan = bool(value != value)
+    except Exception:  # pylint: disable=broad-except
+      is_nan = False
+    if is_nan:
+      raise ValueError('Hamming kernel: a NaN category is not equal to itself (k(x, x) would depend on x).')
+    try:
+      code = self.codes.get(value)
+    except TypeError:
+      raise ValueError('Hamming kernel: category %r is not hashable.' % (value,))
+    if code is None:
+      code = len(self.codes)
+      self.codes[value] = code
+    return code
+
+  def encode_rows(self, X):
+    """ A list of category rows -> (n, d) float64 matrix of codes. """
+    rows = [[self.encode(v) for v in row] for row in X]
+    return np.array(rows, dtype=np.float64).reshape(len(rows), -1)
+
+
+def category_codes(kern):
+  """ The CategoryCodes table of a Hamming kernel -- ours or the reference's object (attached on first use). """
+  table = getattr(kern, 'category_codes', None)
+  if not isinstance(table, CategoryCodes):
+    table = CategoryCodes()
+    kern.category_codes = table
+  return table
+
+
+def hamming_weights(kern):
+  """ dim_weights of a Hamming kernel as float64 (an int weight array compares and sums to the same values). """
+  return np.asarray(kern.hyperparams['dim_weights'], dtype=np.float64).reshape(-1)
+
+
+class HammingKernel(Kernel):
+  """ kernel.py:436-457: sum_q w_q [x_q == y_q] over categorical coordinates (pairwise_hamming_kernel,
+      general_utils.py:113-146).  An int dim_weights d means d uniform weights 1/d.  No scale hyper-parameter. """
+
+  def __init__(self, dim_weights):
+    super(HammingKernel, self).__init__()
+    if isinstance(dim_weights, (int, float)):
+      dim_weights = np.ones((dim_weights,)) / float(dim_weights)
+    dim_weights = np.array(dim_weights)
+    self.set_hyperparams(dim_weights=dim_weights)
+    self.category_codes = CategoryCodes()
+
+  @property
+  def dim(self):
+    return len(self.hyperparams['dim_weights'])
+
+  def is_guaranteed_psd(self):
+    return True
+
+  def _child_evaluate(self, X1, X2):
+    from .device import kernel_matrix
+    table = category_codes(self)
+    return kernel_matrix(self, table.encode_rows(X1), table.encode_rows(X2))
+
+  def __str__(self):
+    return 'Hamming: wts=%s' % (str(list(self.hyperparams['dim_weights'])))
+
+
+def kernel_dim(kern):
+  """ Number of coordinates a kernel acts on; the reference's HammingKernel has no `dim`: its weights count them. """
+  if _kind_of(kern) == 'HammingKernel':
+    return len(kern.hyperparams['dim_weights'])
+  return int(kern.dim)
+
+
 class AdditiveKernel(Kernel):
   """ kernel.py:461-500: scale * sum_g k_g(x[g], y[g]) over non-overlapping groups. """
 
@@ -329,13 +411,14 @@ class _Factor(object):
 def _kind_of(kern):
   """ Duck-typed dispatch on the class name so the reference's own kernel objects work too. """
   names = [c.__name__ for c in type(kern).__mro__]
-  for n in ('SEKernel', 'MaternKernel', 'PolyKernel', 'ExpDecayKernel', 'AdditiveKernel', 'CoordinateProductKernel',
-            'ESPKernel'):
+  for n in ('SEKernel', 'MaternKernel', 'PolyKernel', 'ExpDecayKernel', 'HammingKernel', 'AdditiveKernel',
+            'CoordinateProductKernel', 'ESPKernel'):
     if n in names:
       return n
   raise NotImplementedError(
       'Kernel type %s is outside the GPU hot-path scope (supported: SEKernel, MaternKernel, PolyKernel, ExpDecayKernel, '
-      'AdditiveKernel, CoordinateProductKernel, ESPKernel); there is no CPU fallback.' % (type(kern).__name__))
+      'HammingKernel, AdditiveKernel, CoordinateProductKernel, ESPKernel); there is no CPU fallback.'
+      % (type(kern).__name__))
 
 
 def _nonstationary_factor(kern, kind, train_coords, cand_coords):
@@ -397,6 +480,17 @@ def _expand(kern, train_coords, cand_coords):
     # one factor value each: ExpDecay's offset stays inside its factor, so a product multiplies ((scale k_F) k_D)
     # in CoordinateProductKernel._child_evaluate's order (kernel.py:573-584)
     return 1.0, [(1.0, [_nonstationary_factor(kern, kind, train_coords, cand_coords)])]
+  if kind == 'HammingKernel':
+    # the columns hold category codes (CategoryCodes); the weights ride in the slots, the scale is not read
+    wts = hamming_weights(kern)
+    if len(wts) != len(train_coords):
+      raise ValueError('HammingKernel has %d dim_weights for %d coordinates' % (len(wts), len(train_coords)))
+    f = _Factor()
+    f.train_coords = [int(c) for c in train_coords]
+    f.cand_coords = [int(c) for c in cand_coords]
+    f.kind, f.p, f.scale, f.s8, f.s2, f.gamma_ratio, f.coeffs = _lib.DFB_BASE_HAMMING, 0, 1.0, 0.0, 0.0, 0.0, []
+    f.bandwidths = [float(w) for w in wts]
+    return 1.0, [(1.0, [f])]
   if kind == 'ESPKernel':
     raise NotImplementedError('An ESP kernel inside an additive or product kernel is outside the GPU hot-path scope.')
   if kind == 'AdditiveKernel':
@@ -423,6 +517,9 @@ def _base_at_zero(f):
   """ Base-kernel value at distance 0 in the device's operation order. """
   if f.kind == _lib.DFB_BASE_SE:
     return f.scale * np.exp(-0.0)
+  if f.kind == _lib.DFB_BASE_HAMMING:
+    # every coordinate equal: (np.equal(x, x) * wts).sum(), NumPy's pairwise order
+    return float(np.add.reduce(np.asarray(f.bandwidths, dtype=np.float64)))
   u = 0.0
   for i in range(f.p + 1):
     e = f.p - i
@@ -508,7 +605,7 @@ def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, 
         d.slot_cand_coord[si] = f.cand_coords[q]
         d.slot_bandwidth[si] = f.bandwidths[q]
         si += 1
-      prod = prod * (_base_at_zero(f) if f.kind in (_lib.DFB_BASE_SE, _lib.DFB_BASE_MATERN) else np.nan)
+      prod = prod * (_base_at_zero(f) if f.kind in _STATIONARY_KINDS else np.nan)
       fi += 1
     total = total + prod
   d.term_first_factor[len(terms)] = fi
@@ -522,10 +619,13 @@ def build_descriptor(kern, train_dim=None, cand_coords=None, train_coords=None, 
   return d
 
 
+_STATIONARY_KINDS = (_lib.DFB_BASE_SE, _lib.DFB_BASE_MATERN, _lib.DFB_BASE_HAMMING)
+
+
 def is_stationary(d):
   """ Whether k(x, x) is the same for every x: no factor of the descriptor is POLY or EXPDECAY (api.cu and common.cuh:
       kernel_stationary). """
-  return all(d.factors[f].kind in (_lib.DFB_BASE_SE, _lib.DFB_BASE_MATERN) for f in range(d.n_factors))
+  return all(d.factors[f].kind in _STATIONARY_KINDS for f in range(d.n_factors))
 
 
 def check_esp_descriptor(d):

@@ -82,6 +82,17 @@ extern "C" {
  * A descriptor is stationary when none of its factors is POLY or EXPDECAY; only then is kss meaningful.  The host
  * writes kss = NaN for non-stationary descriptors, and the library never runs the int8 screen or the bound pass of
  * dfb_score_argmax on them (their error model and variance floor rest on a constant k(x, x)).
+ *
+ * One factor kind compares categories (the categorical parts of Cartesian-product domains):
+ *     HAMMING   z = x[coords] (raw: the host's non-negative integer code of each category, stored as fp64),
+ *               slot_bandwidth = the per-coordinate weight w_q >= 0                    general_utils.py:113-146
+ *               b = SUM_q w_q [z_q == z'_q]      each term exactly 0 or w_q, summed in NumPy's pairwise order
+ *                                                (sequential below 8 terms, else 8 interleaved accumulators + tail)
+ *   The factor's scale is 1 and is not read (HammingKernel has no scale).  k(x, x) = SUM_q w_q for every x, so a
+ *   HAMMING factor keeps a descriptor stationary: kss = post_scale * ((pre_scale * k_0(x, x)) * k_1(x, x)) ...
+ *   HammingKernel                : 1 factor; a categorical factor of a CartesianProductKernel (kernel.py:436-457)
+ * HAMMING factors are evaluated by the descriptor interpreter only; the bound pass, dfb_lml_batch and
+ * dfb_lml_gradients refuse them.
  */
 #define DFB_MAX_FACTORS   48
 #define DFB_MAX_TERMS     48
@@ -92,10 +103,11 @@ extern "C" {
 #define DFB_BASE_MATERN    1
 #define DFB_BASE_POLY      2
 #define DFB_BASE_EXPDECAY  3
+#define DFB_BASE_HAMMING   4
 
 typedef struct dfb_factor_desc {
-  int32_t kind;          /* DFB_BASE_SE | DFB_BASE_MATERN | DFB_BASE_POLY | DFB_BASE_EXPDECAY */
-  int32_t p;             /* Matern: nu = p + 1/2 (0 <= p <= DFB_MAX_MATERN_P);  POLY: order;  EXPDECAY: 0 */
+  int32_t kind;          /* DFB_BASE_SE | DFB_BASE_MATERN | DFB_BASE_POLY | DFB_BASE_EXPDECAY | DFB_BASE_HAMMING */
+  int32_t p;             /* Matern: nu = p + 1/2 (0 <= p <= DFB_MAX_MATERN_P);  POLY: order;  EXPDECAY, HAMMING: 0 */
   int32_t n_dims;        /* number of slots of this factor */
   int32_t slot_off;      /* first slot */
   double  scale;         /* SE, POLY, EXPDECAY: scale;  Matern: scale * norm_constant */
@@ -119,7 +131,7 @@ typedef struct dfb_kernel_desc {
   dfb_factor_desc factors[DFB_MAX_FACTORS];
   int32_t slot_train_coord[DFB_MAX_SLOTS];
   int32_t slot_cand_coord[DFB_MAX_SLOTS];
-  double  slot_bandwidth[DFB_MAX_SLOTS];   /* SE / Matern: bandwidth;  POLY: scaling;  EXPDECAY: power */
+  double  slot_bandwidth[DFB_MAX_SLOTS];   /* SE / Matern: bandwidth;  POLY: scaling;  EXPDECAY: power;  HAMMING: weight */
 } dfb_kernel_desc;
 
 /* ---- acquisition descriptor --------------------------------- dragonfly/opt/gpb_acquisitions.py */
@@ -297,6 +309,18 @@ int dfb_ts_argmax(dfb_handle* h, const double* samples_dev, int64_t ld, int32_t 
  * reference's host generation for seeded parity and use this in their throughput mode.)  lo / hi: HOST arrays of d.  */
 int dfb_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int32_t d, const double* lo_host,
                         const double* hi_host, double* out_dev);
+/* dfb_fill_candidates for the flattened rows of a Cartesian-product domain (sample_from_cp_domain_without_constraints,
+ * cp_domain_utils.py:448-489), column s by kinds_host[s], from the same uniform u as dfb_fill_candidates:
+ *   DFB_CAND_REAL        lo[s] + u * (hi[s] - lo[s]), bit for bit what dfb_fill_candidates writes
+ *   DFB_CAND_INTEGER     that value truncated toward zero (.astype(int), oper_utils.py:337-340)
+ *   DFB_CAND_CATEGORICAL a category code uniform on [0, n_levels_host[s]) (lo / hi unread), n_levels >= 1
+ * Rows depend on (seed, global row index) only, as with dfb_fill_candidates.  n_levels_host may be NULL when no column
+ * is categorical.  */
+#define DFB_CAND_REAL        0
+#define DFB_CAND_INTEGER     1
+#define DFB_CAND_CATEGORICAL 2
+int dfb_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int32_t d, const int32_t* kinds_host,
+                              const double* lo_host, const double* hi_host, const int64_t* n_levels_host, double* out_dev);
 
 /* Kernel.__call__(X1, X2) (kernel.py:72-83): the n1 x n2 Gram matrix, device pointers. */
 int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* X1_dev, int64_t n1,
