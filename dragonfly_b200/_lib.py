@@ -74,6 +74,8 @@ PROTOTYPES = {
   'dfb_build_posterior': (C.c_int, [_P, _D, _D, _I32, C.POINTER(_D)]),
   'dfb_lml_batch': (C.c_int, [_P, C.POINTER(KernelDesc), C.POINTER(_D), C.POINTER(_D), _I32, C.POINTER(_D),
                              C.POINTER(_I32)]),
+  'dfb_lml_batch_mixed': (C.c_int, [_P, C.POINTER(KernelDesc), C.POINTER(_D), C.POINTER(_D), _I32, C.POINTER(_D),
+                                   C.POINTER(_I32)]),
   'dfb_extend_posterior': (C.c_int, [_P, _P, _I64, _P, _I32, C.POINTER(_D)]),
   'dfb_restore_posterior': (C.c_int, [_P]),
   'dfb_get_max_diag': (C.c_int, [_P, C.POINTER(_D)]),

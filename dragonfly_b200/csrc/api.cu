@@ -970,8 +970,9 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   return 0;
 }
 
-int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
-                  int32_t B, double* lml_out, int32_t* info_out) {
+// The body of dfb_lml_batch and dfb_lml_batch_mixed: allow_hamming is the one difference.
+static int lml_batch_impl(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var,
+                          const double* mean_const, int32_t B, double* lml_out, int32_t* info_out, bool allow_hamming) {
   DFB_TRY(need(h, true, false, true, false, false));
   if (B < 0 || (B > 0 && (descs == nullptr || noise_var == nullptr || mean_const == nullptr || lml_out == nullptr ||
                           info_out == nullptr))) {
@@ -983,13 +984,17 @@ int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noi
     return -1;
   }
   int ns_max = 1, nf_max = 1;
+  bool any_hamming = false;
   for (int b = 0; b < B; b++) {
     DFB_TRY(check_desc(&descs[b]));
     if (descs[b].esp_order != 0) { set_error("lml_batch: item %d is an ESP kernel", b); return -1; }
     for (int f = 0; f < descs[b].n_factors; f++) {
       if (descs[b].factors[f].kind == DFB_BASE_HAMMING) {
-        set_error("lml_batch: item %d has a HAMMING factor (batched fitting covers Euclidean kernels only)", b);
-        return -1;
+        if (!allow_hamming) {
+          set_error("lml_batch: item %d has a HAMMING factor (dfb_lml_batch_mixed evaluates them)", b);
+          return -1;
+        }
+        any_hamming = true;
       }
     }
     if (descs[b].train_dim != h->d) {
@@ -1035,7 +1040,7 @@ int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noi
     g.ns_max = ns_max; g.nf_max = nf_max;
     g.scratch = scratch; g.item_doubles = item;
     g.red = d_red; g.info = d_info;
-    DFB_TRY(launch_lml_batch(h, g, nb_items));
+    DFB_TRY(launch_lml_batch(h, g, nb_items, any_hamming));
     down.resize(down_bytes);
     DFB_CUDA_OK(cudaMemcpyAsync(down.data(), d_red, down_bytes, cudaMemcpyDeviceToHost, h->stream));
     DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
@@ -1048,6 +1053,16 @@ int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noi
     }
   }
   return 0;
+}
+
+int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
+                  int32_t B, double* lml_out, int32_t* info_out) {
+  return lml_batch_impl(h, descs, noise_var, mean_const, B, lml_out, info_out, false);
+}
+
+int dfb_lml_batch_mixed(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
+                        int32_t B, double* lml_out, int32_t* info_out) {
+  return lml_batch_impl(h, descs, noise_var, mean_const, B, lml_out, info_out, true);
 }
 
 int dfb_restore_posterior(dfb_handle* h);

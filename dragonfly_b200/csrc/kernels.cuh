@@ -113,6 +113,7 @@ struct LmlBatchArgs {
   int* info;                          // [B]: 0, or 1 + the index of the first non-positive pivot
 };
 int64_t lml_batch_item_doubles(int64_t npad, int ns, int nf);
-int launch_lml_batch(dfb_handle* h, const LmlBatchArgs& g, int B);
+// hamming: launch the instantiation that evaluates HAMMING factors (dfb_lml_batch_mixed); without, the Euclidean one
+int launch_lml_batch(dfb_handle* h, const LmlBatchArgs& g, int B, bool hamming);
 
 }  // namespace dfb

@@ -132,9 +132,10 @@ class DevicePosterior(object):
     self.lml = lml.value if info == 0 else None
     return info, self.lml
 
-  def lml_batch(self, descs, noise_vars, mean_consts):
+  def lml_batch(self, descs, noise_vars, mean_consts, mixed=False):
     """ dfb_lml_batch on the training set of set_train (pass the raw Y, mean 0): one LML-only build per item, all in one
-        launch.  Returns (lmls, infos); an item with info > 0 is not positive definite and its lml is NaN. """
+        launch.  Returns (lmls, infos); an item with info > 0 is not positive definite and its lml is NaN.  mixed: call
+        dfb_lml_batch_mixed, which also evaluates HAMMING factors (Cartesian-product kernels with categorical parts). """
     B = len(descs)
     arr = (_lib.KernelDesc * B)(*descs)
     noise = np.ascontiguousarray(noise_vars, dtype=np.float64)
@@ -142,10 +143,11 @@ class DevicePosterior(object):
     assert len(noise) == B and len(mean) == B
     lmls = np.empty(B)
     infos = np.empty(B, dtype=np.int32)
-    _lib.check(self.lib.dfb_lml_batch(self.h, arr, noise.ctypes.data_as(C.POINTER(C.c_double)),
-                                      mean.ctypes.data_as(C.POINTER(C.c_double)), B,
-                                      lmls.ctypes.data_as(C.POINTER(C.c_double)),
-                                      infos.ctypes.data_as(C.POINTER(C.c_int32))), 'dfb_lml_batch')
+    name = 'dfb_lml_batch_mixed' if mixed else 'dfb_lml_batch'
+    _lib.check(getattr(self.lib, name)(self.h, arr, noise.ctypes.data_as(C.POINTER(C.c_double)),
+                                       mean.ctypes.data_as(C.POINTER(C.c_double)), B,
+                                       lmls.ctypes.data_as(C.POINTER(C.c_double)),
+                                       infos.ctypes.data_as(C.POINTER(C.c_int32))), name)
     return lmls, infos
 
   def capacity(self):

@@ -18,7 +18,7 @@ import numpy as np
 
 from . import _lib
 from .kernel import SEKernel, MaternKernel, ExpDecayKernel, AdditiveKernel, CoordinateProductKernel, ESPKernelSE, \
-    ESPKernelMatern, build_descriptor
+    ESPKernelMatern, HammingKernel, CategoryCodes, build_descriptor
 from .gp_core import stable_cholesky_on_device
 
 
@@ -58,12 +58,8 @@ class EuclideanHPLayout(object):
     n += 1 if self.noise_var_type == 'tune' else 0
     return n
 
-  def bounds(self, X, Y, tune_nu=None):
-    """ (cts_hp_bounds, dscr_hp_vals) the way the reference's fitter sets them up from the data
-        (gp_core.py:336-338, 396-416; euclidean_gp.py:253-276): mean value (if tuned), log noise (if tuned),
-        log scale, log bandwidth(s); discrete [0.5, 1.5, 2.5] for a Matern kernel whose nu is tuned
-        (options.matern_nu < 0; default here: tuned iff self.nu is None or negative). """
-    X = np.asarray(X, dtype=np.float64)
+  def _mean_noise_bounds(self, Y):
+    """ (Y_var, [mean bounds]? [log noise bounds]?) as GPFitter._set_up sets them up (gp_core.py:336-338, 396-416). """
     Y = np.asarray(Y, dtype=np.float64)
     Y_var = Y.std() ** 2 + 0.0001 if len(Y) > 0 else 0.0001
     out = []
@@ -75,6 +71,15 @@ class EuclideanHPLayout(object):
       out.append([Y_median - 3 * Y_width, Y_median + 3 * Y_width])
     if self.noise_var_type == 'tune':
       out.append([np.log(0.005 * Y_var), np.log(0.2 * Y_var)])
+    return Y_var, out
+
+  def bounds(self, X, Y, tune_nu=None):
+    """ (cts_hp_bounds, dscr_hp_vals) the way the reference's fitter sets them up from the data
+        (gp_core.py:336-338, 396-416; euclidean_gp.py:253-276): mean value (if tuned), log noise (if tuned),
+        log scale, log bandwidth(s); discrete [0.5, 1.5, 2.5] for a Matern kernel whose nu is tuned
+        (options.matern_nu < 0; default here: tuned iff self.nu is None or negative). """
+    X = np.asarray(X, dtype=np.float64)
+    Y_var, out = self._mean_noise_bounds(Y)
     out.append([np.log(0.1 * Y_var), np.log(10 * Y_var)])
     X_std_norm = np.linalg.norm(X, 'fro') + 1e-4
     single = [np.log(0.01 * X_std_norm), np.log(10 * X_std_norm)]
@@ -248,6 +253,178 @@ class EuclideanMFExpDecayHPLayout(EuclideanMFHPLayout):
     return ExpDecayKernel(self.fidel_dim, 1.0, offset, powers)
 
 
+class CPPart(object):
+  """ One part of a Cartesian-product domain as CPGPFitter sees it: the domain type ('euclidean', 'integral',
+      'prod_discrete_numeric' or 'prod_discrete'), its dimension, the resolved kernel type ('se' / 'matern' for the
+      numeric parts, 'hamming' for prod_discrete), the Matern nu option as given (a float < 0: tuned; 'default': 2.5;
+      > 0: fixed) and the part's same-bandwidth / same-weight flag. """
+
+  NUMERIC = ('euclidean', 'integral', 'prod_discrete_numeric')
+
+  def __init__(self, dom_type, dim, kernel_type, nu='default', same=False):
+    self.dom_type, self.dim, self.kernel_type, self.nu, self.same = dom_type, int(dim), kernel_type, nu, bool(same)
+
+  def nu_tuned(self):
+    """ _set_up_hyperparams_for_domain adds a discrete nu only for a float option < 0 (cartesian_product_gp.py:532). """
+    return self.kernel_type == 'matern' and isinstance(self.nu, float) and self.nu < 0
+
+  def fixed_nu(self):
+    """ The nu a Matern part is built with when it is not tuned; None when that is not a number. """
+    if isinstance(self.nu, str):
+      return 2.5 if self.nu == 'default' else None
+    return self.nu if isinstance(self.nu, (int, float)) and not isinstance(self.nu, bool) else None
+
+
+class CartesianProductHPLayout(EuclideanHPLayout):
+  """ Hyper-parameter vector of the reference's CPGPFitter (cartesian_product_gp.py:325-391, 504-678, 817-945):
+      [mean const]? [log noise]? log kernel scale, then per part in domain order
+        euclidean / integral / prod_discrete_numeric (se, matern): one log bandwidth per dimension;
+        prod_discrete (hamming): none (dim 1 or same weights: 1 / dim each), one linear weight w in [0, 1]
+                                  (dim 2: [w, 1 - w]) or dim linear weights normalised by their sum (dim > 2);
+      one discrete nu in [0.5, 1.5, 2.5] per Matern part whose nu option is a float < 0, in part order.  unpack takes the
+      tuple of discrete hps and returns CartesianProductKernel(scale, [part kernels with scale 1]); its Hamming
+      children carry this layout's CategoryCodes tables, so the rows of encode() and every kernel of a batch share one
+      encoding.  Options the reference itself cannot build with (use_same_bandwidth, an integer or zero Matern nu) and
+      parts outside the device path raise NotImplementedError. """
+
+  def __init__(self, parts, mean_func_type='median', mean_func_const=0.0, noise_var_type='tune', noise_var_label=0.05,
+               noise_var_value=0.1):
+    parts = [p if isinstance(p, CPPart) else CPPart(*p) for p in parts]
+    for p in parts:
+      if p.dom_type in CPPart.NUMERIC:
+        if p.kernel_type not in ('se', 'matern'):
+          raise NotImplementedError('kernel_type %s on a %s part is outside the device path.'
+                                    % (p.kernel_type, p.dom_type))
+        if p.same:
+          raise NotImplementedError('use_same_bandwidth on a Cartesian-product part: the reference raises in '
+                                    '_set_up_dim_bandwidths.')
+        if p.kernel_type == 'matern' and not p.nu_tuned() and not (p.fixed_nu() is not None and p.fixed_nu() > 0):
+          raise NotImplementedError('Matern nu option %r: the reference pops a discrete hp it never set up.' % (p.nu,))
+      elif p.dom_type == 'prod_discrete':
+        if p.kernel_type != 'hamming':
+          raise NotImplementedError('kernel_type %s on a prod_discrete part.' % (p.kernel_type))
+      else:
+        raise NotImplementedError('%s parts are outside the device path.' % (p.dom_type))
+    dim = sum(p.dim for p in parts)
+    super(CartesianProductHPLayout, self).__init__(dim, 'se', mean_func_type=mean_func_type,
+                                                   mean_func_const=mean_func_const, noise_var_type=noise_var_type,
+                                                   noise_var_label=noise_var_label, noise_var_value=noise_var_value)
+    self.kernel_type = 'cartesian_product'
+    self.parts = parts
+    self.codes = [CategoryCodes() if p.dom_type == 'prod_discrete' else None for p in parts]
+
+  @staticmethod
+  def _num_part_hps(p):
+    if p.dom_type != 'prod_discrete':
+      return p.dim
+    if p.same or p.dim == 1:
+      return 0
+    return 1 if p.dim == 2 else p.dim
+
+  def num_hps(self):
+    n = 1 + sum(self._num_part_hps(p) for p in self.parts)
+    n += 1 if self.mean_func_type == 'tune' else 0
+    n += 1 if self.noise_var_type == 'tune' else 0
+    return n
+
+  def num_dscr(self):
+    return sum(p.nu_tuned() for p in self.parts)
+
+  def bounds(self, X, Y, tune_nu=None):
+    """ (cts_hp_bounds, dscr_hp_vals) of CPGPFitter._child_set_up on list-of-parts points X. """
+    cts, dscr, _ = self.bounds_and_order(X, Y)
+    return cts, dscr
+
+  def bounds_and_order(self, X, Y):
+    """ (cts_hp_bounds, dscr_hp_vals, param_order) as CPGPFitter sets them up (gp_core.py:323-350,
+        cartesian_product_gp.py:371-377, 504-678). """
+    Y_var, cts = self._mean_noise_bounds(Y)
+    order = ([['noise_mean', 'cts']] if self.mean_func_type == 'tune' else []) + \
+        ([['noise_var', 'cts']] if self.noise_var_type == 'tune' else [])
+    order.append(['kernel_scale', 'cts'])
+    cts.append([np.log(0.03 * Y_var), np.log(30 * Y_var)])
+    dscr = []
+    for idx, p in enumerate(self.parts):
+      ident = 'dom-%d-%s' % (idx, p.dom_type)
+      if p.dom_type == 'prod_discrete':
+        if p.same or p.dim == 1:
+          continue
+        if p.dim == 2:
+          cts.append([0, 1])
+          order.append([ident + '-hamming_wt-2D', 'cts'])
+        else:
+          cts.extend([[0, 1]] * p.dim)
+          order.extend([['%s-hamming_wts-%d' % (ident, i), 'cts'] for i in range(p.dim)])
+        continue
+      if p.nu_tuned():
+        dscr.append([0.5, 1.5, 2.5])
+        order.append(['%s-matern_nu' % (ident), 'dscr'])
+      if len(X) > 0:
+        part_X = np.array([x[idx] for x in X])
+        diffs = part_X - part_X.mean(axis=0)
+        norms = [np.linalg.norm(diffs[:, i]) + 1e-4 for i in range(p.dim)]
+      else:
+        norms = [1.0] * p.dim
+      cts.extend([[np.log(0.01 * s), np.log(100 * s)] for s in norms])
+      order.extend([['%s-dom_bandwidths-%d' % (ident, i), 'cts'] for i in range(p.dim)])
+    return np.array(cts), dscr, order
+
+  def encode(self, X):
+    """ list-of-parts points -> (n, dim) float64 rows, the parts side by side and every category replaced by its code in
+        the part's table (CartesianProductKernel / flatten_parts layout). """
+    rows = []
+    for x in X:
+      cols = []
+      for part, table in zip(x, self.codes):
+        if table is None:
+          cols.append(np.atleast_1d(np.asarray(part, dtype=np.float64)).reshape(-1))
+        else:
+          cols.append(np.array([table.encode(v) for v in part], dtype=np.float64))
+      rows.append(np.concatenate(cols))
+    return np.ascontiguousarray(np.array(rows, dtype=np.float64).reshape(len(rows), self.dim))
+
+  def unpack(self, hp, Y, nu=None, groupings=None):
+    """ gp_core.py:509-538 + CPGPFitter._child_build_gp / _build_kernel_for_domain (cartesian_product_gp.py:379-391,
+        817-945).  `nu`: the tuple of discrete hps, one per tuned Matern part in part order. """
+    from .cartesian_product_gp import CartesianProductKernel
+    assert groupings is None
+    hp = list(np.asarray(hp, dtype=np.float64))
+    Y = np.asarray(Y, dtype=np.float64)
+    mean_const, noise_var = self._mean_and_noise(hp, Y)
+    dscr = [] if nu is None else list(nu)
+    scale = np.exp(hp[0])
+    hp = np.array(hp[1:])
+    kernels = []
+    for p, table in zip(self.parts, self.codes):
+      if p.dom_type == 'prod_discrete':
+        if p.dim == 1 or p.same:
+          wts = np.ones((p.dim,)) / float(p.dim)
+        elif p.dim == 2:
+          wts = np.array([hp[0], 1 - hp[0]])
+          hp = hp[1:]
+        else:
+          unnorm = np.array(hp[0:p.dim])
+          total = unnorm.sum()
+          wts = unnorm / total if total > 0 else np.ones((p.dim,)) / float(p.dim)
+          hp = hp[p.dim:]
+        kern = HammingKernel(wts)
+        kern.category_codes = table
+      else:
+        bws = np.exp(hp[0:p.dim])
+        hp = hp[p.dim:]
+        if p.kernel_type == 'se':
+          kern = SEKernel(p.dim, 1.0, bws)
+        else:
+          if p.nu_tuned():
+            part_nu, dscr = dscr[0], dscr[1:]
+          else:
+            part_nu = p.fixed_nu()
+          kern = MaternKernel(p.dim, part_nu, 1.0, bws)
+      kernels.append(kern)
+    assert len(hp) == 0 and len(dscr) == 0
+    return float(mean_const), float(noise_var), CartesianProductKernel(scale, kernels)
+
+
 # One LML-only build at N = 5000 is a 40-step dependency chain (chol_diag -> panel -> next column) that leaves most
 # of the GPU idle (7.7 ms for 42 GFLOP); the hp samples are independent, so `lanes` of them are built
 # concurrently -- one DevicePosterior (handle + workspace) per lane, each on its own CUDA stream, driven from its
@@ -326,7 +503,8 @@ LML_BATCH_MAX_N = 512
 
 def lml_batch_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=None):
   """ What lml_for_hyperparams returns, with every LML of a plain (not ESP, not additive) layout on N <= LML_BATCH_MAX_N
-      points from ONE dfb_lml_batch call.  Items that are not positive definite are rebuilt one at a time through
+      points from ONE dfb_lml_batch call (dfb_lml_batch_mixed for a CartesianProductHPLayout, whose kernels have Hamming
+      factors; X is then its encode()d rows).  Items that are not positive definite are rebuilt one at a time through
       stable_cholesky_on_device (its jitter ladder), as lml_for_hyperparams builds them.  Returns (lmls, post). """
   from .device import DevicePosterior
   X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
@@ -348,7 +526,7 @@ def lml_batch_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=Non
     means.append(mean_const)
   if not descs:
     return np.empty(0), post
-  lmls, infos = post.lml_batch(descs, noise, means)
+  lmls, infos = post.lml_batch(descs, noise, means, mixed=isinstance(layout, CartesianProductHPLayout))
   bad = np.nonzero(infos != 0)[0]
   for i in bad:
     post.set_train(X, Y - means[i])
@@ -389,19 +567,26 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   from itertools import product as itertools_product
   from .gp_core import GP, ConstantMean
   from .gpb_acquisitions import map_to_bounds, _reference_fortran_direct_available
+  cp = isinstance(layout, CartesianProductHPLayout)
+  if cp:
+    X_parts = list(X)                                # CPGPFitter's list-of-parts points
+    X = layout.encode(X_parts)
   X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
   Y = np.asarray(Y, dtype=np.float64)
   bounds = np.asarray(cts_hp_bounds, dtype=np.float64)
   dscr_hp_vals = [list(v) for v in dscr_hp_vals]
   additive = bool(getattr(layout, 'use_additive_gp', False))
   esp = getattr(layout, 'kernel_type', None) == 'esp'
-  if len(dscr_hp_vals) > (2 if additive or esp else 1):
+  if not cp and len(dscr_hp_vals) > (2 if additive or esp else 1):
     raise NotImplementedError('Discrete hyper-parameters on the device path: the Matern nu and, for additive '
                               'models, the group size.')
   has_nu = len(dscr_hp_vals) == (2 if additive else 1)       # [nu]? then [group size]? (euclidean_gp.py:226-248)
 
   def kernel_dscr(dscr):
-    """ What unpack / lml_for_hyperparams take per sample: nu (SE / Matern), or the tuple [nu]? [order]? (ESP). """
+    """ What unpack / lml_for_hyperparams take per sample: nu (SE / Matern), the tuple [nu]? [order]? (ESP), or the
+        tuple of every tuned Matern nu (Cartesian product). """
+    if cp:
+      return tuple(dscr)
     if esp:
       return tuple(dscr) if len(dscr) else None
     return dscr[0] if has_nu else None
@@ -412,6 +597,9 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   state = {'post': None}
 
   def lmls_of(hps, nus, groupings=None):
+    if cp:                                           # one dfb_lml_batch_mixed launch per batch up to LML_BATCH_MAX_N
+      vals, state['post'] = lml_batch_for_hyperparams(X, Y, hps, layout, nus=nus, post=state['post'], device=device)
+      return vals
     vals, state['post'] = lml_for_hyperparams(X, Y, hps, layout, nus=nus, post=state['post'], device=device,
                                               groupings=groupings)
     return vals
@@ -420,6 +608,10 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
     if build_gp is not None:                         # e.g. the reference fitter's own build_gp (fit_gp_on_fitter)
       return build_gp(cts, dscr, groupings)
     mean_const, noise_var, kern = layout.unpack(cts, Y, kernel_dscr(dscr), groupings)
+    if cp:
+      from .cartesian_product_gp import CPGP
+      make = CPGP if gp_factory is None else gp_factory
+      return make(X_parts, list(Y), kern, ConstantMean(mean_const), noise_var)
     make = GP if gp_factory is None else gp_factory
     return make(list(X), list(Y), kern, ConstantMean(mean_const), noise_var)
 
@@ -499,6 +691,8 @@ def layout_from_fitter(fitter):
   common = dict(mean_func_type=opt.mean_func_type, mean_func_const=getattr(opt, 'mean_func_const', 0.0),
                 noise_var_type=opt.noise_var_type, noise_var_label=getattr(opt, 'noise_var_label', 0.05),
                 noise_var_value=getattr(opt, 'noise_var_value', 0.1))
+  if hasattr(fitter, 'domain_kernel_ordering') or hasattr(fitter, 'fidel_space'):
+    return _cp_layout_from_fitter(fitter, common)
   if hasattr(fitter, 'fidel_dim') and hasattr(opt, 'fidel_kernel_type'):
     # EuclideanMFGPFitter (euclidean_gp.py:418-716); a 'poly' fidelity or domain kernel stays with the reference,
     # whose fitter raises NotImplementedError for it (:515-519, 587-591, 619-621)
@@ -535,16 +729,67 @@ def layout_from_fitter(fitter):
       num_groups_per_group_size=getattr(opt, 'num_groups_per_group_size', -1))
 
 
+_CP_OPTION_CODES = {'euclidean': 'euc', 'integral': 'int', 'prod_discrete_numeric': 'disc_num', 'prod_discrete': 'disc'}
+_CP_DEFAULT_KERNELS = {'euclidean': 'matern', 'integral': 'matern', 'prod_discrete_numeric': 'matern',
+                       'prod_discrete': 'hamming'}
+
+
+def _cp_layout_from_fitter(fitter, common):
+  """ The CartesianProductHPLayout of a reference CPGPFitter: its domain's parts (fitter.domain.list_of_domains), their
+      kernel types from fitter.domain_kernel_ordering, or the dom_*_kernel_type options when an entry is empty, 'default'
+      resolved by part type (_get_kernel_type_from_options, get_default_kernel_type, cartesian_product_gp.py:188-203,
+      622-634), and the dom_* options of each part.  None for a CPMFGPFitter, precomputed distance lists, additive
+      parts, and anything CartesianProductHPLayout refuses: those fits stay with the reference. """
+  opt = fitter.options
+  domain = getattr(fitter, 'domain', None)
+  ordering = getattr(fitter, 'domain_kernel_ordering', None)
+  if (hasattr(fitter, 'fidel_space') or domain is None or ordering is None or
+      not hasattr(domain, 'list_of_domains') or len(ordering) != len(domain.list_of_domains)):
+    return None
+  if any(d is not None for d in (getattr(fitter, 'domain_lists_of_dists', None) or [])):
+    return None
+  parts = []
+  for dom, kernel_type in zip(domain.list_of_domains, ordering):
+    dom_type = dom.get_type()
+    code = _CP_OPTION_CODES.get(dom_type)
+    if code is None:
+      return None
+    if kernel_type == '' or kernel_type is None:
+      kernel_type = getattr(opt, 'dom_%s_kernel_type' % code, None)
+    if kernel_type == 'default':
+      kernel_type = _CP_DEFAULT_KERNELS[dom_type]
+    if dom_type == 'prod_discrete':
+      parts.append(CPPart(dom_type, dom.get_dim(), kernel_type, same=getattr(opt, 'dom_disc_hamming_use_same_weight',
+                                                                             False)))
+      continue
+    if code in ('euc', 'int') and getattr(opt, 'dom_%s_use_additive_gp' % code, False):
+      return None
+    parts.append(CPPart(dom_type, dom.get_dim(), kernel_type, nu=getattr(opt, 'dom_%s_matern_nu' % code, 'default'),
+                        same=getattr(opt, 'dom_%s_use_same_bandwidth' % code, False)))
+  try:
+    return CartesianProductHPLayout(parts, **common)
+  except NotImplementedError:
+    return None
+
+
 def post_sampling_covers(layout):
   """ The layouts whose 'post_sampling' fits run on the device (post_sampling.post_sample_hps): SE / Matern, not
-      additive; the MF product of SE / Matern fidelity and domain kernels.  ESP and ExpDecay stay with the reference. """
+      additive; the MF product of SE / Matern fidelity and domain kernels; Cartesian products of SE / Matern and Hamming
+      parts without a tuned nu.  ESP and ExpDecay stay with the reference, and so do CP fitters with a tuned nu: the
+      reference's sampler takes hp i as discrete when param_order[i] says so (gp_core.py:689-697), and CPGPFitter lists a
+      part's nu before that part's bandwidths, so its fit fails or samples bandwidths as categories. """
   if type(layout) is EuclideanHPLayout:
     return layout.kernel_type in ('se', 'matern') and not layout.use_additive_gp
+  if type(layout) is CartesianProductHPLayout:
+    return layout.num_dscr() == 0
   return type(layout) is EuclideanMFHPLayout
 
 
 def _fitter_data(fitter, layout):
-  """ The rows the fitter's GPs are built on: [z || x] for an MF fitter. """
+  """ The rows the fitter's GPs are built on: [z || x] for an MF fitter, the list-of-parts points for a CP fitter (the
+      layout encodes them). """
+  if isinstance(layout, CartesianProductHPLayout):
+    return list(fitter.X), np.array(fitter.Y)
   if isinstance(layout, EuclideanMFHPLayout):
     X_mat = np.concatenate((np.asarray(fitter.ZZ, dtype=np.float64).reshape(len(fitter.YY), -1),
                             np.asarray(fitter.XX, dtype=np.float64).reshape(len(fitter.YY), -1)), axis=1)

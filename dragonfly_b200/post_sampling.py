@@ -23,7 +23,7 @@ Without ever-rejected speculation an LML is evaluated once, so the consumed sequ
 """
 import numpy as np
 
-from .hp_grid import lml_batch_for_hyperparams, LML_BATCH_MAX_N
+from .hp_grid import lml_batch_for_hyperparams, LML_BATCH_MAX_N, CartesianProductHPLayout
 
 # Speculation depth where one batch is one dfb_lml_batch launch (N <= LML_BATCH_MAX_N).  Above the cap every LML is a
 # build of its own, so speculation only adds builds: depth 1 there (DESIGN.md 10: 37.7 s against 96.6 s per fit at
@@ -46,8 +46,13 @@ def device_lml_batch(X, Y, layout, has_nu, device=None, batch_fn=lml_batch_for_h
       that is kept across calls. """
   state = {'post': None}
 
+  cp = isinstance(layout, CartesianProductHPLayout)
+
   def lml_batch(cts_rows, dscr_rows):
-    nus = [d[0] for d in dscr_rows] if has_nu else None
+    if cp:                                   # every tuned Matern nu of the product, as one tuple per item
+      nus = [tuple(d) for d in dscr_rows]
+    else:
+      nus = [d[0] for d in dscr_rows] if has_nu else None
     vals, state['post'] = batch_fn(X, Y, np.array(cts_rows), layout, nus=nus, post=state['post'], device=device)
     return vals
   return lml_batch
@@ -265,11 +270,16 @@ def post_sample_hps(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), num_samples=1,
       LMLs of a batch (default: device_lml_batch); `depth` bounds the speculation (default: DEFAULT_DEPTH up to
       LML_BATCH_MAX_N training points, 1 above).  `stats` (PostSamplingStats) and
       `trace` (a list: (hp vector, LML) per consumed LML, in the reference's order) are filled when given.  Returns
-      ('post_fitted_gp', gp, (cts, dscr)) or ('post_sample_hps_with_probs', cts, dscr, [None] * num_samples). """
+      ('post_fitted_gp', gp, (cts, dscr)) or ('post_sample_hps_with_probs', cts, dscr, [None] * num_samples).
+      With a CartesianProductHPLayout X holds CPGPFitter's list-of-parts points (encoded here) and there may be a
+      discrete hp per tuned Matern part: each has its own Metropolis chain, and every LML item gets the whole tuple. """
+  cp = isinstance(layout, CartesianProductHPLayout)
+  if cp:
+    X = layout.encode(X)
   X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
   Y = np.asarray(Y, dtype=np.float64)
   dscr_hp_vals = [list(v) for v in dscr_hp_vals]
-  if len(dscr_hp_vals) > 1:
+  if len(dscr_hp_vals) > 1 and not cp:
     raise NotImplementedError('One discrete hyper-parameter (the Matern nu) on the device path.')
   if lml_batch is None:
     lml_batch = device_lml_batch(X, Y, layout, len(dscr_hp_vals) == 1, device=device)

@@ -91,8 +91,8 @@ extern "C" {
  *   The factor's scale is 1 and is not read (HammingKernel has no scale).  k(x, x) = SUM_q w_q for every x, so a
  *   HAMMING factor keeps a descriptor stationary: kss = post_scale * ((pre_scale * k_0(x, x)) * k_1(x, x)) ...
  *   HammingKernel                : 1 factor; a categorical factor of a CartesianProductKernel (kernel.py:436-457)
- * HAMMING factors are evaluated by the descriptor interpreter only; the bound pass, dfb_lml_batch and
- * dfb_lml_gradients refuse them.
+ * HAMMING factors are evaluated by the descriptor interpreter and by dfb_lml_batch_mixed (the same comparison and sum
+ * on the same staged codes); the bound pass, dfb_lml_batch and dfb_lml_gradients refuse them.
  */
 #define DFB_MAX_FACTORS   48
 #define DFB_MAX_TERMS     48
@@ -209,6 +209,13 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
  * host copy in, one launch, one copy out per batch that fits the scoring chunk buffer; larger B runs as several. */
 int dfb_lml_batch(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
                   int32_t B, double* lml_out, int32_t* info_out);
+/* dfb_lml_batch for kernels with HAMMING factors as well (a CartesianProductKernel over Euclidean, integral, numeric and
+ * categorical parts: CPGPFitter's tuning objective, cartesian_product_gp.py:379-391).  Same arguments, limits and
+ * contract: every item is bit for bit dfb_build_posterior(descs[b], ..., DFB_BUILD_LML_ONLY) on the same data, whatever
+ * else the batch holds.  A batch with a HAMMING factor runs a second instantiation of the batch kernel that compares
+ * category codes; a batch without one runs dfb_lml_batch's kernel. */
+int dfb_lml_batch_mixed(dfb_handle* h, const dfb_kernel_desc* descs, const double* noise_var, const double* mean_const,
+                        int32_t B, double* lml_out, int32_t* info_out);
 /* GP.add_data_multiple (gp_core.py:139-146) and the (N + q)-point factorisation of
  * eval_with_hallucinated_observations (gp_core.py:200-206) WITHOUT the reference's full rebuild: appends q
  * training points (X_new: q x d, y_centred_new: q) to a built posterior and re-derives only the last row block
