@@ -18,7 +18,7 @@ DFB_MAX_MATERN_P = 3
 DFB_BASE_SE, DFB_BASE_MATERN, DFB_BASE_POLY, DFB_BASE_EXPDECAY, DFB_BASE_HAMMING = 0, 1, 2, 3, 4
 DFB_CAND_REAL, DFB_CAND_INTEGER, DFB_CAND_CATEGORICAL = 0, 1, 2
 DFB_DEVICE, DFB_HOST = 0, 1
-DFB_ACQ_MEAN, DFB_ACQ_UCB, DFB_ACQ_EI, DFB_ACQ_PI, DFB_ACQ_TTEI = 0, 1, 2, 3, 4
+DFB_ACQ_MEAN, DFB_ACQ_UCB, DFB_ACQ_EI, DFB_ACQ_PI, DFB_ACQ_TTEI, DFB_ACQ_TS_MARGINAL = 0, 1, 2, 3, 4, 5
 DFB_BUILD_FULL, DFB_BUILD_LML_ONLY, DFB_BUILD_NO_ALPHA = 0, 1, 2
 DFB_EXTEND_SAVE = 16
 DFB_MOO_MAX_OBJ = 8
@@ -87,6 +87,8 @@ PROTOTYPES = {
   'dfb_eval_covar': (C.c_int, [_P, _P, _I64, _I32, _D, _P, _P]),
   'dfb_score_argmax': (C.c_int, [_P, C.POINTER(AcqDesc), _P, _I64, _I32, _I32, _D, _P,
                                  C.POINTER(_D), C.POINTER(_I64)]),
+  'dfb_score_argmax_ts': (C.c_int, [_P, _P, _I64, _I32, _I32, _D, _P, C.c_uint64, _I64, _P, C.POINTER(_D),
+                                    C.POINTER(_I64), C.POINTER(_I64)]),
   'dfb_moo_score_argmax': (C.c_int, [_P, C.POINTER(MooDesc), C.POINTER(_P), C.POINTER(_P), _I64, _P,
                                      C.POINTER(_D), C.POINTER(_I64)]),
   'dfb_kernel_matrix': (C.c_int, [_P, C.POINTER(KernelDesc), _P, _I64, _I32, _P, _I64, _I32, _P]),

@@ -100,8 +100,13 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   // dfb_extend_posterior's snapshot of what it overwrites: the last row block of L, the last block
   // column of L^-T, that block of the y row, alpha
   double* ext_save = c.take<double>((size_t)(2 * TILE + 1) * npad + TILE);
+  // dfb_score_argmax_ts: the normals of the shortlist and of one chunk, and the count of non-positive variances
+  double* list_z = c.take<double>((size_t)SHORTLIST_CAP);
+  double* ts_z = c.take<double>((size_t)chunk);
+  int* ts_nonpos = c.take<int>(4);
   if (h != nullptr && base != nullptr) {
     h->ext_save = ext_save;
+    h->list_z = list_z; h->ts_z = ts_z; h->ts_nonpos = ts_nonpos;
     h->cprep = cprep; h->mu_part = mu_part;
     h->T = T; h->W = W; h->Dinv = Dinv; h->X = X; h->yc = yc; h->alpha = alpha;
     h->tr.xs = tr_xs; h->tr.nrm = tr_nrm; h->te.xs = te_xs; h->te.nrm = te_nrm;
@@ -595,6 +600,11 @@ struct ChunkMode {
   bool allow_small = false;            // dfb_eval of <= SMALL_EVAL_M points: row-streaming kernel instead of the tile GEMM
   bool keep_scores = false;            // leave the scores of a single-chunk pass in h->score (self-check of the shortlist)
   bool keep_best = false;              // continue the running arg-max and best_lb of an earlier pass instead of resetting them
+  // DFB_ACQ_TS_MARGINAL: the pass's m normals in the space of its rows, or NULL for rng_normal(ts_seed, ts_row0 + global
+  // index).  The fp64 passes (use_i8 false) count the non-positive variances into h->ts_nonpos.
+  const double* ts_z = nullptr;
+  uint64_t ts_seed = 0;
+  int64_t ts_row0 = 0;
 };
 constexpr int64_t SMALL_EVAL_M = 32;      // up to four 8-wide passes over W's rows (105 MB each at N = 5000): still ~10x cheaper than one 128-wide tile pass
 
@@ -753,11 +763,26 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
     if (want_std || do_argmax || sc_dev != nullptr) {
       DFB_TRY(prof_begin(h, DFB_PROF_ACQ));
       const int64_t* idx_map = md.idx_map ? md.idx_map + c0 : nullptr;
+      const bool ts = acq.kind == DFB_ACQ_TS_MARGINAL;
+      TsZ tz;
+      memset(&tz, 0, sizeof(tz));
+      if (ts) {
+        if (md.ts_z != nullptr && st.host) {          // host normals: staged chunk by chunk with their rows
+          DFB_CUDA_OK(cudaMemcpyAsync(h->ts_z, md.ts_z + c0, sizeof(double) * mc, cudaMemcpyHostToDevice, h->stream));
+          tz.z = h->ts_z;
+        } else if (md.ts_z != nullptr) {
+          tz.z = md.ts_z + c0;
+        }
+        tz.seed = md.ts_seed; tz.row0 = md.ts_row0;
+        tz.z_out = (tz.z == nullptr && md.collect) ? h->ts_z : nullptr;    // generated normals for the shortlist
+        tz.nonpos = md.use_i8 ? nullptr : h->ts_nonpos;
+      }
       DFB_TRY(launch_acq(h, acq, mu_dev, h->partial, small ? SMALL_EVAL_M : Mc, small ? small_warps : nb, h->kssv, mc,
                          md.idx_base + c0, want_std ? 1 : 0, want_std ? sd_dev : nullptr, sc_dev, do_argmax, idx_map,
-                         md.collect ? &md.em : nullptr));
+                         md.collect ? &md.em : nullptr, ts ? &tz : nullptr));
       if (md.collect)
-        DFB_TRY(launch_collect_shortlist(h, sc_dev, sd_dev, mc, md.idx_base + c0, idx_map, md.em, md.pad, xc_dev, dc));
+        DFB_TRY(launch_collect_shortlist(h, sc_dev, sd_dev, mc, md.idx_base + c0, idx_map, md.em, md.pad, xc_dev, dc,
+                                         ts ? (tz.z != nullptr ? tz.z : h->ts_z) : nullptr));
       DFB_TRY(prof_end(h, DFB_PROF_ACQ, (double)mc));
     }
     if (st.host) {
@@ -1328,22 +1353,20 @@ static int read_best(dfb_handle* h, double* best_score_host, int64_t* best_index
   return 0;
 }
 
-int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m, int32_t dc,
-                     int32_t space, double mean_const, double* scores, double* best_score_host,
-                     int64_t* best_index_host) {
-  if (acq == nullptr) { set_error("acq is NULL"); return -1; }
+// The body of dfb_score_argmax and dfb_score_argmax_ts.  base: the normals of DFB_ACQ_TS_MARGINAL (ChunkMode::ts_*),
+// else default.  TS: every fp64 pass starts h->ts_nonpos from 0, so it ends holding the count of the pass that decided.
+static int score_argmax_impl(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m, int32_t dc,
+                             int32_t space, double mean_const, double* scores, double* best_score_host,
+                             int64_t* best_index_host, const ChunkMode& base) {
   const bool want_std = (acq->kind != DFB_ACQ_MEAN);
-  DFB_TRY(need(h, true, true, true, true, want_std));
-  if (m < 1 || Xc == nullptr) { set_error("bad score arguments (m = %lld)", (long long)m); return -1; }
-  if (acq->kind < DFB_ACQ_MEAN || acq->kind > DFB_ACQ_TTEI) { set_error("unknown acquisition kind %d", acq->kind); return -1; }
-  DFB_CUDA_OK(cudaSetDevice(h->device));
+  const bool ts = acq->kind == DFB_ACQ_TS_MARGINAL;
   ChunkOut out = {nullptr, nullptr, scores};
   const dfb_kernel_desc& desc = active_kernel(h).desc;
   // A caller that asks for the full score vector gets fp64 scores (parity use); the shortlist scheme
   // only guarantees the arg-max, so the int8 pass is reserved for arg-max-only calls unless forced.
   const bool fast = want_std && h->score_impl != 0 && i8_usable(h, desc) &&
                     (scores == nullptr || h->score_impl == 1);
-  ChunkMode exact;                       // the fp64 arg-max
+  ChunkMode exact = base;                // the fp64 arg-max
   exact.want_std = want_std; exact.do_argmax = true;
   ChunkMode md = exact;
   md.use_i8 = fast;
@@ -1362,10 +1385,11 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
     double scale = sk;                    // natural score scale, for the slack only
     if (acq->kind == DFB_ACQ_UCB) scale = (1.0 + fabs(acq->beta)) * sk + fabs(mean_const);
     else if (acq->kind == DFB_ACQ_PI) scale = 1.0;
+    else if (ts) scale = 9.0 * sk + fabs(mean_const);     // UCB's with |z| <= 8 (Box-Muller's on 53-bit uniforms: 8.6)
     md.collect = true;
     md.em.b2 = i8_sigma2_bound(h, desc);
     md.em.kind = acq->kind;
-    md.em.sens = (acq->kind == DFB_ACQ_UCB) ? fabs(acq->beta) : (acq->kind == DFB_ACQ_PI ? 0.25 : 0.4);
+    md.em.sens = (acq->kind == DFB_ACQ_UCB) ? fabs(acq->beta) : (acq->kind == DFB_ACQ_PI ? 0.25 : 0.4);   // TS: |z_i|
     md.pad = 1e-9 * scale;
     DFB_CUDA_OK(cudaMemsetAsync(h->list_count, 0, sizeof(int) * 4, h->stream));
     if (scores == nullptr && bound_pass_applies(h, *acq, desc, m, dc, md.em.b2))
@@ -1384,6 +1408,10 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
       h->last_shortlist = count;
       ChunkMode ex = exact;
       ex.idx_map = h->list_idx; ex.keep_scores = true;
+      if (ts) {
+        ex.ts_z = h->list_z;                         // the normals of the first pass
+        DFB_CUDA_OK(cudaMemsetAsync(h->ts_nonpos, 0, sizeof(int), h->stream));
+      }
       ChunkOut none = {nullptr, nullptr, nullptr};
       DFB_TRY(run_chunks(h, *acq, h->list_X, count, dc, DFB_DEVICE, mean_const, none, ex));
       DFB_TRY(launch_selfcheck(h, h->score, count));
@@ -1395,8 +1423,47 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
       if (chk[0] > 0) need_exact_pass = true;      // the error model failed on a candidate that matters: fp64
     }
   }
-  if (need_exact_pass) DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, exact));
+  if (need_exact_pass) {
+    if (ts) DFB_CUDA_OK(cudaMemsetAsync(h->ts_nonpos, 0, sizeof(int), h->stream));
+    DFB_TRY(run_chunks(h, *acq, Xc, m, dc, space, mean_const, out, exact));
+  }
   return read_best(h, best_score_host, best_index_host);
+}
+
+int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m, int32_t dc,
+                     int32_t space, double mean_const, double* scores, double* best_score_host,
+                     int64_t* best_index_host) {
+  if (acq == nullptr) { set_error("acq is NULL"); return -1; }
+  const bool want_std = (acq->kind != DFB_ACQ_MEAN);
+  DFB_TRY(need(h, true, true, true, true, want_std));
+  if (m < 1 || Xc == nullptr) { set_error("bad score arguments (m = %lld)", (long long)m); return -1; }
+  if (acq->kind < DFB_ACQ_MEAN || acq->kind > DFB_ACQ_TTEI) { set_error("unknown acquisition kind %d", acq->kind); return -1; }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  return score_argmax_impl(h, acq, Xc, m, dc, space, mean_const, scores, best_score_host, best_index_host, ChunkMode());
+}
+
+int dfb_score_argmax_ts(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t space, double mean_const,
+                        const double* z, uint64_t seed, int64_t row0, double* scores, double* best_score_host,
+                        int64_t* best_index_host, int64_t* n_nonpos_host) {
+  DFB_TRY(need(h, true, true, true, true, true));
+  if (m < 1 || Xc == nullptr || row0 < 0 || (space != DFB_HOST && space != DFB_DEVICE)) {
+    set_error("bad score_ts arguments (m = %lld, row0 = %lld)", (long long)m, (long long)row0);
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  dfb_acq_desc acq;
+  memset(&acq, 0, sizeof(acq));
+  acq.kind = DFB_ACQ_TS_MARGINAL;
+  ChunkMode base;
+  base.ts_z = z; base.ts_seed = seed; base.ts_row0 = row0;
+  DFB_TRY(score_argmax_impl(h, &acq, Xc, m, dc, space, mean_const, scores, best_score_host, best_index_host, base));
+  if (n_nonpos_host != nullptr) {
+    int nonpos = 0;
+    DFB_CUDA_OK(cudaMemcpyAsync(&nonpos, h->ts_nonpos, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+    *n_nonpos_host = nonpos;
+  }
+  return 0;
 }
 
 int dfb_moo_score_argmax(dfb_handle* h, const dfb_moo_desc* desc, const double* const* a_dev,

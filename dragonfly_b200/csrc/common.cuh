@@ -141,6 +141,9 @@ struct dfb_handle {
   int* list_count = nullptr;      // [0] entries wanted (> cap = overflow), [1] self-check violations, [2] max ratio x 1e6
   double* list_s8 = nullptr;      // int8-pass score of each shortlist entry
   double* list_err = nullptr;     // its error allowance E_i (< 0: none -- suspect / NaN)
+  double* list_z = nullptr;       // DFB_ACQ_TS_MARGINAL: its normal z_i
+  double* ts_z = nullptr;         // DFB_ACQ_TS_MARGINAL: one chunk of normals (host normals staged, or the generated ones)
+  int* ts_nonpos = nullptr;       // DFB_ACQ_TS_MARGINAL: candidates of the fp64 pass whose sigma^2 is not > 0
   double* blk_lb = nullptr;       // per-block max of (score - E): certain lower bounds of the fp64 maximum
   double* best_lb = nullptr;      // running maximum of those
   // survivor list of the bound pass of dfb_score_argmax (api.cu)

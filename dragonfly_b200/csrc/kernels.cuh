@@ -52,20 +52,32 @@ int launch_copy_pad(dfb_handle* h, const double* src, int64_t n_src, double* dst
 int launch_copy_rows(dfb_handle* h, const double* src, int64_t ld_src, double* dst, int64_t ld_dst,
                      int64_t rows, int64_t cols);
 // Error model of the int8-slice scoring pass handed to the acquisition / shortlist kernels (kernels.cu:
-// i8_score_err): |sigma^2_int8 - sigma^2_fp64| <= b2; sens = |beta| (UCB), 0.4 (EI, TTEI), 0.25 (PI).
+// i8_score_err): |sigma^2_int8 - sigma^2_fp64| <= b2; sens = |beta| (UCB), 0.4 (EI, TTEI), 0.25 (PI), |z_i| (TS).
 struct I8ErrModel {
   double b2;       // a-priori bound on |d sigma^2|; 0 = no int8 pass (no lower-bound tracking)
   double sens;
   int kind;        // DFB_ACQ_*
 };
 constexpr int SHORTLIST_CAP = 4096;
+// The normals of DFB_ACQ_TS_MARGINAL for one chunk (dfb_score_argmax_ts).  z: this chunk's normals on the device, or
+// NULL for the counter-based ones, rng_normal(seed, row0 + the candidate's global index).  z_out (may be NULL): the
+// z of every candidate is written there (the shortlist's source).  nonpos (may be NULL): counts the candidates whose
+// sigma^2 is not > 0.  In I8ErrModel, kind DFB_ACQ_TS_MARGINAL takes sens = |z_i| per candidate.
+struct TsZ {
+  const double* z;
+  uint64_t seed;
+  int64_t row0;
+  double* z_out;
+  int* nonpos;
+};
 int launch_acq(dfb_handle* h, const dfb_acq_desc& acq, const double* mu, const double* partial,
                int64_t ld_partial, int nrb, const double* kss, int64_t m, int64_t idx_base,
                int want_std, double* sd_out, double* score_out, bool do_argmax,
-               const int64_t* idx_map = nullptr, const I8ErrModel* em = nullptr);
+               const int64_t* idx_map = nullptr, const I8ErrModel* em = nullptr, const TsZ* ts = nullptr);
+// z (device, mc values): the chunk's normals when the acquisition is DFB_ACQ_TS_MARGINAL (copied to h->list_z), else NULL
 int launch_collect_shortlist(dfb_handle* h, const double* score, const double* sd, int64_t mc,
                              int64_t idx_base, const int64_t* idx_map, const I8ErrModel& em, double pad, const double* Xc,
-                             int dc);
+                             int dc, const double* z = nullptr);
 // bound pass of dfb_score_argmax (plain kernels): keeps the m candidates Xc (device) whose acquisition at
 // (mu_bar, sqrt(k**)) reaches *best_lb - pad, mu_bar a certified upper bound of mu, and appends them (x rows, global
 // index idx_base + row) to the survivor list in row order; m <= h->keep_cap.  mu_ub non-NULL: writes mu_bar instead

@@ -247,6 +247,37 @@ class DevicePosterior(object):
         C.byref(bi)), 'dfb_score_argmax')
     return bs.value, bi.value, sc
 
+  def score_argmax_ts(self, Xc, mean_const=0.0, z=None, seed=0, row0=0, want_scores=False):
+    """ dfb_score_argmax_ts: one marginal posterior draw per candidate, mu_i + sqrt(sigma^2_i) z_i, and its arg-max.
+        z: the m normals, kept in the memory space of Xc (host ndarray for a host Xc, CUDA tensor for a CUDA one), or None
+        for the device's counter-based normals of (seed, row0 + row).  Returns (best_score, best_index, scores or None,
+        the number of candidates whose variance is not > 0). """
+    bs, bi, nonpos = C.c_double(0.0), C.c_int64(-1), C.c_int64(0)
+    seed = C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF)
+    if isinstance(Xc, torch.Tensor):
+      Xd = _dev_f64(Xc, self.device)
+      m, dc = int(Xd.shape[0]), int(Xd.shape[1])
+      zd = None if z is None else _dev_f64(z, self.device).reshape(-1)
+      assert zd is None or int(zd.shape[0]) == m
+      sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
+      _lib.check(self.lib.dfb_score_argmax_ts(
+          self.h, C.c_void_p(Xd.data_ptr()), m, dc, _lib.DFB_DEVICE, float(mean_const),
+          None if zd is None else C.c_void_p(zd.data_ptr()), seed, int(row0),
+          C.c_void_p(sc.data_ptr()) if want_scores else None, C.byref(bs), C.byref(bi), C.byref(nonpos)),
+          'dfb_score_argmax_ts')
+      return bs.value, bi.value, sc, nonpos.value
+    Xh = np.ascontiguousarray(np.asarray(Xc, dtype=np.float64))
+    m, dc = Xh.shape
+    zh = None if z is None else np.ascontiguousarray(np.asarray(z, dtype=np.float64).reshape(-1))
+    assert zh is None or len(zh) == m
+    sc = np.empty((m,), dtype=np.float64) if want_scores else None
+    _lib.check(self.lib.dfb_score_argmax_ts(
+        self.h, Xh.ctypes.data_as(C.c_void_p), m, dc, _lib.DFB_HOST, float(mean_const),
+        None if zh is None else zh.ctypes.data_as(C.c_void_p), seed, int(row0),
+        sc.ctypes.data_as(C.c_void_p) if want_scores else None, C.byref(bs), C.byref(bi), C.byref(nonpos)),
+        'dfb_score_argmax_ts')
+    return bs.value, bi.value, sc, nonpos.value
+
   # -- joint posterior over one block: covariance and Thompson draws -----------------------------
   TS_BLOCK = 4096
 

@@ -741,10 +741,64 @@ def asy_ts(gp, anc_data):
   if anc_data.acq_opt_method != 'rand':
     anc_data.acq_opt_method = 'rand'
     anc_data.max_evals = 4 * anc_data.max_evals
+  if _is_cp_domain(anc_data):
+    return _cp_ts(gp, anc_data)
   halluc = _halluc_points(anc_data)
   rand_pts = draw_candidates(anc_data.domain.bounds, anc_data.max_evals)
   sample = _draw_one_sample(gp, rand_pts, halluc)
   return rand_pts[_argmax_of_sharded_sample(sample)]
+
+
+def _cp_ts(gp, anc_data):
+  """ asy_ts on a CP domain (anc_data already forced to 'rand').  The reference's vectorised objective is called one
+      point at a time there (exd_utils.py:247-274), so each candidate gets its own 1 x 1 draw: sqrt(sigma^2) z + mu with
+      one np.random.normal(size=(1, 1)) per candidate, in candidate order (gp_core.py:250-261, general_utils.py:224-232).
+      Legacy NumPy draws normals in pairs and caches the second, so np.random.normal(size=M) after the candidates gives
+      the same M normals and leaves the stream where the M one-normal calls leave it.  Every candidate is scored in
+      fused device slabs (dfb_score_argmax_ts) and the arg-max follows np.argmax.  candidate_rng 'device' generates the
+      rows (dfb_fill_mixed_candidates) and the normals (in the scoring kernel) from one seed drawn as _cp_fused_maximise
+      draws it.  A candidate whose variance is not > 0 raises ValueError, as the reference's stable_cholesky does. """
+  from . import dist as dfb_dist
+  if getattr(anc_data, 'is_mf', False) or hasattr(gp, 'fidel_space_kernel') or hasattr(gp, 'mfgp'):
+    raise NotImplementedError('Thompson sampling with a multi-fidelity GP on a Cartesian-product domain is outside the '
+                              'GPU hot-path scope.')
+  parts = _cp_parts(anc_data.domain, gp.kernel)
+  if _shard_info()[1] > 1:
+    raise NotImplementedError('Cartesian-product candidate draws are not sharded across ranks.')
+  mode = getattr(anc_data, 'candidate_rng', None) or CANDIDATE_RNG
+  if mode not in ('numpy', 'device'):
+    raise ValueError("candidate_rng should be 'numpy' or 'device'.")
+  M = int(anc_data.max_evals)
+  if mode == 'device':
+    seed = (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
+  else:
+    rows, draws = draw_cp_candidates(parts, M)
+    z = np.random.normal(size=M)
+  nonpos = 0
+  with gp._fused_session(None, _halluc_points(anc_data)) as sess:
+    slab = sess.slab_rows(2 * STREAM_SLAB_ROWS if mode == 'device' else STREAM_SLAB_ROWS)
+    layout = _cp_device_layout(parts) if mode == 'device' else None
+    best_s, best_i, buf = 0.0, -1, None
+    for r0 in range(0, M, slab):
+      m = min(slab, M - r0)
+      if mode == 'device':
+        buf = _cp_device_rows(sess, seed, r0, m, layout, out=None if buf is None else buf[:m])
+        res = sess.score_ts(buf, seed=seed, row0=r0)
+      else:
+        res = sess.score_ts(rows[r0:r0 + m], z=z[r0:r0 + m])
+      nonpos += int(res[3])
+      s, gi = float(res[0]), r0 + int(res[1])
+      if dfb_dist.better(s, gi, best_s, best_i):
+        best_s, best_i = s, gi
+    if nonpos > 0:
+      raise ValueError('Could not compute Cholesky decomposition despite adding jitter to the diagonal: the posterior '
+                       'variance of %d candidate(s) is not positive. This is likely because the M is not positive '
+                       'semi-definite or has infinities/nans.' % (nonpos))
+    if mode == 'device':
+      kinds, bounds, n_levels, _ = layout
+      row = sess.post.fill_mixed_candidates(seed, best_i, 1, kinds, bounds, n_levels).cpu().numpy()[0]
+      return _cp_point_from_device_row(parts, row)
+  return point_from_draws(parts, draws, best_i)
 
 
 def _ts_block(gp):

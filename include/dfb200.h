@@ -140,6 +140,7 @@ typedef struct dfb_kernel_desc {
 #define DFB_ACQ_EI    2   /* sigma (z Phi(z) + phi(z)), z=(mu-best)/sigma :247-260                */
 #define DFB_ACQ_PI    3   /* Phi((mu - best)/sigma)                       :230-238                */
 #define DFB_ACQ_TTEI  4   /* EI against a reference arm (ref_mean, ref_std) :269-279              */
+#define DFB_ACQ_TS_MARGINAL 5   /* mu_i + sqrt(sigma^2_i) z_i, one normal z_i per candidate: dfb_score_argmax_ts only */
 
 typedef struct dfb_acq_desc {
   int32_t kind;
@@ -285,6 +286,23 @@ int dfb_eval_covar(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, d
 int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, int64_t m,
                      int32_t dc, int32_t space, double mean_const, double* scores,
                      double* best_score_host, int64_t* best_index_host);
+
+/* Thompson sampling on Cartesian-product domains (asy_ts, gpb_acquisitions.py:119-127, with the `rand` maximiser of
+ * _rand_maximise_vectorised_objective_in_cp_domain, exd_utils.py:247-274): the reference calls gp.draw_samples(1, [x])
+ * (gp_core.py:250-254; draw_gaussian_samples, general_utils.py:224-232) once per candidate -- a 1 x 1 covariance, its
+ * Cholesky factor sqrt(sigma^2) and one normal -- and takes np.argmax of the values.  Each candidate's draw is
+ * independent of the others, so this is dfb_score_argmax with the acquisition DFB_ACQ_TS_MARGINAL:
+ *     score_i = fl(fl(sqrt(sigma^2_i) * z_i) + mu_i)          (no FMA contraction)
+ * z (m values, in the space of Xc) holds the caller's normals (np.random.normal(size=m) for seeded parity).  z = NULL:
+ * the kernel generates them, z_i = element (0, row0 + i) of dfb_fill_rng(seed, ..., DFB_RNG_NORMAL), so a candidate's
+ * normal depends on (seed, its global row) only.  The int8 screen applies with UCB's allowance, |z_i| in place of
+ * |beta|; the bound pass (option "prune") does not run for this kind.  *n_nonpos_host (may be NULL) receives the
+ * number of candidates whose fp64 sigma^2 is not > 0, NaN included: the reference's stable_cholesky raises there
+ * (general_utils.py:183-203).  Their scores follow the usual NaN rules.  scores, best_score_host and best_index_host
+ * as for dfb_score_argmax.  */
+int dfb_score_argmax_ts(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t space, double mean_const,
+                        const double* z, uint64_t seed, int64_t row0, double* scores, double* best_score_host,
+                        int64_t* best_index_host, int64_t* n_nonpos_host);
 
 /* The multi-objective acquisitions' scalarisation + random_maximise's arg-max (np.argmax order) over m
  * candidates that n_obj GPs have already scored with dfb_eval on the device: a_dev[k] = mu_k (UCB kinds) or the
