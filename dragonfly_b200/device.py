@@ -205,46 +205,38 @@ class DevicePosterior(object):
     torch.cuda.synchronize(self.device)
 
   # -- prediction ---------------------------------------------------------------------------------
+  def _operands(self, Xc, z=None):
+    """ Candidate rows Xc (and normals z) as the scoring calls take them: (X, z, DFB_HOST or DFB_DEVICE, ptr, vec).
+        A host Xc stays on the host (the C call copies it) with host outputs, a CUDA tensor stays on the device with
+        CUDA outputs.  A C-contiguous float64 host array is used as is, not copied: page-locked slabs must stay
+        page-locked to take the double-buffered copies.  ptr(a) is the C pointer of X, z or an output (NULL for None);
+        vec() allocates one output vector of len(X) in the same memory space. """
+    if isinstance(Xc, torch.Tensor):
+      X = _dev_f64(Xc, self.device)
+      z = None if z is None else _dev_f64(z, self.device).reshape(-1)
+      vec = lambda: torch.empty((int(X.shape[0]),), dtype=torch.float64, device=self.device)
+      return X, z, _lib.DFB_DEVICE, lambda a: None if a is None else C.c_void_p(a.data_ptr()), vec
+    X = np.ascontiguousarray(np.asarray(Xc, dtype=np.float64))
+    z = None if z is None else np.ascontiguousarray(np.asarray(z, dtype=np.float64).reshape(-1))
+    vec = lambda: np.empty((X.shape[0],), dtype=np.float64)
+    return X, z, _lib.DFB_HOST, lambda a: None if a is None else a.ctypes.data_as(C.c_void_p), vec
+
   def eval(self, Xc, mean_const=0.0, want_std=True):
     """ Xc: host ndarray (results are host ndarrays, copies inside the C call) or CUDA tensor
         (results are CUDA tensors).  Returns (mu, sd or None). """
-    if isinstance(Xc, torch.Tensor):
-      Xd = _dev_f64(Xc, self.device)
-      m, dc = int(Xd.shape[0]), int(Xd.shape[1])
-      mu = torch.empty((m,), dtype=torch.float64, device=self.device)
-      sd = torch.empty((m,), dtype=torch.float64, device=self.device) if want_std else None
-      _lib.check(self.lib.dfb_eval(self.h, C.c_void_p(Xd.data_ptr()), m, dc, _lib.DFB_DEVICE,
-                                   float(mean_const), C.c_void_p(mu.data_ptr()),
-                                   C.c_void_p(sd.data_ptr()) if want_std else None), 'dfb_eval')
-      return mu, sd
-    Xh = np.ascontiguousarray(np.asarray(Xc, dtype=np.float64))
-    m, dc = Xh.shape
-    mu = np.empty((m,), dtype=np.float64)
-    sd = np.empty((m,), dtype=np.float64) if want_std else None
-    _lib.check(self.lib.dfb_eval(self.h, Xh.ctypes.data_as(C.c_void_p), m, dc, _lib.DFB_HOST,
-                                 float(mean_const), mu.ctypes.data_as(C.c_void_p),
-                                 sd.ctypes.data_as(C.c_void_p) if want_std else None), 'dfb_eval')
+    X, _, space, ptr, vec = self._operands(Xc)
+    mu, sd = vec(), (vec() if want_std else None)
+    _lib.check(self.lib.dfb_eval(self.h, ptr(X), int(X.shape[0]), int(X.shape[1]), space, float(mean_const), ptr(mu),
+                                 ptr(sd)), 'dfb_eval')
     return mu, sd
 
   def score_argmax(self, acq_desc, Xc, mean_const=0.0, want_scores=False):
     """ Fused scoring + arg-max.  Returns (best_score, best_index, scores or None). """
     bs, bi = C.c_double(0.0), C.c_int64(-1)
-    if isinstance(Xc, torch.Tensor):
-      Xd = _dev_f64(Xc, self.device)
-      m, dc = int(Xd.shape[0]), int(Xd.shape[1])
-      sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
-      _lib.check(self.lib.dfb_score_argmax(
-          self.h, C.byref(acq_desc), C.c_void_p(Xd.data_ptr()), m, dc, _lib.DFB_DEVICE,
-          float(mean_const), C.c_void_p(sc.data_ptr()) if want_scores else None, C.byref(bs),
-          C.byref(bi)), 'dfb_score_argmax')
-      return bs.value, bi.value, sc
-    Xh = np.ascontiguousarray(np.asarray(Xc, dtype=np.float64))
-    m, dc = Xh.shape
-    sc = np.empty((m,), dtype=np.float64) if want_scores else None
-    _lib.check(self.lib.dfb_score_argmax(
-        self.h, C.byref(acq_desc), Xh.ctypes.data_as(C.c_void_p), m, dc, _lib.DFB_HOST,
-        float(mean_const), sc.ctypes.data_as(C.c_void_p) if want_scores else None, C.byref(bs),
-        C.byref(bi)), 'dfb_score_argmax')
+    X, _, space, ptr, vec = self._operands(Xc)
+    sc = vec() if want_scores else None
+    _lib.check(self.lib.dfb_score_argmax(self.h, C.byref(acq_desc), ptr(X), int(X.shape[0]), int(X.shape[1]), space,
+                                         float(mean_const), ptr(sc), C.byref(bs), C.byref(bi)), 'dfb_score_argmax')
     return bs.value, bi.value, sc
 
   def score_argmax_ts(self, Xc, mean_const=0.0, z=None, seed=0, row0=0, want_scores=False):
@@ -253,28 +245,12 @@ class DevicePosterior(object):
         for the device's counter-based normals of (seed, row0 + row).  Returns (best_score, best_index, scores or None,
         the number of candidates whose variance is not > 0). """
     bs, bi, nonpos = C.c_double(0.0), C.c_int64(-1), C.c_int64(0)
-    seed = C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF)
-    if isinstance(Xc, torch.Tensor):
-      Xd = _dev_f64(Xc, self.device)
-      m, dc = int(Xd.shape[0]), int(Xd.shape[1])
-      zd = None if z is None else _dev_f64(z, self.device).reshape(-1)
-      assert zd is None or int(zd.shape[0]) == m
-      sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
-      _lib.check(self.lib.dfb_score_argmax_ts(
-          self.h, C.c_void_p(Xd.data_ptr()), m, dc, _lib.DFB_DEVICE, float(mean_const),
-          None if zd is None else C.c_void_p(zd.data_ptr()), seed, int(row0),
-          C.c_void_p(sc.data_ptr()) if want_scores else None, C.byref(bs), C.byref(bi), C.byref(nonpos)),
-          'dfb_score_argmax_ts')
-      return bs.value, bi.value, sc, nonpos.value
-    Xh = np.ascontiguousarray(np.asarray(Xc, dtype=np.float64))
-    m, dc = Xh.shape
-    zh = None if z is None else np.ascontiguousarray(np.asarray(z, dtype=np.float64).reshape(-1))
-    assert zh is None or len(zh) == m
-    sc = np.empty((m,), dtype=np.float64) if want_scores else None
+    X, z, space, ptr, vec = self._operands(Xc, z)
+    assert z is None or int(z.shape[0]) == int(X.shape[0])
+    sc = vec() if want_scores else None
     _lib.check(self.lib.dfb_score_argmax_ts(
-        self.h, Xh.ctypes.data_as(C.c_void_p), m, dc, _lib.DFB_HOST, float(mean_const),
-        None if zh is None else zh.ctypes.data_as(C.c_void_p), seed, int(row0),
-        sc.ctypes.data_as(C.c_void_p) if want_scores else None, C.byref(bs), C.byref(bi), C.byref(nonpos)),
+        self.h, ptr(X), int(X.shape[0]), int(X.shape[1]), space, float(mean_const), ptr(z),
+        C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), int(row0), ptr(sc), C.byref(bs), C.byref(bi), C.byref(nonpos)),
         'dfb_score_argmax_ts')
     return bs.value, bi.value, sc, nonpos.value
 

@@ -130,24 +130,23 @@ class _FusedSession(object):
   def __init__(self, gp, post, acq, mean_const):
     self.gp, self.post, self.acq, self.mean_const = gp, post, acq, mean_const
 
-  def score(self, pts, want_scores=False):
-    """ dfb_score_argmax over one slab: (best_score, best_index within the slab, scores or None). """
+  def _slab(self, pts):
+    """ (candidate matrix, mean constant) of one slab; raises if the mean is not a constant on the candidates. """
     mc = self.gp._mean_const_for(pts) if self.mean_const is None else self.mean_const
     if mc is None:
       raise NotImplementedError('Fused acquisition scoring needs a mean function that is constant on the '
                                 'candidates (what GPFitter.build_gp produces, gp_core.py:527-530).')
-    return self.post.score_argmax(self.acq, self.gp._test_matrix(pts), mean_const=mc, want_scores=want_scores)
+    return self.gp._test_matrix(pts), mc
+
+  def score(self, pts, want_scores=False):
+    """ dfb_score_argmax over one slab: (best_score, best_index within the slab, scores or None). """
+    return self.post.score_argmax(self.acq, *self._slab(pts), want_scores=want_scores)
 
   def score_ts(self, pts, z=None, seed=0, row0=0, want_scores=False):
     """ dfb_score_argmax_ts over one slab: one marginal posterior draw per candidate (the session's acq is not used),
         with the normals z (same memory space as pts) or the device's counter-based normals of (seed, row0 + row).
         Returns (best_score, best_index within the slab, scores or None, count of variances that are not > 0). """
-    mc = self.gp._mean_const_for(pts) if self.mean_const is None else self.mean_const
-    if mc is None:
-      raise NotImplementedError('Fused acquisition scoring needs a mean function that is constant on the '
-                                'candidates (what GPFitter.build_gp produces, gp_core.py:527-530).')
-    return self.post.score_argmax_ts(self.gp._test_matrix(pts), mean_const=mc, z=z, seed=seed, row0=row0,
-                                     want_scores=want_scores)
+    return self.post.score_argmax_ts(*self._slab(pts), z=z, seed=seed, row0=row0, want_scores=want_scores)
 
   def slab_rows(self, target):
     """ Rows per streamed slab: a whole number of the handle's scoring chunks (no ragged chunk inside a slab). """

@@ -198,39 +198,42 @@ def _cp_fused_maximise(gp, anc_data, acq):
       exd_utils.py:247-274): the reference scores its sampled points one gp.eval at a time; here every candidate is
       scored in fused device slabs and the arg-max follows np.argmax over the per-point values (first index on ties).
       candidate_rng 'numpy' draws the reference's points (draw_cp_candidates), 'device' draws them with
-      dfb_fill_mixed_candidates keyed by (seed, global row, column). """
-  from . import dist as dfb_dist
+      dfb_fill_mixed_candidates keyed by (seed, global row, column).  acq None scores Thompson sampling's marginal draws
+      instead (_cp_ts): with the normals drawn right after the reference's points, or the device's normals of the seed. """
   parts = _cp_parts(anc_data.domain, gp.kernel)
   if _shard_info()[1] > 1:
     raise NotImplementedError('Cartesian-product candidate draws are not sharded across ranks.')
-  mode = getattr(anc_data, 'candidate_rng', None) or CANDIDATE_RNG
-  if mode not in ('numpy', 'device'):
-    raise ValueError("candidate_rng should be 'numpy' or 'device'.")
+  mode = _candidate_rng(anc_data)
   M = int(anc_data.max_evals)
-  if mode == 'device':
-    seed = (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
-  else:
-    rows, draws = draw_cp_candidates(parts, M)
   with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
-    slab = sess.slab_rows(2 * STREAM_SLAB_ROWS if mode == 'device' else STREAM_SLAB_ROWS)
-    layout = _cp_device_layout(parts) if mode == 'device' else None
-    best_s, best_i, buf = 0.0, -1, None
-    for r0 in range(0, M, slab):
-      m = min(slab, M - r0)
-      if mode == 'device':
-        buf = _cp_device_rows(sess, seed, r0, m, layout, out=None if buf is None else buf[:m])
-        pts = buf
-      else:
-        pts = rows[r0:r0 + m]
-      res = sess.score(pts)
-      s, gi = float(res[0]), r0 + int(res[1])
-      if dfb_dist.better(s, gi, best_s, best_i):
-        best_s, best_i = s, gi
     if mode == 'device':
+      seed = _device_seed()
+      layout = _cp_device_layout(parts)
       kinds, bounds, n_levels, _ = layout
-      row = sess.post.fill_mixed_candidates(seed, best_i, 1, kinds, bounds, n_levels).cpu().numpy()[0]
-      return _cp_point_from_device_row(parts, row)
-  return point_from_draws(parts, draws, best_i)
+      source = _IndexedRows(
+          sess.slab_rows(2 * STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: _cp_device_rows(sess, seed, r0, m, layout, out),
+          lambda i: _cp_point_from_device_row(
+              parts, sess.post.fill_mixed_candidates(seed, i, 1, kinds, bounds, n_levels).cpu().numpy()[0]))
+    else:
+      rows, draws = draw_cp_candidates(parts, M)
+      source = _IndexedRows(sess.slab_rows(STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: rows[r0:r0 + m],
+                            lambda i: point_from_draws(parts, draws, i))
+    if acq is not None:
+      return source.point(*_slab_argmax(source, lambda pts, r0: sess.score(pts)))
+    z = np.random.normal(size=M) if mode == 'numpy' else None
+    nonpos = 0
+
+    def score_ts(pts, r0):
+      nonlocal nonpos
+      res = sess.score_ts(pts, seed=seed, row0=r0) if z is None else sess.score_ts(pts, z=z[r0:r0 + len(pts)])
+      nonpos += int(res[3])
+      return res
+    best = _slab_argmax(source, score_ts)
+    if nonpos > 0:
+      raise ValueError('Could not compute Cholesky decomposition despite adding jitter to the diagonal: the posterior '
+                       'variance of %d candidate(s) is not positive. This is likely because the M is not positive '
+                       'semi-definite or has infinities/nans.' % (nonpos))
+    return source.point(*best)
 
 
 def _cp_other_maximiser(acq_fn, anc_data):
@@ -353,122 +356,171 @@ def _slab_schedule(max_evals, slab, unit):
   return starts
 
 
-def _maximise_streamed(score, bounds, max_evals, slab, unit=0):
-  """ random_maximise (oper_utils.py:70-80) with the candidate draw pipelined against the scoring.
-      score(pts) -> (best_score, best_index_within_pts, ...).  np.random.random((M, d)) and consecutive
-      np.random.random((m_k, d)) slabs consume the MT19937 stream identically (row-major fill), so the candidates
-      -- and the state the global RNG is left in -- are the reference's.  `unit` = rows of one scoring chunk. """
-  import queue
-  import threading
-  from . import dist as dfb_dist
-  M, dim = int(max_evals), len(bounds)
-  rank, world, dev = _shard_info()
-  lo_r, hi_r = dfb_dist.shard_bounds(M, rank, world) if world > 1 else (0, M)
-  starts = _slab_schedule(M, slab, unit) if M > 0 else []
-  q = queue.Queue(maxsize=2)
-  bnds = np.asarray(bounds, dtype=np.float64)
-  width, low = bnds[:, 1] - bnds[:, 0], bnds[:, 0]
-  # staging buffers sized by the largest slab actually scheduled (never by the nominal slab size), and only while they
-  # stay modest: 4 x 256 MB at most
-  rows_max = max([r for _, r in starts] or [0])
-  pinned = _pinned_slab_buffers(rows_max, dim) if (len(starts) > 1 and rows_max * dim * 8 <= (256 << 20)) else None
-
-  def _producer():
-    try:
-      for k, (r0, rows) in enumerate(starts):
-        raw = np.random.random((rows, dim))
-        if not min(hi_r, r0 + rows) > max(lo_r, r0):
-          q.put((r0, None))                            # another rank's rows: drawn (the stream must advance), not mapped
-          continue
-        if pinned is not None:
-          pts = pinned[k % len(pinned)][:rows]
-          np.multiply(raw, width, out=pts)             # map_to_bounds: pts * (hi - lo) + lo, written in place
-          np.add(pts, low, out=pts)
-        else:
-          pts = raw * width + low
-        q.put((r0, pts))
-    except BaseException as exc:  # pylint: disable=broad-except
-      q.put(exc)
-
-  if len(starts) > 1:
-    th = threading.Thread(target=_producer, daemon=True)
-    th.start()
-  else:
-    th = None
-    _producer()
-  best_s, best_i, best_pt, err = 0.0, -1, None, None
-  for _ in starts:
-    item = q.get()
-    if isinstance(item, BaseException):
-      err = item
-      break
-    if err is not None:
-      continue            # keep draining: the global RNG must end where the reference leaves it
-    r0, pts = item
-    if pts is None:
-      continue
-    a, b = max(lo_r, r0), min(hi_r, r0 + len(pts))
-    if b <= a:
-      continue
-    try:
-      res = score(pts[a - r0:b - r0])
-    except BaseException as exc:  # pylint: disable=broad-except
-      err = exc
-      continue
-    s, gi = float(res[0]), a + int(res[1])
-    if dfb_dist.better(s, gi, best_s, best_i):
-      best_s, best_i, best_pt = s, gi, np.array(pts[gi - r0], dtype=np.float64)
-  if th is not None:
-    th.join()
-  if err is not None:
-    raise err
-  if world > 1:
-    best_s, best_i, best_pt = dfb_dist.all_reduce_argmax_point(best_s, best_i, best_pt, dim, device=dev)
-  return best_pt
-
-
-def _maximise_device_candidates(session, bounds, max_evals):
-  """ Throughput mode of the `rand` maximiser: candidates generated on the device by global row index. """
-  from . import dist as dfb_dist
-  M = int(max_evals)
-  seed = (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
-  rank, world, dev = _shard_info()
-  lo_r, hi_r = dfb_dist.shard_bounds(M, rank, world) if world > 1 else (0, M)
-  slab = session.slab_rows(2 * STREAM_SLAB_ROWS)
-  best_s, best_i, buf = 0.0, -1, None
-  for r0 in range(lo_r, hi_r, slab):
-    m = min(slab, hi_r - r0)
-    if buf is None:
-      buf = session.post.fill_candidates(seed, r0, m, bounds)
-      pts = buf
-    else:
-      pts = session.post.fill_candidates(seed, r0, m, bounds, out=buf[:m])
-    res = session.score(pts)
-    s, gi = float(res[0]), r0 + int(res[1])
-    if dfb_dist.better(s, gi, best_s, best_i):
-      best_s, best_i = s, gi
-  if world > 1:
-    best_s, best_i = dfb_dist.all_reduce_argmax(best_s, best_i, device=dev)
-  return session.post.fill_candidates(seed, int(best_i), 1, bounds).cpu().numpy()[0]
-
-
-def _fused_maximise(scorer, anc_data, bounds=None, session=None):
-  """ maximise_acquisition (:23-40) for the `rand` method: candidates scored slab by slab through fused device
-      calls (per rank), the arg-max point returned.  `session` (a context-manager factory, GP._fused_session) binds
-      hallucinations / test kernel once for all slabs; a plain `scorer(pts)` callable works too. """
-  bounds = anc_data.domain.bounds if bounds is None else bounds
+def _candidate_rng(anc_data):
+  """ The candidate source of one `rand` maximisation: anc_data.candidate_rng, else CANDIDATE_RNG. """
   mode = getattr(anc_data, 'candidate_rng', None) or CANDIDATE_RNG
+  if mode not in ('numpy', 'device'):
+    raise ValueError("candidate_rng should be 'numpy' or 'device'.")
+  return mode
+
+
+def _device_seed():
+  """ The seed of the device's candidates (and normals): two draws from the global NumPy stream. """
+  return (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
+
+
+def _slab_argmax(source, score):
+  """ random_maximise's arg-max (oper_utils.py:70-80) over a candidate source: score(pts, r0) -> (best_score,
+      best_index_within_pts, ...) for every slab of this rank's rows, folded in np.argmax order (first index on ties,
+      NaN counts as the maximum) and joined across the ranks the source is sharded over.  Returns (global index, row):
+      the row is a copy of the winning host row when the source has row_dim set (slab buffers are reused; the row
+      rides along the 16-byte join), else None and source.point regenerates it from the index.  When a score call
+      raises, the source is closed -- the streamed draw still consumes the whole stream -- before the error propagates. """
+  from . import dist as dfb_dist
+  best_s, best_i, best_row = 0.0, -1, None
+  slabs = source.slabs()
+  try:
+    for r0, pts in slabs:
+      res = score(pts, r0)
+      s, gi = float(res[0]), r0 + int(res[1])
+      if dfb_dist.better(s, gi, best_s, best_i):
+        best_s, best_i = s, gi
+        if source.row_dim is not None:
+          best_row = np.array(pts[gi - r0], dtype=np.float64)
+  finally:
+    slabs.close()
+  _, world, dev = source.shard
+  if world > 1 and source.row_dim is not None:
+    best_s, best_i, best_row = dfb_dist.all_reduce_argmax_point(best_s, best_i, best_row, source.row_dim, device=dev)
+  elif world > 1:
+    best_s, best_i = dfb_dist.all_reduce_argmax(best_s, best_i, device=dev)
+  return best_i, best_row
+
+
+class _StreamedRows(object):
+  """ Candidate source 'numpy' on a Euclidean domain, drawn slab by slab on a producer thread: np.random.random((M, d))
+      and consecutive np.random.random((m_k, d)) slabs consume the MT19937 stream identically (row-major fill), so the
+      candidates -- and the state the global RNG is left in -- are the reference's.  `unit` = rows of one scoring chunk. """
+
+  def __init__(self, bounds, max_evals, slab, unit=0):
+    self.bounds = np.asarray(bounds, dtype=np.float64)
+    self.M, self.row_dim = int(max_evals), len(self.bounds)
+    self.slab, self.unit = slab, unit
+    self.shard = _shard_info()
+
+  def slabs(self):
+    import queue
+    import threading
+    from . import dist as dfb_dist
+    M, dim = self.M, self.row_dim
+    rank, world, _ = self.shard
+    lo_r, hi_r = dfb_dist.shard_bounds(M, rank, world) if world > 1 else (0, M)
+    starts = _slab_schedule(M, self.slab, self.unit) if M > 0 else []
+    q = queue.Queue(maxsize=2)
+    width, low = self.bounds[:, 1] - self.bounds[:, 0], self.bounds[:, 0]
+    # staging buffers sized by the largest slab actually scheduled (never by the nominal slab size), and only while they
+    # stay modest: 4 x 256 MB at most
+    rows_max = max([r for _, r in starts] or [0])
+    pinned = _pinned_slab_buffers(rows_max, dim) if (len(starts) > 1 and rows_max * dim * 8 <= (256 << 20)) else None
+
+    def _producer():
+      try:
+        for k, (r0, rows) in enumerate(starts):
+          raw = np.random.random((rows, dim))
+          if not min(hi_r, r0 + rows) > max(lo_r, r0):
+            q.put((r0, None))                            # another rank's rows: drawn (the stream must advance), not mapped
+            continue
+          if pinned is not None:
+            pts = pinned[k % len(pinned)][:rows]
+            np.multiply(raw, width, out=pts)             # map_to_bounds: pts * (hi - lo) + lo, written in place
+            np.add(pts, low, out=pts)
+          else:
+            pts = raw * width + low
+          q.put((r0, pts))
+      except BaseException as exc:  # pylint: disable=broad-except
+        q.put(exc)
+
+    if len(starts) > 1:
+      th = threading.Thread(target=_producer, daemon=True)
+      th.start()
+    else:
+      th = None
+      _producer()
+    pending = len(starts)
+    try:
+      while pending:
+        item = q.get()
+        pending -= 1
+        if isinstance(item, BaseException):
+          pending = 0
+          raise item
+        r0, pts = item
+        if pts is None:
+          continue
+        a, b = max(lo_r, r0), min(hi_r, r0 + len(pts))
+        if b > a:
+          yield a, pts[a - r0:b - r0]
+    finally:
+      while pending:        # closed early: keep draining, the global RNG must end where the reference leaves it
+        pending -= 1
+        if isinstance(q.get(), BaseException):
+          break
+      if th is not None:
+        th.join()
+
+  def point(self, i, row):
+    return row
+
+
+class _IndexedRows(object):
+  """ Candidates addressed by global row index: rows lo .. hi-1 in slabs, fill(r0, m, out) returning rows r0 .. r0+m-1
+      (device sources write them into out, the previous slab's buffer, when it is not None), point_of(i) the point of
+      row i. """
+  row_dim = None
+
+  def __init__(self, slab, lo, hi, fill, point_of, shard=(0, 1, None)):
+    self.slab, self.lo, self.hi, self.fill, self.point_of, self.shard = slab, lo, hi, fill, point_of, shard
+
+  def slabs(self):
+    buf = None
+    for r0 in range(self.lo, self.hi, self.slab):
+      m = min(self.slab, self.hi - r0)
+      buf = self.fill(r0, m, None if buf is None else buf[:m])
+      yield r0, buf
+
+  def point(self, i, row):
+    return self.point_of(int(i))
+
+
+def _maximise_streamed(score, bounds, max_evals, slab, unit=0):
+  """ random_maximise (oper_utils.py:70-80) over the streamed host draw (_StreamedRows): score(pts) -> (best_score,
+      best_index_within_pts, ...) per slab; returns the arg-max point. """
+  source = _StreamedRows(bounds, max_evals, slab, unit)
+  return source.point(*_slab_argmax(source, lambda pts, r0: score(pts)))
+
+
+def _fused_maximise(scorer, anc_data, session=None):
+  """ maximise_acquisition (:23-40) for the `rand` method on a Euclidean domain: candidates scored slab by slab
+      through fused device calls (per rank), the arg-max point returned.  `session` (a context-manager factory,
+      GP._fused_session) binds hallucinations / test kernel once for all slabs; a plain `scorer(pts)` callable works
+      too, on host candidates. """
+  from . import dist as dfb_dist
+  bounds, M = anc_data.domain.bounds, int(anc_data.max_evals)
+  mode = _candidate_rng(anc_data)
   if session is None:
     if mode == 'device':
       raise NotImplementedError('device candidate generation needs a GP session')
-    return _maximise_streamed(scorer, bounds, anc_data.max_evals, STREAM_SLAB_ROWS)
+    return _maximise_streamed(scorer, bounds, M, STREAM_SLAB_ROWS)
   with session() as sess:
-    if mode == 'device':
-      return _maximise_device_candidates(sess, bounds, anc_data.max_evals)
-    if mode != 'numpy':
-      raise ValueError("candidate_rng should be 'numpy' or 'device'.")
-    return _maximise_streamed(sess.score, bounds, anc_data.max_evals, sess.slab_rows(STREAM_SLAB_ROWS),
-                              unit=sess.slab_rows(1))
+    if mode == 'numpy':
+      return _maximise_streamed(sess.score, bounds, M, sess.slab_rows(STREAM_SLAB_ROWS), unit=sess.slab_rows(1))
+    seed = _device_seed()
+    shard = _shard_info()
+    lo, hi = dfb_dist.shard_bounds(M, shard[0], shard[1]) if shard[1] > 1 else (0, M)
+    fill = lambda r0, m, out: sess.post.fill_candidates(seed, r0, m, bounds, out=out)
+    source = _IndexedRows(sess.slab_rows(2 * STREAM_SLAB_ROWS), lo, hi, fill,
+                          lambda i: fill(i, 1, None).cpu().numpy()[0], shard)
+    return source.point(*_slab_argmax(source, lambda pts, r0: sess.score(pts)))
 
 
 def _reference_fortran_direct_available():
@@ -574,12 +626,17 @@ def _get_gp_ucb_dim(gp):
   return 3.0
 
 
-def _acq_on_cp_domain(gp, anc_data, acq, acq_fn):
-  """ CP-domain dispatch of the acquisitions below: the fused 'rand' maximiser, else _cp_other_maximiser with the
-      host objective acq_fn(list of points). """
-  if anc_data.acq_opt_method in ['rand']:
-    return _cp_fused_maximise(gp, anc_data, acq)
-  return _cp_other_maximiser(acq_fn, anc_data)
+def _maximise_acq(gp, anc_data, acq, acq_fn):
+  """ maximise_acquisition (:23-40) of the acquisitions below: the fused 'rand' maximiser (device descriptor acq) on
+      Cartesian-product and Euclidean domains, else the other maximisers with the host objective acq_fn (on a CP
+      domain it takes a list of list-of-parts points). """
+  if _is_cp_domain(anc_data):
+    if anc_data.acq_opt_method in ['rand']:
+      return _cp_fused_maximise(gp, anc_data, acq)
+    return _cp_other_maximiser(acq_fn, anc_data)
+  if _check_rand_euclidean(anc_data):
+    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
+  return _delegate_to_reference_maximiser(acq_fn, anc_data)
 
 
 def _get_ucb_beta_th(dim, time_step):
@@ -593,12 +650,7 @@ def asy_ucb(gp, anc_data):
   def _ucb_acq(x):
     mu, sigma = gp_eval(x)
     return mu + beta_th * sigma
-  if _is_cp_domain(anc_data):
-    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ucb', beta=beta_th), _ucb_acq)
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ucb', beta=beta_th)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  return _delegate_to_reference_maximiser(_ucb_acq, anc_data)
+  return _maximise_acq(gp, anc_data, make_acq_desc('ucb', beta=beta_th), _ucb_acq)
 
 
 def syn_ucb(num_workers, list_of_gps, anc_datas):
@@ -615,12 +667,7 @@ def asy_pi(gp, anc_data):
     from scipy.stats import norm as normal_distro
     mu, sigma = gp_eval(x)
     return normal_distro.cdf((mu - curr_best) / sigma)
-  if _is_cp_domain(anc_data):
-    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('pi', best=curr_best), _pi_acq)
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('pi', best=curr_best)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  return _delegate_to_reference_maximiser(_pi_acq, anc_data)
+  return _maximise_acq(gp, anc_data, make_acq_desc('pi', best=curr_best), _pi_acq)
 
 
 def syn_pi(num_workers, list_of_gps, anc_datas):
@@ -635,12 +682,7 @@ def asy_ei(gp, anc_data):
     mu, sigma = gp_eval(x)
     z = (mu - curr_best) / sigma
     return sigma * (z * normal_distro.cdf(z) + normal_distro.pdf(z))
-  if _is_cp_domain(anc_data):
-    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ei', best=curr_best), _ei_acq)
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ei', best=curr_best)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  return _delegate_to_reference_maximiser(_ei_acq, anc_data)
+  return _maximise_acq(gp, anc_data, make_acq_desc('ei', best=curr_best), _ei_acq)
 
 
 def syn_ei(num_workers, list_of_gps, anc_datas):
@@ -659,12 +701,7 @@ def _ttei(gp, anc_data, ref_point):
     comb_std = np.sqrt(ref_std ** 2 + sigma ** 2)
     z = (mu - ref_mean) / comb_std
     return comb_std * (z * normal_distro.cdf(z) + normal_distro.pdf(z))
-  if _is_cp_domain(anc_data):
-    return _acq_on_cp_domain(gp, anc_data, make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std), _tt_ei_acq)
-  if _check_rand_euclidean(anc_data):
-    acq = make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std)
-    return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
-  return _delegate_to_reference_maximiser(_tt_ei_acq, anc_data)
+  return _maximise_acq(gp, anc_data, make_acq_desc('ttei', ref_mean=ref_mean, ref_std=ref_std), _tt_ei_acq)
 
 
 def asy_ttei(gp, anc_data):
@@ -689,38 +726,40 @@ def _get_add_ucb_beta_th(dim, time_step):
   return np.sqrt(0.2 * dim * np.log(2 * dim * time_step + 1))
 
 
+def _add_ucb_groups(anc_data, groupings, maximise_group):
+  """ The group loop of Add-UCB (:139-189, :334-388): group j's UCB, with the beta of its d_j coordinates, is maximised
+      over the d_j-dimensional sub-box with max_evals // (number of groups) candidates by
+      maximise_group(j, acq_desc, anc_data_j) -> point_j, and the group points are put back into one point. """
+  if not _check_rand_euclidean(anc_data):
+    raise NotImplementedError("Add-UCB on device needs acq_opt_method == 'rand'.")
+  domain_bounds = np.asarray(anc_data.domain_bounds)
+  group_points = []
+  for j, group_j in enumerate(groupings):
+    anc_data_j = copy(anc_data)
+    anc_data_j.max_evals = anc_data.max_evals // len(groupings)
+    anc_data_j.domain = EuclideanDomain(domain_bounds[group_j])
+    acq = make_acq_desc('ucb', beta=_get_add_ucb_beta_th(len(group_j), anc_data.t))
+    group_points.append(maximise_group(j, acq, anc_data_j))
+  ret = np.zeros((sum(len(point_j) for point_j in group_points),))
+  for point_j, group_j in zip(group_points, groupings):
+    ret[group_j] = point_j
+  return ret
+
+
 def _add_ucb(gp, add_kernel, mean_funcs, anc_data):
   """ :139-189.  Per group j the candidates live in the d_j-dimensional sub-box; K_*j =
       scale * k_j(X*_j, X[:, g_j]) is scored against the FULL additive GP's L and alpha. """
   if mean_funcs is not None:
     raise NotImplementedError('Add-UCB with per-group mean functions is not used by GPBandit '
                               '(asy_add_ucb passes None).')
-  if not _check_rand_euclidean(anc_data):
-    raise NotImplementedError("Add-UCB on device needs acq_opt_method == 'rand'.")
-  kernel_list = add_kernel.kernel_list
   groupings = add_kernel.groupings
-  total_max_evals = anc_data.max_evals
-  domain_bounds = np.asarray(anc_data.domain_bounds)
-  num_groups = len(kernel_list)
-  group_points = []
-  num_coordinates = 0
-  anc_data.max_evals = total_max_evals // num_groups
   train_dim = gp._train_matrix().shape[1]
-  for group_j, kernel_j in zip(groupings, kernel_list):
-    betath_j = _get_add_ucb_beta_th(len(group_j), anc_data.t)
-    desc_j = gp._group_test_descriptor(add_kernel, kernel_j, group_j, train_dim)
-    acq = make_acq_desc('ucb', beta=betath_j)
-    anc_data_j = copy(anc_data)
-    anc_data_j.domain = EuclideanDomain(domain_bounds[group_j])
-    point_j = _fused_maximise(None, anc_data_j, session=lambda _d=desc_j, _a=acq: gp._fused_session(
-        _a, [], test_desc=_d, mean_const=0.0))
-    group_points.append(point_j)
-    num_coordinates += len(point_j)
-  anc_data.max_evals = total_max_evals
-  ret = np.zeros((num_coordinates,))
-  for point_j, group_j in zip(group_points, groupings):
-    ret[group_j] = point_j
-  return ret
+
+  def maximise_group(j, acq, anc_data_j):
+    desc_j = gp._group_test_descriptor(add_kernel, add_kernel.kernel_list[j], groupings[j], train_dim)
+    return _fused_maximise(None, anc_data_j, session=lambda: gp._fused_session(acq, [], test_desc=desc_j,
+                                                                               mean_const=0.0))
+  return _add_ucb_groups(anc_data, groupings, maximise_group)
 
 
 def asy_add_ucb(gp, anc_data):
@@ -734,13 +773,20 @@ def syn_add_ucb(num_workers, list_of_gps, anc_datas):
 # ---------------------------------------------------------------------------------------------
 # Thompson sampling (:118-131)
 # ---------------------------------------------------------------------------------------------
-def asy_ts(gp, anc_data):
-  """ :119-127 -- always the random maximiser with 4x the evaluations; the objective is one joint
-      posterior draw over all candidates (gp.draw_samples(1, x)). """
+def _ts_anc_data(anc_data):
+  """ :119-124 -- a copy of anc_data for Thompson sampling, which always runs the random maximiser: with 4x the
+      evaluations when another maximiser was asked for. """
   anc_data = copy(anc_data)
   if anc_data.acq_opt_method != 'rand':
     anc_data.acq_opt_method = 'rand'
     anc_data.max_evals = 4 * anc_data.max_evals
+  return anc_data
+
+
+def asy_ts(gp, anc_data):
+  """ :119-127 -- always the random maximiser with 4x the evaluations; the objective is one joint
+      posterior draw over all candidates (gp.draw_samples(1, x)). """
+  anc_data = _ts_anc_data(anc_data)
   if _is_cp_domain(anc_data):
     return _cp_ts(gp, anc_data)
   halluc = _halluc_points(anc_data)
@@ -756,49 +802,12 @@ def _cp_ts(gp, anc_data):
       Legacy NumPy draws normals in pairs and caches the second, so np.random.normal(size=M) after the candidates gives
       the same M normals and leaves the stream where the M one-normal calls leave it.  Every candidate is scored in
       fused device slabs (dfb_score_argmax_ts) and the arg-max follows np.argmax.  candidate_rng 'device' generates the
-      rows (dfb_fill_mixed_candidates) and the normals (in the scoring kernel) from one seed drawn as _cp_fused_maximise
-      draws it.  A candidate whose variance is not > 0 raises ValueError, as the reference's stable_cholesky does. """
-  from . import dist as dfb_dist
+      rows (dfb_fill_mixed_candidates) and the normals (in the scoring kernel) from one seed.  A candidate whose variance
+      is not > 0 raises ValueError, as the reference's stable_cholesky does. """
   if getattr(anc_data, 'is_mf', False) or hasattr(gp, 'fidel_space_kernel') or hasattr(gp, 'mfgp'):
     raise NotImplementedError('Thompson sampling with a multi-fidelity GP on a Cartesian-product domain is outside the '
                               'GPU hot-path scope.')
-  parts = _cp_parts(anc_data.domain, gp.kernel)
-  if _shard_info()[1] > 1:
-    raise NotImplementedError('Cartesian-product candidate draws are not sharded across ranks.')
-  mode = getattr(anc_data, 'candidate_rng', None) or CANDIDATE_RNG
-  if mode not in ('numpy', 'device'):
-    raise ValueError("candidate_rng should be 'numpy' or 'device'.")
-  M = int(anc_data.max_evals)
-  if mode == 'device':
-    seed = (int(np.random.randint(0, 2 ** 31 - 1)) << 31) | int(np.random.randint(0, 2 ** 31 - 1))
-  else:
-    rows, draws = draw_cp_candidates(parts, M)
-    z = np.random.normal(size=M)
-  nonpos = 0
-  with gp._fused_session(None, _halluc_points(anc_data)) as sess:
-    slab = sess.slab_rows(2 * STREAM_SLAB_ROWS if mode == 'device' else STREAM_SLAB_ROWS)
-    layout = _cp_device_layout(parts) if mode == 'device' else None
-    best_s, best_i, buf = 0.0, -1, None
-    for r0 in range(0, M, slab):
-      m = min(slab, M - r0)
-      if mode == 'device':
-        buf = _cp_device_rows(sess, seed, r0, m, layout, out=None if buf is None else buf[:m])
-        res = sess.score_ts(buf, seed=seed, row0=r0)
-      else:
-        res = sess.score_ts(rows[r0:r0 + m], z=z[r0:r0 + m])
-      nonpos += int(res[3])
-      s, gi = float(res[0]), r0 + int(res[1])
-      if dfb_dist.better(s, gi, best_s, best_i):
-        best_s, best_i = s, gi
-    if nonpos > 0:
-      raise ValueError('Could not compute Cholesky decomposition despite adding jitter to the diagonal: the posterior '
-                       'variance of %d candidate(s) is not positive. This is likely because the M is not positive '
-                       'semi-definite or has infinities/nans.' % (nonpos))
-    if mode == 'device':
-      kinds, bounds, n_levels, _ = layout
-      row = sess.post.fill_mixed_candidates(seed, best_i, 1, kinds, bounds, n_levels).cpu().numpy()[0]
-      return _cp_point_from_device_row(parts, row)
-  return point_from_draws(parts, draws, best_i)
+  return _cp_fused_maximise(gp, anc_data, None)
 
 
 def _ts_block(gp):
@@ -944,44 +953,27 @@ def _add_ucb_for_boca(mfgp, fidel_to_opt, mean_funcs, anc_data):
       scored against the MF-GP's full L and alpha. """
   if mean_funcs is not None:
     raise NotImplementedError('per-group mean functions are not used by GPBandit.')
-  if not _check_rand_euclidean(anc_data):
-    raise NotImplementedError("Add-UCB on device needs acq_opt_method == 'rand'.")
   from .kernel import CoordinateProductKernel
-  domain_kernel_list = mfgp.domain_kernel.kernel_list
   groupings = mfgp.domain_kernel.groupings
-  total_max_evals = anc_data.max_evals
   kern_scale = mfgp.kernel.hyperparams['scale']
-  domain_bounds = np.asarray(anc_data.domain_bounds)
-  num_groups = len(domain_kernel_list)
   f2o = np.asarray(fidel_to_opt, dtype=np.float64).reshape(-1)
   dz = len(f2o)
   train_dim = mfgp._train_matrix().shape[1]
-  group_points = []
-  num_coordinates = 0
-  anc_data.max_evals = total_max_evals // num_groups
-  for group_j, kernel_j in zip(groupings, domain_kernel_list):
+
+  def maximise_group(j, acq, anc_data_j):
+    group_j = groupings[j]
     d_j = len(group_j)
-    betath_j = _get_add_ucb_beta_th(d_j, anc_data.t)
-    prod_j = CoordinateProductKernel(dz + d_j, kern_scale, [mfgp.fidel_kernel, kernel_j],
+    prod_j = CoordinateProductKernel(dz + d_j, kern_scale, [mfgp.fidel_kernel, mfgp.domain_kernel.kernel_list[j]],
                                      [list(range(dz)), list(range(dz, dz + d_j))])
     train_coords = [mfgp.fidel_coords[i] for i in range(dz)] + \
                    [mfgp.domain_coords[int(g)] for g in group_j]
     desc_j = build_descriptor(prod_j, train_dim=train_dim, cand_dim=dz + d_j,
                               train_coords=train_coords, cand_coords=list(range(dz + d_j)))
-    acq = make_acq_desc('ucb', beta=betath_j)
-    anc_data_j = copy(anc_data)
-    anc_data_j.domain = EuclideanDomain(domain_bounds[group_j])
-    def scorer(pts, _d=desc_j, _a=acq):
+    def scorer(pts):
       zx = np.concatenate((np.repeat(f2o.reshape(1, -1), len(pts), axis=0), pts), axis=1)
-      return mfgp._fused_score(_a, zx, [], test_desc=_d, mean_const=0.0)
-    point_j = _fused_maximise(scorer, anc_data_j)
-    group_points.append(point_j)
-    num_coordinates += len(point_j)
-  anc_data.max_evals = total_max_evals
-  ret = np.zeros((num_coordinates,))
-  for point_j, group_j in zip(group_points, groupings):
-    ret[group_j] = point_j
-  return ret
+      return mfgp._fused_score(acq, zx, [], test_desc=desc_j, mean_const=0.0)
+    return _fused_maximise(scorer, anc_data_j)
+  return _add_ucb_groups(anc_data, groupings, maximise_group)
 
 
 def asy_add_ucb_for_boca(mfgp, fidel_to_opt, anc_data):

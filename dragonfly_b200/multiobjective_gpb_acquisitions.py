@@ -8,14 +8,13 @@ takes random_maximise's arg-max (oper_utils.py:70-80).  Same names, arguments an
 (obj_weights, reference_point) as the reference; `asy`, `syn`, `seq` tables at the bottom.
 """
 from argparse import Namespace
-from copy import copy
 
 import numpy as np
 
 from . import _lib
 from .gpb_acquisitions import (draw_candidates, _check_rand_euclidean, _halluc_points,
                                _delegate_to_reference_maximiser, _sharded_argmax, _draw_one_sample,
-                               _ts_cols, _shard_info)
+                               _ts_cols, _shard_info, _ts_anc_data)
 
 
 def _get_ucb_beta_th(dim, time_step):
@@ -71,10 +70,7 @@ def mo_tch_asy_ucb(gps, anc_data):
 
 
 def _mo_ts(kind, gps, anc_data):
-  anc_data = copy(anc_data)
-  if anc_data.acq_opt_method != 'rand':          # :23-26 -- always the random maximiser, 4x the evaluations
-    anc_data.acq_opt_method = 'rand'
-    anc_data.max_evals = 4 * anc_data.max_evals
+  anc_data = _ts_anc_data(anc_data)              # :23-26 -- always the random maximiser, 4x the evaluations
   halluc = _halluc_points(anc_data)
   rand_pts = draw_candidates(anc_data.domain.bounds, anc_data.max_evals)
   # one joint draw per objective, in order (global RNG); under torch.distributed each rank computes only
