@@ -14,49 +14,77 @@ the y row riding along; no L^-1, no alpha).  The samples are independent, so und
 they shard across ranks with one all-gather of the LML values at the end (NCCL on GPUs, gloo in the
 CPU tests of the sharding logic).
 """
+from argparse import Namespace
+
 import numpy as np
 
 from . import _lib
 from .kernel import SEKernel, MaternKernel, ExpDecayKernel, AdditiveKernel, CoordinateProductKernel, ESPKernelSE, \
     ESPKernelMatern, HammingKernel, CategoryCodes, build_descriptor
-from .gp_core import stable_cholesky_on_device
+from .gp_core import GP, ConstantMean, stable_cholesky_on_device
 
 
-class EuclideanHPLayout(object):
-  """ How a continuous hp vector maps to (mean const, noise var, kernel) for an SE / Matern / ESP GP.
-      ESP (kernel_type 'esp', euclidean_gp.py:283-299, 249-251, 816-892): log scale and d log bandwidths whatever
-      use_same_bandwidth says; discrete hps [nu]? (esp_kernel_type 'matern' with esp_matern_nu < 0) then [order]?
-      (esp_order == -1), handed to unpack as one tuple per sample. """
+def _pop_bandwidths(hp, n, same):
+  """ Pops n log bandwidths (one, repeated, when they are shared) from the front of `hp`. """
+  return [np.exp(hp.pop(0))] * n if same else [np.exp(hp.pop(0)) for _ in range(n)]
 
-  def __init__(self, dim, kernel_type='matern', nu=2.5, use_same_bandwidth=False,
-               mean_func_type='median', mean_func_const=0.0, noise_var_type='tune',
-               noise_var_label=0.05, noise_var_value=0.1, use_additive_gp=False, add_max_group_size=6,
-               num_groups_per_group_size=-1, esp_kernel_type='se', esp_order=-1, esp_matern_nu=-1.0):
-    if kernel_type not in ('se', 'matern', 'esp'):
-      raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kernel_type))
-    if kernel_type == 'esp':
-      if esp_kernel_type not in ('se', 'matern'):
-        raise NotImplementedError('esp_kernel_type %s is not implemented (euclidean_gp.py:285-286).'
-                                  % (esp_kernel_type))
-      if use_additive_gp:
-        raise NotImplementedError('use_additive_gp with an ESP kernel is outside the device path.')
-    self.esp_kernel_type, self.esp_order, self.esp_matern_nu = esp_kernel_type, esp_order, esp_matern_nu
-    self.dim, self.kernel_type, self.nu = dim, kernel_type, nu
-    self.use_same_bandwidth = use_same_bandwidth
+
+def _se_or_matern(kernel_type, dim, nu, scale, bws):
+  return SEKernel(dim, scale, bws) if kernel_type == 'se' else MaternKernel(dim, nu, scale, bws)
+
+
+class HPLayout(object):
+  """ How a continuous hp vector and one sample's discrete hps map to (mean const, noise var, kernel), and what fit_gp,
+      the LML batchers and the slice sampler have to know about that map.  This base owns what GPFitter owns
+      (gp_core.py:396-416, 501-543): [mean const]? [log noise]? log scale at the head of the vector.  A layout adds its
+      kernel's hps (_num_kernel_hps, _kernel) and overrides the answers below that differ from the common one. """
+  max_dscr_hps = 1            # discrete hps the device path accepts (None: any number)
+  lml_batchable = True        # dfb_lml_batch builds this layout's kernels ...
+  mixed = False               # ... through its dfb_lml_batch_mixed entry (kernels with Hamming factors)
+  ml_fit_batched = False      # an 'ml' fit asks lml_batch_for_hyperparams, not lml_for_hyperparams' build lanes
+  use_additive_gp = False     # every objective evaluation carries a random grouping of the coordinates
+  post_sampling_on_device = False   # 'post_sampling' fits run post_sampling.post_sample_hps, not the reference
+
+  def __init__(self, dim, mean_func_type='median', mean_func_const=0.0, noise_var_type='tune', noise_var_label=0.05,
+               noise_var_value=0.1):
+    self.dim = dim
     self.mean_func_type, self.mean_func_const = mean_func_type, mean_func_const
     self.noise_var_type = noise_var_type
     self.noise_var_label, self.noise_var_value = noise_var_label, noise_var_value
-    # additive models (euclidean_gp.py:50-60, 243-248): the group size is one more discrete hyper-parameter and
-    # every objective evaluation carries a random grouping of the coordinates
-    self.use_additive_gp = use_additive_gp
-    self.add_max_group_size = min(add_max_group_size, dim)
-    self.num_groups_per_group_size = num_groups_per_group_size
 
   def num_hps(self):
-    n = 1 + (1 if self.use_same_bandwidth and self.kernel_type != 'esp' else self.dim)
-    n += 1 if self.mean_func_type == 'tune' else 0
-    n += 1 if self.noise_var_type == 'tune' else 0
-    return n
+    head = (1 if self.mean_func_type == 'tune' else 0) + (1 if self.noise_var_type == 'tune' else 0)
+    return head + 1 + self._num_kernel_hps()
+
+  def unpack(self, hp, Y, nu=None, groupings=None):
+    """ (mean const, noise var, kernel) of one hp vector (gp_core.py:509-538); `nu` is dscr_arg() of the sample's
+        discrete hps, `groupings` the coordinate groups of an additive model. """
+    hp = list(np.asarray(hp, dtype=np.float64))
+    Y = np.asarray(Y, dtype=np.float64)
+    mean_const, noise_var = self._mean_and_noise(hp, Y)
+    scale = np.exp(hp.pop(0))
+    return float(mean_const), float(noise_var), self._kernel(scale, hp, nu, groupings)
+
+  def dscr_arg(self, dscr_row):
+    """ What unpack takes as `nu` for one sample's discrete hps, and so what one entry of the `nus` of
+        lml_for_hyperparams / lml_batch_for_hyperparams is.  Here: the Matern nu when it is the one discrete hp, else
+        None (the kernel is built with the layout's own nu).  EuclideanHPLayout: that, with an additive model's group
+        size after the nu ([nu]? [group size], euclidean_gp.py:226-248: a single discrete hp of an additive layout is
+        the group size, so None), or for ESP the tuple [nu]? [order]? (None when empty).  CartesianProductHPLayout: the
+        tuple of every tuned Matern nu in part order. """
+    return dscr_row[0] if len(dscr_row) == 1 else None
+
+  def rows(self, X):
+    """ The (n, dim) float64 device rows of the fitter's points. """
+    return np.ascontiguousarray(np.asarray(X, dtype=np.float64))
+
+  def gp_on(self, points, rows):
+    """ (GP class, its points) for the GP fit_gp returns when it is given no build_gp. """
+    return GP, list(rows)
+
+  def fitter_data(self, fitter):
+    """ (points, Y) a reference fitter of this layout holds, the points as rows() takes them. """
+    return np.array(fitter.X), np.array(fitter.Y)
 
   def _mean_noise_bounds(self, Y):
     """ (Y_var, [mean bounds]? [log noise bounds]?) as GPFitter._set_up sets them up (gp_core.py:336-338, 396-416). """
@@ -72,29 +100,6 @@ class EuclideanHPLayout(object):
     if self.noise_var_type == 'tune':
       out.append([np.log(0.005 * Y_var), np.log(0.2 * Y_var)])
     return Y_var, out
-
-  def bounds(self, X, Y, tune_nu=None):
-    """ (cts_hp_bounds, dscr_hp_vals) the way the reference's fitter sets them up from the data
-        (gp_core.py:336-338, 396-416; euclidean_gp.py:253-276): mean value (if tuned), log noise (if tuned),
-        log scale, log bandwidth(s); discrete [0.5, 1.5, 2.5] for a Matern kernel whose nu is tuned
-        (options.matern_nu < 0; default here: tuned iff self.nu is None or negative). """
-    X = np.asarray(X, dtype=np.float64)
-    Y_var, out = self._mean_noise_bounds(Y)
-    out.append([np.log(0.1 * Y_var), np.log(10 * Y_var)])
-    X_std_norm = np.linalg.norm(X, 'fro') + 1e-4
-    single = [np.log(0.01 * X_std_norm), np.log(10 * X_std_norm)]
-    out += [single] * (1 if self.use_same_bandwidth and self.kernel_type != 'esp' else self.dim)
-    if self.kernel_type == 'esp':
-      dscr = [[0.5, 1.5, 2.5]] if (self.esp_kernel_type == 'matern' and self.esp_matern_nu < 0) else []
-      if self.esp_order == -1:
-        dscr.append(list(range(1, max(self.dim, self.esp_order) + 1)))
-      return np.array(out), dscr
-    if tune_nu is None:
-      tune_nu = self.kernel_type == 'matern' and (self.nu is None or self.nu < 0)
-    dscr = [[0.5, 1.5, 2.5]] if (self.kernel_type == 'matern' and tune_nu) else []
-    if self.use_additive_gp:
-      dscr.append([x + 1 for x in range(self.add_max_group_size)])
-    return np.array(out), dscr
 
   def _mean_and_noise(self, hp, Y):
     """ Pops the mean value / log noise from the front of `hp` when they are tuned (gp_core.py:509-538). """
@@ -118,32 +123,86 @@ class EuclideanHPLayout(object):
       noise_var = self.noise_var_value
     return mean_const, noise_var
 
-  def unpack(self, hp, Y, nu=None, groupings=None):
-    """ gp_core.py:509-538 + euclidean_gp.py:801-861 """
-    hp = list(np.asarray(hp, dtype=np.float64))
-    Y = np.asarray(Y, dtype=np.float64)
-    mean_const, noise_var = self._mean_and_noise(hp, Y)
-    scale = np.exp(hp.pop(0))
+
+class EuclideanHPLayout(HPLayout):
+  """ The hp vector of an SE / Matern / ESP GP (EuclideanGPFitter): the head, then the log bandwidth(s).
+      ESP (kernel_type 'esp', euclidean_gp.py:283-299, 249-251, 816-892): log scale and d log bandwidths whatever
+      use_same_bandwidth says; discrete hps [nu]? (esp_kernel_type 'matern' with esp_matern_nu < 0) then [order]?
+      (esp_order == -1), handed to unpack as one tuple per sample. """
+
+  def __init__(self, dim, kernel_type='matern', nu=2.5, use_same_bandwidth=False,
+               mean_func_type='median', mean_func_const=0.0, noise_var_type='tune',
+               noise_var_label=0.05, noise_var_value=0.1, use_additive_gp=False, add_max_group_size=6,
+               num_groups_per_group_size=-1, esp_kernel_type='se', esp_order=-1, esp_matern_nu=-1.0):
+    if kernel_type not in ('se', 'matern', 'esp'):
+      raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope.' % (kernel_type))
+    if kernel_type == 'esp':
+      if esp_kernel_type not in ('se', 'matern'):
+        raise NotImplementedError('esp_kernel_type %s is not implemented (euclidean_gp.py:285-286).'
+                                  % (esp_kernel_type))
+      if use_additive_gp:
+        raise NotImplementedError('use_additive_gp with an ESP kernel is outside the device path.')
+    super(EuclideanHPLayout, self).__init__(dim, mean_func_type, mean_func_const, noise_var_type, noise_var_label,
+                                            noise_var_value)
+    self.esp_kernel_type, self.esp_order, self.esp_matern_nu = esp_kernel_type, esp_order, esp_matern_nu
+    self.kernel_type, self.nu = kernel_type, nu
+    self.use_same_bandwidth = use_same_bandwidth
+    # additive models (euclidean_gp.py:50-60, 243-248): the group size is one more discrete hyper-parameter and
+    # every objective evaluation carries a random grouping of the coordinates
+    self.use_additive_gp = use_additive_gp
+    self.add_max_group_size = min(add_max_group_size, dim)
+    self.num_groups_per_group_size = num_groups_per_group_size
+    # ESP ([nu]? [order]?) and additive ([nu]? [group size]) layouts have a second discrete hp and kernels that only
+    # the LML-only build of lml_for_hyperparams takes, and their 'post_sampling' fits stay with the reference
+    plain = not (use_additive_gp or kernel_type == 'esp')
+    self.max_dscr_hps = 1 if plain else 2
+    self.lml_batchable = self.post_sampling_on_device = plain
+
+  def _num_kernel_hps(self):
+    return 1 if self.use_same_bandwidth and self.kernel_type != 'esp' else self.dim
+
+  def dscr_arg(self, dscr_row):
     if self.kernel_type == 'esp':
-      return float(mean_const), float(noise_var), self._esp_kernel(scale, hp, nu)
-    if self.use_same_bandwidth:
-      bws = [np.exp(hp.pop(0))] * self.dim
-    else:
-      bws = [np.exp(hp.pop(0)) for _ in range(self.dim)]
+      return tuple(dscr_row) if len(dscr_row) else None
+    return dscr_row[0] if len(dscr_row) == (2 if self.use_additive_gp else 1) else None
+
+  def bounds(self, X, Y, tune_nu=None):
+    """ (cts_hp_bounds, dscr_hp_vals) the way the reference's fitter sets them up from the data
+        (gp_core.py:336-338, 396-416; euclidean_gp.py:253-276): mean value (if tuned), log noise (if tuned),
+        log scale, log bandwidth(s); discrete [0.5, 1.5, 2.5] for a Matern kernel whose nu is tuned
+        (options.matern_nu < 0; default here: tuned iff self.nu is None or negative). """
+    X = np.asarray(X, dtype=np.float64)
+    Y_var, out = self._mean_noise_bounds(Y)
+    out.append([np.log(0.1 * Y_var), np.log(10 * Y_var)])
+    X_std_norm = np.linalg.norm(X, 'fro') + 1e-4
+    single = [np.log(0.01 * X_std_norm), np.log(10 * X_std_norm)]
+    out += [single] * self._num_kernel_hps()
+    if self.kernel_type == 'esp':
+      dscr = [[0.5, 1.5, 2.5]] if (self.esp_kernel_type == 'matern' and self.esp_matern_nu < 0) else []
+      if self.esp_order == -1:
+        dscr.append(list(range(1, max(self.dim, self.esp_order) + 1)))
+      return np.array(out), dscr
+    if tune_nu is None:
+      tune_nu = self.kernel_type == 'matern' and (self.nu is None or self.nu < 0)
+    dscr = [[0.5, 1.5, 2.5]] if (self.kernel_type == 'matern' and tune_nu) else []
+    if self.use_additive_gp:
+      dscr.append([x + 1 for x in range(self.add_max_group_size)])
+    return np.array(out), dscr
+
+  def _kernel(self, scale, hp, nu, groupings):
+    """ euclidean_gp.py:801-861 """
+    if self.kernel_type == 'esp':
+      return self._esp_kernel(scale, hp, nu)
+    bws = _pop_bandwidths(hp, self.dim, self.use_same_bandwidth)
     assert len(hp) == 0
     nu = self.nu if nu is None else nu
     if groupings is not None:
       # get_euclidean_integral_gp_kernel_with_scale (euclidean_gp.py:826-831, 850-861, 895-897): group kernels
       # with scale 1 on their own bandwidths, the outer scale on the sum
       groups = [[int(i) for i in grp] for grp in groupings]
-      make = (lambda grp: SEKernel(len(grp), 1.0, [bws[i] for i in grp])) if self.kernel_type == 'se' else \
-             (lambda grp: MaternKernel(len(grp), nu, 1.0, [bws[i] for i in grp]))
-      kern = AdditiveKernel(scale, [make(grp) for grp in groups], groups)
-    elif self.kernel_type == 'se':
-      kern = SEKernel(self.dim, scale, bws)
-    else:
-      kern = MaternKernel(self.dim, nu, scale, bws)
-    return float(mean_const), float(noise_var), kern
+      make = lambda grp: _se_or_matern(self.kernel_type, len(grp), nu, 1.0, [bws[i] for i in grp])
+      return AdditiveKernel(scale, [make(grp) for grp in groups], groups)
+    return _se_or_matern(self.kernel_type, self.dim, nu, scale, bws)
 
   def _esp_kernel(self, scale, hp, dscr):
     """ get_euclidean_integral_gp_kernel_with_scale for kernel_type 'esp' (euclidean_gp.py:816-824, 841-847,
@@ -161,27 +220,26 @@ class EuclideanHPLayout(object):
     return ESPKernelMatern(self.dim, [nu] * self.dim, scale, int(order), bws)
 
 
-class EuclideanMFHPLayout(EuclideanHPLayout):
+class EuclideanMFHPLayout(HPLayout):
   """ Hyper-parameter vector of the reference's EuclideanMFGPFitter (euclidean_gp.py:432-483, 680-709) with SE / Matern
       fidelity and domain kernels: [mean const]? [log noise]? log scale, log fidelity bandwidth(s), log domain
       bandwidth(s); at most one tuned Matern nu (fidelity or domain) as the discrete hp.  The GP lives on [z || x] rows
       with the product kernel scale * k_F(z, z') * k_D(x, x') (fidelity and domain kernels with scale 1).  An ExpDecay
       fidelity kernel has no bandwidths: EuclideanMFExpDecayHPLayout below. """
   FIDEL_KERNEL_TYPES = ('se', 'matern')
+  post_sampling_on_device = True
 
   def __init__(self, fidel_dim, domain_dim, fidel_kernel_type='se', domain_kernel_type='se', fidel_nu=2.5,
-               domain_nu=2.5, fidel_use_same_bandwidth=False, domain_use_same_bandwidth=False, **kwargs):
+               domain_nu=2.5, fidel_use_same_bandwidth=False, domain_use_same_bandwidth=False, **mean_noise):
     for kt, allowed in ((fidel_kernel_type, self.FIDEL_KERNEL_TYPES), (domain_kernel_type, ('se', 'matern'))):
       if kt not in allowed:
         raise NotImplementedError('kernel_type %s is outside the GPU hot-path scope of %s.' % (kt, type(self).__name__))
-    super(EuclideanMFHPLayout, self).__init__(fidel_dim + domain_dim, 'se', **kwargs)
+    super(EuclideanMFHPLayout, self).__init__(fidel_dim + domain_dim, **mean_noise)
     self.fidel_dim, self.domain_dim = fidel_dim, domain_dim
     self.fidel_kernel_type, self.domain_kernel_type = fidel_kernel_type, domain_kernel_type
     self.fidel_nu, self.domain_nu = fidel_nu, domain_nu
     self.fidel_use_same_bandwidth = fidel_use_same_bandwidth
     self.domain_use_same_bandwidth = domain_use_same_bandwidth
-    if self.use_additive_gp:
-      raise NotImplementedError('Additive domain kernels in the MF fitter are outside the device path.')
 
   def tuned_nus(self):
     return [self.fidel_kernel_type == 'matern' and self.fidel_nu < 0,
@@ -190,45 +248,31 @@ class EuclideanMFHPLayout(EuclideanHPLayout):
   def _num_fidel_hps(self):
     return 1 if self.fidel_use_same_bandwidth else self.fidel_dim
 
-  def num_hps(self):
-    n = 1 + self._num_fidel_hps()
-    n += 1 if self.domain_use_same_bandwidth else self.domain_dim
-    n += 1 if self.mean_func_type == 'tune' else 0
-    n += 1 if self.noise_var_type == 'tune' else 0
-    return n
+  def _num_kernel_hps(self):
+    return self._num_fidel_hps() + (1 if self.domain_use_same_bandwidth else self.domain_dim)
 
-  def bounds(self, X, Y, tune_nu=None):
-    raise NotImplementedError('Use the bounds of the reference EuclideanMFGPFitter (fitter.cts_hp_bounds).')
-
-  @staticmethod
-  def _bandwidths(hp, n, same):
-    return [np.exp(hp.pop(0))] * n if same else [np.exp(hp.pop(0)) for _ in range(n)]
+  def fitter_data(self, fitter):
+    """ The [z || x] rows the fitter's GPs are built on. """
+    X_mat = np.concatenate((np.asarray(fitter.ZZ, dtype=np.float64).reshape(len(fitter.YY), -1),
+                            np.asarray(fitter.XX, dtype=np.float64).reshape(len(fitter.YY), -1)), axis=1)
+    return X_mat, np.array(fitter.YY)
 
   def _fidel_kernel(self, hp, nu):
     """ Pops the fidelity kernel's hps from the front of `hp` (after the scale) and returns the kernel (scale 1). """
-    bws = self._bandwidths(hp, self.fidel_dim, self.fidel_use_same_bandwidth)
-    if self.fidel_kernel_type == 'se':
-      return SEKernel(self.fidel_dim, 1.0, bws)
-    return MaternKernel(self.fidel_dim, nu, 1.0, bws)
+    bws = _pop_bandwidths(hp, self.fidel_dim, self.fidel_use_same_bandwidth)
+    return _se_or_matern(self.fidel_kernel_type, self.fidel_dim, nu, 1.0, bws)
 
-  def unpack(self, hp, Y, nu=None, groupings=None):
-    """ gp_core.py:509-538 + euclidean_gp.py:680-709 """
-    hp = list(np.asarray(hp, dtype=np.float64))
-    Y = np.asarray(Y, dtype=np.float64)
-    mean_const, noise_var = self._mean_and_noise(hp, Y)
-    scale = np.exp(hp.pop(0))
+  def _kernel(self, scale, hp, nu, groupings):
+    """ euclidean_gp.py:680-709 """
     f_tuned, d_tuned = self.tuned_nus()
     assert not (f_tuned and d_tuned), 'at most one tuned Matern nu on the device path'
     k_f = self._fidel_kernel(hp, nu if f_tuned else self.fidel_nu)
-    d_bws = self._bandwidths(hp, self.domain_dim, self.domain_use_same_bandwidth)
+    d_bws = _pop_bandwidths(hp, self.domain_dim, self.domain_use_same_bandwidth)
     assert len(hp) == 0
-    d_nu = nu if d_tuned else self.domain_nu
-    k_d = SEKernel(self.domain_dim, 1.0, d_bws) if self.domain_kernel_type == 'se' else \
-        MaternKernel(self.domain_dim, d_nu, 1.0, d_bws)
+    k_d = _se_or_matern(self.domain_kernel_type, self.domain_dim, nu if d_tuned else self.domain_nu, 1.0, d_bws)
     fidel_coords = list(range(self.fidel_dim))
     domain_coords = list(range(self.fidel_dim, self.fidel_dim + self.domain_dim))
-    kern = CoordinateProductKernel(self.dim, scale, [k_f, k_d], [fidel_coords, domain_coords])
-    return float(mean_const), float(noise_var), kern
+    return CoordinateProductKernel(self.dim, scale, [k_f, k_d], [fidel_coords, domain_coords])
 
 
 class EuclideanMFExpDecayHPLayout(EuclideanMFHPLayout):
@@ -237,6 +281,7 @@ class EuclideanMFExpDecayHPLayout(EuclideanMFHPLayout):
       into ExpDecayKernel(fidel_dim, 1.0, exp(offset), exp(powers)) (get_euclidean_integral_gp_kernel_with_scale,
       :871-877); fidel_use_same_bandwidth plays no part, as in the reference.  The domain kernel is SE or Matern. """
   FIDEL_KERNEL_TYPES = ('expdecay',)
+  post_sampling_on_device = False                    # stays with the reference
 
   def __init__(self, fidel_dim, domain_dim, domain_kernel_type='se', domain_nu=2.5, domain_use_same_bandwidth=False,
                **kwargs):
@@ -275,7 +320,7 @@ class CPPart(object):
     return self.nu if isinstance(self.nu, (int, float)) and not isinstance(self.nu, bool) else None
 
 
-class CartesianProductHPLayout(EuclideanHPLayout):
+class CartesianProductHPLayout(HPLayout):
   """ Hyper-parameter vector of the reference's CPGPFitter (cartesian_product_gp.py:325-391, 504-678, 817-945):
       [mean const]? [log noise]? log kernel scale, then per part in domain order
         euclidean / integral / prod_discrete_numeric (se, matern): one log bandwidth per dimension;
@@ -286,6 +331,9 @@ class CartesianProductHPLayout(EuclideanHPLayout):
       children carry this layout's CategoryCodes tables, so the rows of encode() and every kernel of a batch share one
       encoding.  Options the reference itself cannot build with (use_same_bandwidth, an integer or zero Matern nu) and
       parts outside the device path raise NotImplementedError. """
+  max_dscr_hps = None         # one nu per tuned Matern part
+  mixed = True
+  ml_fit_batched = True       # one dfb_lml_batch_mixed launch per batch up to LML_BATCH_MAX_N
 
   def __init__(self, parts, mean_func_type='median', mean_func_const=0.0, noise_var_type='tune', noise_var_label=0.05,
                noise_var_value=0.1):
@@ -305,13 +353,14 @@ class CartesianProductHPLayout(EuclideanHPLayout):
           raise NotImplementedError('kernel_type %s on a prod_discrete part.' % (p.kernel_type))
       else:
         raise NotImplementedError('%s parts are outside the device path.' % (p.dom_type))
-    dim = sum(p.dim for p in parts)
-    super(CartesianProductHPLayout, self).__init__(dim, 'se', mean_func_type=mean_func_type,
-                                                   mean_func_const=mean_func_const, noise_var_type=noise_var_type,
-                                                   noise_var_label=noise_var_label, noise_var_value=noise_var_value)
-    self.kernel_type = 'cartesian_product'
+    super(CartesianProductHPLayout, self).__init__(sum(p.dim for p in parts), mean_func_type, mean_func_const,
+                                                   noise_var_type, noise_var_label, noise_var_value)
     self.parts = parts
     self.codes = [CategoryCodes() if p.dom_type == 'prod_discrete' else None for p in parts]
+    # not with a tuned nu: the reference's sampler takes hp i as discrete when param_order[i] says so
+    # (gp_core.py:689-697), and CPGPFitter lists a part's nu before that part's bandwidths, so its fit fails or samples
+    # bandwidths as categories
+    self.post_sampling_on_device = self.num_dscr() == 0
 
   @staticmethod
   def _num_part_hps(p):
@@ -321,16 +370,23 @@ class CartesianProductHPLayout(EuclideanHPLayout):
       return 0
     return 1 if p.dim == 2 else p.dim
 
-  def num_hps(self):
-    n = 1 + sum(self._num_part_hps(p) for p in self.parts)
-    n += 1 if self.mean_func_type == 'tune' else 0
-    n += 1 if self.noise_var_type == 'tune' else 0
-    return n
+  def _num_kernel_hps(self):
+    return sum(self._num_part_hps(p) for p in self.parts)
 
   def num_dscr(self):
     return sum(p.nu_tuned() for p in self.parts)
 
-  def bounds(self, X, Y, tune_nu=None):
+  def dscr_arg(self, dscr_row):
+    return tuple(dscr_row)
+
+  def gp_on(self, points, rows):
+    from .cartesian_product_gp import CPGP
+    return CPGP, list(points)                        # CPGPFitter's list-of-parts points
+
+  def fitter_data(self, fitter):
+    return list(fitter.X), np.array(fitter.Y)
+
+  def bounds(self, X, Y):
     """ (cts_hp_bounds, dscr_hp_vals) of CPGPFitter._child_set_up on list-of-parts points X. """
     cts, dscr, _ = self.bounds_and_order(X, Y)
     return cts, dscr
@@ -383,17 +439,15 @@ class CartesianProductHPLayout(EuclideanHPLayout):
       rows.append(np.concatenate(cols))
     return np.ascontiguousarray(np.array(rows, dtype=np.float64).reshape(len(rows), self.dim))
 
-  def unpack(self, hp, Y, nu=None, groupings=None):
-    """ gp_core.py:509-538 + CPGPFitter._child_build_gp / _build_kernel_for_domain (cartesian_product_gp.py:379-391,
-        817-945).  `nu`: the tuple of discrete hps, one per tuned Matern part in part order. """
+  rows = encode
+
+  def _kernel(self, scale, hp, nu, groupings):
+    """ CPGPFitter._child_build_gp / _build_kernel_for_domain (cartesian_product_gp.py:379-391, 817-945).  `nu`: the
+        tuple of discrete hps, one per tuned Matern part in part order. """
     from .cartesian_product_gp import CartesianProductKernel
     assert groupings is None
-    hp = list(np.asarray(hp, dtype=np.float64))
-    Y = np.asarray(Y, dtype=np.float64)
-    mean_const, noise_var = self._mean_and_noise(hp, Y)
     dscr = [] if nu is None else list(nu)
-    scale = np.exp(hp[0])
-    hp = np.array(hp[1:])
+    hp = np.array(hp)
     kernels = []
     for p, table in zip(self.parts, self.codes):
       if p.dom_type == 'prod_discrete':
@@ -412,17 +466,14 @@ class CartesianProductHPLayout(EuclideanHPLayout):
       else:
         bws = np.exp(hp[0:p.dim])
         hp = hp[p.dim:]
-        if p.kernel_type == 'se':
-          kern = SEKernel(p.dim, 1.0, bws)
+        if p.nu_tuned():
+          part_nu, dscr = dscr[0], dscr[1:]
         else:
-          if p.nu_tuned():
-            part_nu, dscr = dscr[0], dscr[1:]
-          else:
-            part_nu = p.fixed_nu()
-          kern = MaternKernel(p.dim, part_nu, 1.0, bws)
+          part_nu = p.fixed_nu()
+        kern = _se_or_matern(p.kernel_type, p.dim, part_nu, 1.0, bws)
       kernels.append(kern)
     assert len(hp) == 0 and len(dscr) == 0
-    return float(mean_const), float(noise_var), CartesianProductKernel(scale, kernels)
+    return CartesianProductKernel(scale, kernels)
 
 
 # One LML-only build at N = 5000 is a 40-step dependency chain (chol_diag -> panel -> next column) that leaves most
@@ -449,9 +500,9 @@ def _lane_worker(lane_post, stream, X, Y, hps, idxs, layout, nus, out, groupings
 
 
 def lml_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=None, lanes=None, groupings=None):
-  """ LML of the GP built from each hp vector (rows of `hps`); `nus` optionally gives the discrete
-      Matern nu per sample.  Returns (lmls, post) -- `post` can be passed back in to reuse the
-      device workspaces (it carries the extra lanes). """
+  """ LML of the GP built from each hp vector (rows of `hps`); `nus` optionally gives, per sample, what the layout
+      takes for its discrete hps (HPLayout.dscr_arg).  Returns (lmls, post) -- `post` can be passed back in to reuse
+      the device workspaces (it carries the extra lanes). """
   import threading
   import torch
   from .device import DevicePosterior
@@ -502,15 +553,15 @@ LML_BATCH_MAX_N = 512
 
 
 def lml_batch_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=None):
-  """ What lml_for_hyperparams returns, with every LML of a plain (not ESP, not additive) layout on N <= LML_BATCH_MAX_N
-      points from ONE dfb_lml_batch call (dfb_lml_batch_mixed for a CartesianProductHPLayout, whose kernels have Hamming
-      factors; X is then its encode()d rows).  Items that are not positive definite are rebuilt one at a time through
-      stable_cholesky_on_device (its jitter ladder), as lml_for_hyperparams builds them.  Returns (lmls, post). """
+  """ What lml_for_hyperparams returns (same `nus`), with every LML of a layout that is lml_batchable (not ESP, not
+      additive) on N <= LML_BATCH_MAX_N points from ONE dfb_lml_batch call (dfb_lml_batch_mixed for a layout that is
+      `mixed`: a CartesianProductHPLayout, whose kernels have Hamming factors; X is then its encode()d rows).  Items that
+      are not positive definite are rebuilt one at a time through stable_cholesky_on_device (its jitter ladder), as
+      lml_for_hyperparams builds them.  Returns (lmls, post). """
   from .device import DevicePosterior
   X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
   Y = np.asarray(Y, dtype=np.float64)
-  if (len(X) > LML_BATCH_MAX_N or getattr(layout, 'kernel_type', None) == 'esp' or
-      getattr(layout, 'use_additive_gp', False)):
+  if len(X) > LML_BATCH_MAX_N or not layout.lml_batchable:
     return lml_for_hyperparams(X, Y, hps, layout, nus=nus, post=post, device=device)
   if post is None or post.n_max < len(X):
     post = DevicePosterior(len(X), device=device)
@@ -526,7 +577,7 @@ def lml_batch_for_hyperparams(X, Y, hps, layout, nus=None, post=None, device=Non
     means.append(mean_const)
   if not descs:
     return np.empty(0), post
-  lmls, infos = post.lml_batch(descs, noise, means, mixed=isinstance(layout, CartesianProductHPLayout))
+  lmls, infos = post.lml_batch(descs, noise, means, mixed=layout.mixed)
   bad = np.nonzero(infos != 0)[0]
   for i in bad:
     post.set_train(X, Y - means[i])
@@ -562,34 +613,19 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
                              gp_core.py:439-445): one call for all samples.
       The global NumPy RNG is consumed exactly like the reference does, so a seeded run picks the same
       hyper-parameters.  `cts_hp_bounds` / `dscr_hp_vals` are the fitter's (euclidean_gp.py:222-320); the discrete
-      hps are the Matern nu (and for additive models the group size), or for an ESP layout [nu]? [order]?.  Returns what the reference returns:
+      hps are what the layout says they are (HPLayout.dscr_arg), X its points (HPLayout.rows: the list-of-parts points
+      of a CartesianProductHPLayout).  Returns what the reference returns:
         ('fitted_gp', gp, (cts_hps, dscr_hps))   or   ('sample_hps_with_probs', cts, dscr, [None] * n, probs). """
   from itertools import product as itertools_product
-  from .gp_core import GP, ConstantMean
   from .gpb_acquisitions import map_to_bounds, _reference_fortran_direct_available
-  cp = isinstance(layout, CartesianProductHPLayout)
-  if cp:
-    X_parts = list(X)                                # CPGPFitter's list-of-parts points
-    X = layout.encode(X_parts)
-  X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
+  points, X = X, layout.rows(X)
   Y = np.asarray(Y, dtype=np.float64)
   bounds = np.asarray(cts_hp_bounds, dtype=np.float64)
   dscr_hp_vals = [list(v) for v in dscr_hp_vals]
-  additive = bool(getattr(layout, 'use_additive_gp', False))
-  esp = getattr(layout, 'kernel_type', None) == 'esp'
-  if not cp and len(dscr_hp_vals) > (2 if additive or esp else 1):
+  additive = bool(layout.use_additive_gp)
+  if layout.max_dscr_hps is not None and len(dscr_hp_vals) > layout.max_dscr_hps:
     raise NotImplementedError('Discrete hyper-parameters on the device path: the Matern nu and, for additive '
                               'models, the group size.')
-  has_nu = len(dscr_hp_vals) == (2 if additive else 1)       # [nu]? then [group size]? (euclidean_gp.py:226-248)
-
-  def kernel_dscr(dscr):
-    """ What unpack / lml_for_hyperparams take per sample: nu (SE / Matern), the tuple [nu]? [order]? (ESP), or the
-        tuple of every tuned Matern nu (Cartesian product). """
-    if cp:
-      return tuple(dscr)
-    if esp:
-      return tuple(dscr) if len(dscr) else None
-    return dscr[0] if has_nu else None
   dim = layout.dim
   if max_evals is None:
     max_evals = default_max_evals(method, len(bounds) + len(dscr_hp_vals))
@@ -597,7 +633,7 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   state = {'post': None}
 
   def lmls_of(hps, nus, groupings=None):
-    if cp:                                           # one dfb_lml_batch_mixed launch per batch up to LML_BATCH_MAX_N
+    if layout.ml_fit_batched:
       vals, state['post'] = lml_batch_for_hyperparams(X, Y, hps, layout, nus=nus, post=state['post'], device=device)
       return vals
     vals, state['post'] = lml_for_hyperparams(X, Y, hps, layout, nus=nus, post=state['post'], device=device,
@@ -607,13 +643,10 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
   def build(cts, dscr, groupings=None):
     if build_gp is not None:                         # e.g. the reference fitter's own build_gp (fit_gp_on_fitter)
       return build_gp(cts, dscr, groupings)
-    mean_const, noise_var, kern = layout.unpack(cts, Y, kernel_dscr(dscr), groupings)
-    if cp:
-      from .cartesian_product_gp import CPGP
-      make = CPGP if gp_factory is None else gp_factory
-      return make(X_parts, list(Y), kern, ConstantMean(mean_const), noise_var)
-    make = GP if gp_factory is None else gp_factory
-    return make(list(X), list(Y), kern, ConstantMean(mean_const), noise_var)
+    mean_const, noise_var, kern = layout.unpack(cts, Y, layout.dscr_arg(dscr), groupings)
+    gp_class, gp_points = layout.gp_on(points, X)
+    make = gp_class if gp_factory is None else gp_factory
+    return make(gp_points, list(Y), kern, ConstantMean(mean_const), noise_var)
 
   def random_grouping(group_size):
     rand_perm = list(np.random.permutation(dim))               # euclidean_gp.py:733-735, 760-761
@@ -632,14 +665,14 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
         cur[-1] = group_size
         dscr.append(cur)
         cts.append(map_to_bounds(np.random.random((len(bounds),)), bounds))
-      vals = lmls_of(np.array(cts), [d[0] for d in dscr] if has_nu else None, groupings)
+      nus = [layout.dscr_arg(d) for d in dscr]
+      vals = lmls_of(np.array(cts), None if all(nu is None for nu in nus) else nus, groupings)
       probs = np.exp(vals)
-      from argparse import Namespace
       other = [Namespace(add_gp_groupings=grp) for grp in groupings]      # as the reference returns them (:762)
       return 'sample_hps_with_probs', cts, dscr, other, probs / probs.sum()
     cts = map_to_bounds(np.random.random((n_evals, len(bounds))), bounds)
     dscr = [[np.random.choice(categ) for categ in dscr_hp_vals] for _ in range(n_evals)]
-    vals = lmls_of(cts, [kernel_dscr(d) for d in dscr] if dscr_hp_vals else None)
+    vals = lmls_of(cts, [layout.dscr_arg(d) for d in dscr] if dscr_hp_vals else None)
     return 'sample_hps_with_probs', cts, dscr, [None] * n_evals, rand_exp_sampling_probs(vals)
   if method == 'direct' and _reference_fortran_direct_available():
     raise NotImplementedError('Fortran DIRECT is a sequential host optimiser; use pdoo / rand / rand_exp_sampling.')
@@ -661,7 +694,7 @@ def fit_gp(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), method='rand_exp_sampli
 
   best_val, best_cts, best_dscr, best_groupings = -np.inf, None, None, None
   for dscr in itertools_product(*dscr_hp_vals):
-    nu = kernel_dscr(dscr)
+    nu = layout.dscr_arg(dscr)
     if not additive:
       opt_val, opt_pt, opt_groupings = optimise_cts(nu, max_evals) + (None,)
     else:
@@ -721,12 +754,9 @@ def layout_from_fitter(fitter):
     return None
   return EuclideanHPLayout(
       fitter.dim, kernel_type, nu=getattr(opt, 'matern_nu', 2.5),
-      use_same_bandwidth=bool(getattr(opt, 'use_same_bandwidth', False)),
-      mean_func_type=opt.mean_func_type, mean_func_const=getattr(opt, 'mean_func_const', 0.0),
-      noise_var_type=opt.noise_var_type, noise_var_label=getattr(opt, 'noise_var_label', 0.05),
-      noise_var_value=getattr(opt, 'noise_var_value', 0.1), use_additive_gp=additive,
+      use_same_bandwidth=bool(getattr(opt, 'use_same_bandwidth', False)), use_additive_gp=additive,
       add_max_group_size=getattr(fitter, 'add_max_group_size', getattr(opt, 'add_max_group_size', 6)),
-      num_groups_per_group_size=getattr(opt, 'num_groups_per_group_size', -1))
+      num_groups_per_group_size=getattr(opt, 'num_groups_per_group_size', -1), **common)
 
 
 _CP_OPTION_CODES = {'euclidean': 'euc', 'integral': 'int', 'prod_discrete_numeric': 'disc_num', 'prod_discrete': 'disc'}
@@ -772,47 +802,22 @@ def _cp_layout_from_fitter(fitter, common):
     return None
 
 
-def post_sampling_covers(layout):
-  """ The layouts whose 'post_sampling' fits run on the device (post_sampling.post_sample_hps): SE / Matern, not
-      additive; the MF product of SE / Matern fidelity and domain kernels; Cartesian products of SE / Matern and Hamming
-      parts without a tuned nu.  ESP and ExpDecay stay with the reference, and so do CP fitters with a tuned nu: the
-      reference's sampler takes hp i as discrete when param_order[i] says so (gp_core.py:689-697), and CPGPFitter lists a
-      part's nu before that part's bandwidths, so its fit fails or samples bandwidths as categories. """
-  if type(layout) is EuclideanHPLayout:
-    return layout.kernel_type in ('se', 'matern') and not layout.use_additive_gp
-  if type(layout) is CartesianProductHPLayout:
-    return layout.num_dscr() == 0
-  return type(layout) is EuclideanMFHPLayout
-
-
-def _fitter_data(fitter, layout):
-  """ The rows the fitter's GPs are built on: [z || x] for an MF fitter, the list-of-parts points for a CP fitter (the
-      layout encodes them). """
-  if isinstance(layout, CartesianProductHPLayout):
-    return list(fitter.X), np.array(fitter.Y)
-  if isinstance(layout, EuclideanMFHPLayout):
-    X_mat = np.concatenate((np.asarray(fitter.ZZ, dtype=np.float64).reshape(len(fitter.YY), -1),
-                            np.asarray(fitter.XX, dtype=np.float64).reshape(len(fitter.YY), -1)), axis=1)
-    return X_mat, np.array(fitter.YY)
-  return np.array(fitter.X), np.array(fitter.Y)
-
-
 def fit_gp_on_fitter(fitter, reference_fit_gp, num_samples=1, hp_tune_criterion=None):
   """ GPFitter.fit_gp (gp_core.py:783-821) for a reference EuclideanGPFitter instance: hp_tune_criterion 'ml' with
       ml_hp_tune_opt rand / rand_exp_sampling / pdoo / direct-without-Fortran runs fit_gp above (every batch of
       _tuning_objective evaluations as one lml_for_hyperparams call; same global-RNG consumption, same selection,
       the final GP built by the fitter's own build_gp); 'post_sampling' with the slice sampler on a layout that
-      post_sampling_covers runs post_sampling.post_sample_hps; everything else is handed to `reference_fit_gp`. """
-  from argparse import Namespace
+      is post_sampling_on_device runs post_sampling.post_sample_hps; everything else is handed to `reference_fit_gp`. """
   from .gpb_acquisitions import _reference_fortran_direct_available
   crit = fitter.options.hp_tune_criterion if hp_tune_criterion is None else hp_tune_criterion
   method = getattr(fitter, 'ml_hp_tune_opt_method', None)
   if crit == 'post_sampling':
     layout = layout_from_fitter(fitter)
-    if getattr(fitter.options, 'post_hp_tune_method', None) != 'slice' or not post_sampling_covers(layout):
+    if (getattr(fitter.options, 'post_hp_tune_method', None) != 'slice' or layout is None or
+        not layout.post_sampling_on_device):
       return reference_fit_gp(fitter, num_samples, hp_tune_criterion)
     from .post_sampling import post_sample_hps
-    X_mat, Y_vec = _fitter_data(fitter, layout)
+    X_mat, Y_vec = layout.fitter_data(fitter)
     return post_sample_hps(X_mat, Y_vec, layout, fitter.cts_hp_bounds, fitter.dscr_hp_vals, num_samples=num_samples,
                            offset=fitter.options.post_hp_tune_offset, burn=fitter.options.post_hp_tune_burn,
                            build_gp=lambda cts, dscr: fitter.build_gp(cts, dscr, other_gp_params=None))
@@ -821,7 +826,7 @@ def fit_gp_on_fitter(fitter, reference_fit_gp, num_samples=1, hp_tune_criterion=
       (method == 'direct' and _reference_fortran_direct_available())):
     return reference_fit_gp(fitter, num_samples, hp_tune_criterion)
   other = lambda grp: None if grp is None else Namespace(add_gp_groupings=grp)
-  X_mat, Y_vec = _fitter_data(fitter, layout)
+  X_mat, Y_vec = layout.fitter_data(fitter)
   return fit_gp(X_mat, Y_vec, layout, fitter.cts_hp_bounds, fitter.dscr_hp_vals,
                 method=method, max_evals=fitter.hp_tune_max_evals,
                 build_gp=lambda cts, dscr, grp: fitter.build_gp(cts, dscr, other_gp_params=other(grp)))
@@ -847,7 +852,6 @@ def rand_exp_sampling_probs(lml_vals):
 def sharded_lml_grid(X, Y, hps, layout, nus=None, device=None, group=None):
   """ Rank r evaluates hps[lo:hi]; one all-gather of the fp64 LML values.  Every rank returns the
       full vector and the rand_exp_sampling probabilities. """
-  import torch
   import torch.distributed as dist
   from .dist import shard_bounds
   hps = np.asarray(hps, dtype=np.float64)

@@ -23,7 +23,7 @@ Without ever-rejected speculation an LML is evaluated once, so the consumed sequ
 """
 import numpy as np
 
-from .hp_grid import lml_batch_for_hyperparams, LML_BATCH_MAX_N, CartesianProductHPLayout
+from .hp_grid import lml_batch_for_hyperparams, LML_BATCH_MAX_N
 
 # Speculation depth where one batch is one dfb_lml_batch launch (N <= LML_BATCH_MAX_N).  Above the cap every LML is a
 # build of its own, so speculation only adds builds: depth 1 there (DESIGN.md 10: 37.7 s against 96.6 s per fit at
@@ -41,18 +41,15 @@ class PostSamplingStats(object):
     self.round_trips = 0
 
 
-def device_lml_batch(X, Y, layout, has_nu, device=None, batch_fn=lml_batch_for_hyperparams):
+def device_lml_batch(X, Y, layout, device=None, batch_fn=lml_batch_for_hyperparams):
   """ The sampler's default LML source: batch_fn (lml_batch_for_hyperparams or lml_for_hyperparams) on one posterior
-      that is kept across calls. """
+      that is kept across calls, each item with what the layout takes for its discrete hps (HPLayout.dscr_arg). """
   state = {'post': None}
 
-  cp = isinstance(layout, CartesianProductHPLayout)
-
   def lml_batch(cts_rows, dscr_rows):
-    if cp:                                   # every tuned Matern nu of the product, as one tuple per item
-      nus = [tuple(d) for d in dscr_rows]
-    else:
-      nus = [d[0] for d in dscr_rows] if has_nu else None
+    nus = [layout.dscr_arg(d) for d in dscr_rows]
+    if all(nu is None for nu in nus):
+      nus = None
     vals, state['post'] = batch_fn(X, Y, np.array(cts_rows), layout, nus=nus, post=state['post'], device=device)
     return vals
   return lml_batch
@@ -263,26 +260,24 @@ class _Sampler(object):
 
 def post_sample_hps(X, Y, layout, cts_hp_bounds, dscr_hp_vals=(), num_samples=1, offset=25, burn=-1, build_gp=None,
                     lml_batch=None, depth=None, device=None, stats=None, trace=None):
-  """ GPFitter.fit_gp(num_samples, 'post_sampling') with the slice sampler (gp_core.py:592-726, 811-821) on an
-      EuclideanHPLayout / EuclideanMFHPLayout.  `cts_hp_bounds` / `dscr_hp_vals` are the fitter's; `offset` and `burn`
+  """ GPFitter.fit_gp(num_samples, 'post_sampling') with the slice sampler (gp_core.py:592-726, 811-821) on any
+      hp_grid.HPLayout.  `cts_hp_bounds` / `dscr_hp_vals` are the fitter's; `offset` and `burn`
       its post_hp_tune_offset / post_hp_tune_burn (-1: int(sqrt(num_hps) * 100), unclipped as in the reference).
       `build_gp(cts, dscr)` builds the returned GP when num_samples == 1.  `lml_batch(cts_rows, dscr_rows)` returns the
       LMLs of a batch (default: device_lml_batch); `depth` bounds the speculation (default: DEFAULT_DEPTH up to
       LML_BATCH_MAX_N training points, 1 above).  `stats` (PostSamplingStats) and
       `trace` (a list: (hp vector, LML) per consumed LML, in the reference's order) are filled when given.  Returns
       ('post_fitted_gp', gp, (cts, dscr)) or ('post_sample_hps_with_probs', cts, dscr, [None] * num_samples).
-      With a CartesianProductHPLayout X holds CPGPFitter's list-of-parts points (encoded here) and there may be a
-      discrete hp per tuned Matern part: each has its own Metropolis chain, and every LML item gets the whole tuple. """
-  cp = isinstance(layout, CartesianProductHPLayout)
-  if cp:
-    X = layout.encode(X)
-  X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
+      X holds the points the layout's rows() takes: with a CartesianProductHPLayout CPGPFitter's list-of-parts points
+      (encoded here), and there may then be a discrete hp per tuned Matern part: each has its own Metropolis chain, and
+      every LML item gets the whole tuple. """
+  X = layout.rows(X)
   Y = np.asarray(Y, dtype=np.float64)
   dscr_hp_vals = [list(v) for v in dscr_hp_vals]
-  if len(dscr_hp_vals) > 1 and not cp:
-    raise NotImplementedError('One discrete hyper-parameter (the Matern nu) on the device path.')
+  if layout.max_dscr_hps is not None and len(dscr_hp_vals) > layout.max_dscr_hps:
+    raise NotImplementedError('More discrete hyper-parameters than the layout takes on the device path.')
   if lml_batch is None:
-    lml_batch = device_lml_batch(X, Y, layout, len(dscr_hp_vals) == 1, device=device)
+    lml_batch = device_lml_batch(X, Y, layout, device=device)
   if depth is None:
     depth = DEFAULT_DEPTH if len(X) <= LML_BATCH_MAX_N else 1
   stats = PostSamplingStats() if stats is None else stats

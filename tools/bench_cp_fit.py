@@ -102,7 +102,7 @@ def main():
             batch_fn = orig if arm == 'batched' else single_batch
             post_sampling.post_sample_hps(X, Y, lay, bounds, dscr, num_samples=1, burn=args.burn,
                                           build_gp=lambda c, d: None, stats=stats, depth=None if arm == 'batched'
-                                          else 1, lml_batch=post_sampling.device_lml_batch(Xc, Y, lay, False,
+                                          else 1, lml_batch=post_sampling.device_lml_batch(Xc, Y, lay,
                                                                                            batch_fn=batch_fn))
             lmls = stats.consumed
           torch.cuda.synchronize()

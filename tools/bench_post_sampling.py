@@ -74,7 +74,7 @@ def whole_fit(sizes, burn, reps, num_samples):
     samples = {}
     for _ in range(reps):
       for name, fn, depth in arms:
-        src = post_sampling.device_lml_batch(X, Y, layout, True, batch_fn=fn)
+        src = post_sampling.device_lml_batch(X, Y, layout, batch_fn=fn)
         ms, st, res = _fit(X, Y, layout, bounds, dscr, burn, num_samples, src, depth)
         results[name].append((ms, st))
         samples[name] = (np.array(res[1]), np.array(res[2]))
