@@ -268,19 +268,59 @@ static int launch_train_kstar(dfb_handle* h, int64_t row0, int64_t m_rows, doubl
   return launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS));
 }
 
-// The blocked right-looking factorisation of the tall matrix [A ; I ; y^T] (see gemm.cuh):
+// ---- optional per-class event timing -------------------------------------------------------------
+static int prof_flush(dfb_handle* h, int cls) {
+  ProfClass& pc = h->prof[cls];
+  if (pc.n == 0) return 0;
+  DFB_CUDA_OK(cudaEventSynchronize(pc.stop[pc.n - 1]));
+  for (int i = 0; i < pc.n; i++) {
+    float ms = 0.f;
+    DFB_CUDA_OK(cudaEventElapsedTime(&ms, pc.start[i], pc.stop[i]));
+    pc.acc_ms += ms;
+    pc.acc_units += pc.units[i];
+    pc.acc_launches += 1;
+  }
+  pc.n = 0;
+  return 0;
+}
+// cls < 0: the interval is not profiled
+static int prof_begin(dfb_handle* h, int cls) {
+  if (!h->prof_on || cls < 0) return 0;
+  ProfClass& pc = h->prof[cls];
+  if (!pc.created) {
+    for (int i = 0; i < PROF_RING; i++) {
+      DFB_CUDA_OK(cudaEventCreate(&pc.start[i]));
+      DFB_CUDA_OK(cudaEventCreate(&pc.stop[i]));
+    }
+    pc.created = true;
+  }
+  if (pc.n == PROF_RING) DFB_TRY(prof_flush(h, cls));
+  DFB_CUDA_OK(cudaEventRecord(pc.start[pc.n], h->stream));
+  return 0;
+}
+static int prof_end(dfb_handle* h, int cls, double units) {
+  if (!h->prof_on || cls < 0) return 0;
+  ProfClass& pc = h->prof[cls];
+  DFB_CUDA_OK(cudaEventRecord(pc.stop[pc.n], h->stream));
+  pc.units[pc.n] = units;
+  pc.n++;
+  return 0;
+}
+
+// The blocked right-looking factorisation of the tall matrix [A ; I ; y^T] (factor_tma.cuh):
 // top -> L, bottom -> L^-T, y row -> (L^-1 y)^T.
 //
-// Schedule: chol_diag is a one-CTA, latency-bound kernel (~0.1 ms x npad/128 steps), so the plain
-// step-after-step order leaves 147 SMs idle for a third of the build.  With look-ahead the trailing update of
+// Schedule: chol_diag is a one-CTA, latency-bound kernel run once per step (npad/128 steps), so in the plain
+// step-after-step order the other SMs wait for it at every step.  With look-ahead the trailing update of
 // step k is split: the column of the NEXT panel (block k+1) is updated first on the critical-path stream, so
 // chol_diag(k+1) and the panel solve of step k+1 run while the bulk of update k (column blocks >= k+2) is still
 // in flight on a second stream.
 //   hi:  chol(k) panel(k) [P_k] wait(R_k-1) next(k)  chol(k+1) panel(k+1) [P_k+1] wait(R_k) next(k+1) ...
 //   lo:                   wait(P_k) rest(k) [R_k]                         wait(P_k+1) rest(k+1) [R_k+1]
 // next(k) and rest(k-1) both accumulate into column block k+1, hence wait(R_k-1); rest(k) after rest(k-1) by
-// stream order.  The arithmetic per tile is unchanged (same kernel, same k-order): results are bit-identical
-// to the single-stream schedule.
+// stream order.  panel(k) and next(k) take factor_update_kernel's small chain shape, so each spreads over ~4x as many
+// SMs as it has 128 x 128 tiles; the bulk launches take its throughput shape.  The arithmetic per element does not
+// depend on the shape or the stream: results are bit-identical to the single-stream schedule.
 struct StreamSwap {
   dfb_handle* h;
   cudaStream_t user;
@@ -299,10 +339,22 @@ static int ensure_factor_streams(dfb_handle* h) {
   return 0;
 }
 
+// One launch of factor_update_kernel inside an interval of profiling class cls (< 0: none).
+static int factor_update(dfb_handle* h, const FactorMaps& m, const FactorArgs& g, bool chain, int cls) {
+  DFB_TRY(prof_begin(h, cls));
+  DFB_TRY(launch_factor_update(h, m, g, chain));
+  return prof_end(h, cls, 1.0);
+}
+
+// profile: time the stages in the DFB_PROF_BUILD_* classes (the posterior build; not the Thompson blocks)
 static int factorise_tall(dfb_handle* h, double* T, int64_t npad, double* Dinv, int* info,
-                          bool with_bottom) {
+                          bool with_bottom, bool profile) {
   const int nb = (int)(npad / TILE);
+  const int c_chol = profile ? DFB_PROF_BUILD_CHOL : -1, c_chain = profile ? DFB_PROF_BUILD_CHAIN : -1;
+  const int c_rest = profile ? DFB_PROF_BUILD_REST : -1;
   const bool la = h->lookahead != 0 && nb >= 4;
+  FactorMaps maps;
+  DFB_TRY(make_factor_maps(&maps, T, npad, Dinv));
   StreamSwap guard(h);
   if (la) {
     DFB_TRY(ensure_factor_streams(h));
@@ -313,30 +365,30 @@ static int factorise_tall(dfb_handle* h, double* T, int64_t npad, double* Dinv, 
   bool rest_pending = false;
   for (int step = 0; step < nb; step++) {
     if (la) h->stream = h->fs_hi;
+    DFB_TRY(prof_begin(h, c_chol));
     DFB_TRY(launch_chol_diag(h, T, npad, step, Dinv, info));
-    GemmArgs g;
+    DFB_TRY(prof_end(h, c_chol, 1.0));
+    FactorArgs g;
     memset(&g, 0, sizeof(g));
-    g.A = T; g.lda = npad; g.B = Dinv; g.ldb = TILE; g.D = T; g.ldd = npad;
-    g.alpha = 1.0; g.mode = MODE_PANEL; g.K = TILE; g.step = step; g.nb = nb; g.info = info;
-    g.skip_bottom = with_bottom ? 0 : 1;
-    const int rows = 2 * nb + 1 - (step + 1);
-    DFB_TRY(launch_gemm(h, g, EPI_STORE, rows));
-    const int ncols = nb - step - 1;
-    if (ncols <= 0) continue;
-    g.mode = MODE_TRAIL; g.alpha = -1.0; g.B = nullptr; g.ldb = npad;
+    g.T = T; g.ld = npad; g.step = step; g.nb = nb; g.skip_bottom = with_bottom ? 0 : 1; g.info = info;
+    g.panel = 1;
+    DFB_TRY(factor_update(h, maps, g, true, c_chain));
+    if (step + 1 >= nb) continue;
+    g.panel = 0;
     if (!la) {
-      DFB_TRY(launch_gemm(h, g, EPI_STORE, rows * ncols));
+      g.j0 = step + 1; g.j1 = nb;
+      DFB_TRY(factor_update(h, maps, g, false, c_rest));
       continue;
     }
     DFB_CUDA_OK(cudaEventRecord(h->fe_panel, h->fs_hi));
     if (rest_pending) DFB_CUDA_OK(cudaStreamWaitEvent(h->fs_hi, h->fe_rest, 0));
-    g.tr_j0 = 0; g.tr_nc = 1;                       // the next panel's column, on the critical path
-    DFB_TRY(launch_gemm(h, g, EPI_STORE, rows));
-    if (ncols > 1) {
+    g.j0 = step + 1; g.j1 = step + 2;                 // the next panel's column, on the critical path
+    DFB_TRY(factor_update(h, maps, g, true, c_chain));
+    if (step + 2 < nb) {
       h->stream = h->fs_lo;
       DFB_CUDA_OK(cudaStreamWaitEvent(h->fs_lo, h->fe_panel, 0));
-      g.tr_j0 = 1; g.tr_nc = ncols - 1;
-      DFB_TRY(launch_gemm(h, g, EPI_STORE, rows * (ncols - 1)));
+      g.j0 = step + 2; g.j1 = nb;
+      DFB_TRY(factor_update(h, maps, g, false, c_rest));
       DFB_CUDA_OK(cudaEventRecord(h->fe_rest, h->fs_lo));
       rest_pending = true;
     }
@@ -347,44 +399,6 @@ static int factorise_tall(dfb_handle* h, double* T, int64_t npad, double* Dinv, 
     DFB_CUDA_OK(cudaStreamWaitEvent(guard.user, h->fe_join_hi, 0));
     DFB_CUDA_OK(cudaStreamWaitEvent(guard.user, h->fe_join_lo, 0));
   }
-  return 0;
-}
-
-// ---- optional per-class event timing -------------------------------------------------------------
-static int prof_flush(dfb_handle* h, int cls) {
-  ProfClass& pc = h->prof[cls];
-  if (pc.n == 0) return 0;
-  DFB_CUDA_OK(cudaEventSynchronize(pc.stop[pc.n - 1]));
-  for (int i = 0; i < pc.n; i++) {
-    float ms = 0.f;
-    DFB_CUDA_OK(cudaEventElapsedTime(&ms, pc.start[i], pc.stop[i]));
-    pc.acc_ms += ms;
-    pc.acc_units += pc.units[i];
-    pc.acc_launches += 1;
-  }
-  pc.n = 0;
-  return 0;
-}
-static int prof_begin(dfb_handle* h, int cls) {
-  if (!h->prof_on) return 0;
-  ProfClass& pc = h->prof[cls];
-  if (!pc.created) {
-    for (int i = 0; i < PROF_RING; i++) {
-      DFB_CUDA_OK(cudaEventCreate(&pc.start[i]));
-      DFB_CUDA_OK(cudaEventCreate(&pc.stop[i]));
-    }
-    pc.created = true;
-  }
-  if (pc.n == PROF_RING) DFB_TRY(prof_flush(h, cls));
-  DFB_CUDA_OK(cudaEventRecord(pc.start[pc.n], h->stream));
-  return 0;
-}
-static int prof_end(dfb_handle* h, int cls, double units) {
-  if (!h->prof_on) return 0;
-  ProfClass& pc = h->prof[cls];
-  DFB_CUDA_OK(cudaEventRecord(pc.stop[pc.n], h->stream));
-  pc.units[pc.n] = units;
-  pc.n++;
   return 0;
 }
 
@@ -481,14 +495,18 @@ static double lml(double quad, double log_det_half, int64_t n) { return -0.5 * q
 
 // The tail of a factorisation of [A ; I ; y^T]: W = L^-1 from L^-T (unless LML-only), alpha (DFB_BUILD_FULL), the LML
 // sums, then the read-back of the sums and the pivot status.  A non-stationary training kernel reads back 7 sums: red[6]
-// is the max(diag K) launch_diag_max left.  end_build closes the DFB_PROF_BUILD interval before the read-back.
+// is the max(diag K) launch_diag_max left.  end_build (the posterior build) times the tail in
+// DFB_PROF_BUILD_TAIL and closes the DFB_PROF_BUILD interval before the read-back.
 static int posterior_tail(dfb_handle* h, int32_t flags, bool end_build, double red[7], int* info) {
   const int64_t n = h->n, npad = h->npad;
   const double* Wt = h->T + (size_t)npad * npad;
   const double* v = h->T + (size_t)2 * npad * npad;
+  const int c_tail = end_build ? DFB_PROF_BUILD_TAIL : -1;
+  DFB_TRY(prof_begin(h, c_tail));
   if (flags != DFB_BUILD_LML_ONLY) DFB_TRY(launch_transpose(h, Wt, h->W, npad));
   if (flags == DFB_BUILD_FULL) DFB_TRY(launch_alpha(h, Wt, v, h->alpha, n, npad));
   DFB_TRY(launch_lml_reduce(h, h->T, h->yc, flags == DFB_BUILD_FULL ? h->alpha : nullptr, v, n, npad, h->red));
+  DFB_TRY(prof_end(h, c_tail, 1.0));
   if (end_build) DFB_TRY(prof_end(h, DFB_PROF_BUILD, 1.0));
   const size_t red_bytes = sizeof(double) * (kernel_stationary(h->desc_tr) ? 3 : 7);
   DFB_CUDA_OK(cudaMemcpyAsync(red, h->red, red_bytes, cudaMemcpyDeviceToHost, h->stream));
@@ -565,10 +583,12 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   else DFB_TRY(launch_gemm(h, g, EPI_STORE, 1));
   // replay of factorisation step nb-1
   DFB_TRY(launch_chol_diag(h, h->T, npad, step, h->Dinv, h->info));
-  memset(&g, 0, sizeof(g));
-  g.A = h->T; g.lda = npad; g.B = h->Dinv; g.ldb = TILE; g.D = h->T; g.ldd = npad;
-  g.alpha = 1.0; g.mode = MODE_PANEL; g.K = TILE; g.step = step; g.nb = nb; g.info = h->info;
-  DFB_TRY(launch_gemm(h, g, EPI_STORE, 2 * nb + 1 - (step + 1)));
+  FactorMaps maps;
+  DFB_TRY(make_factor_maps(&maps, h->T, npad, h->Dinv));
+  FactorArgs fa;
+  memset(&fa, 0, sizeof(fa));
+  fa.T = h->T; fa.ld = npad; fa.step = step; fa.nb = nb; fa.panel = 1; fa.info = h->info;
+  DFB_TRY(launch_factor_update(h, maps, fa, true));
   double red[7];
   int info = 0;
   DFB_TRY(posterior_tail(h, flags, false, red, &info));
@@ -971,13 +991,15 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   DFB_TRY(prof_begin(h, DFB_PROF_BUILD));
   DFB_CUDA_OK(cudaMemsetAsync(h->info, 0, sizeof(int) * 4, h->stream));
   DFB_CUDA_OK(cudaMemsetAsync(h->T, 0, sizeof(double) * (size_t)(2 * npad + TILE) * npad, h->stream));
+  DFB_TRY(prof_begin(h, DFB_PROF_BUILD_KXX));
   DFB_TRY(ensure_train_scaled(h));
   DFB_TRY(launch_train_kstar(h, 0, n, h->T, npad, npad));
   // the jitter ladder's scale max(diag K) + noise: kss for a stationary kernel, else read off the diagonal just built
   const bool stationary = kernel_stationary(h->desc_tr);
   if (!stationary) DFB_TRY(launch_diag_max(h, h->T, npad, n, h->red + 6));
   DFB_TRY(launch_init_tall(h, h->T, n, npad, noise_var + jitter, h->yc, with_bottom ? 1 : 0));
-  DFB_TRY(factorise_tall(h, h->T, npad, h->Dinv, h->info, with_bottom));
+  DFB_TRY(prof_end(h, DFB_PROF_BUILD_KXX, 1.0));
+  DFB_TRY(factorise_tall(h, h->T, npad, h->Dinv, h->info, with_bottom, true));
   double red[7];
   int info = 0;
   DFB_TRY(posterior_tail(h, flags, true, red, &info));
@@ -990,7 +1012,9 @@ int dfb_build_posterior(dfb_handle* h, double noise_var, double jitter, int32_t 
   h->noise_plus_jitter = noise_var + jitter;
   h->have_post = true;
   h->have_w = with_bottom;
+  DFB_TRY(prof_begin(h, DFB_PROF_BUILD_I8));
   DFB_TRY(prepare_scoring(h, true, true));
+  DFB_TRY(prof_end(h, DFB_PROF_BUILD_I8, 1.0));
   if (lml_out_host != nullptr) *lml_out_host = lml((flags == DFB_BUILD_FULL) ? red[1] : red[2], red[0], n);
   return 0;
 }
@@ -1587,7 +1611,7 @@ int dfb_ts_draws(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, dou
   DFB_TRY(launch_copy_rows(h, h->ts_Cov, mbp, h->ts_T, mbp, mbp, mbp));
   DFB_TRY(launch_set_diag(h, h->ts_T, mbp, 0, m, jitter, 1));
   DFB_TRY(launch_set_diag(h, h->ts_T, mbp, m, mbp, 1.0, 0));
-  DFB_TRY(factorise_tall(h, h->ts_T, mbp, h->Dinv, h->ts_info, false));
+  DFB_TRY(factorise_tall(h, h->ts_T, mbp, h->Dinv, h->ts_info, false, false));
   // samples^T = L_post U: samples[s][a] = sum_{b <= a} U^T[s][b] L[a][b]
   const int64_t Sp = round_up(S, TILE);
   DFB_CUDA_OK(cudaMemsetAsync(h->ts_Ut, 0, sizeof(double) * (size_t)Sp * mbp, h->stream));

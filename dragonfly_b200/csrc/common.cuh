@@ -50,7 +50,7 @@ struct ScaledSet {        // scaled training coordinates for one kernel descript
 }  // namespace dfb
 
 namespace dfb {
-constexpr int PROF_CLASSES = 5;
+constexpr int PROF_CLASSES = 11;
 constexpr int PROF_RING = 1024;
 struct ProfClass {
   cudaEvent_t start[PROF_RING];

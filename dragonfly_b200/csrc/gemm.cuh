@@ -13,8 +13,6 @@
 //                             fused reduction |v|^2 per candidate column -- V is never stored.
 //                             Replaces solve_lower_triangular(L, K_tetr.T) + V.T.dot(V) + diag
 //                             (dragonfly/gp/gp_core.py:180-187).
-//   MODE_PANEL  + EPI_STORE : panel solve   P = P * inv(L_kk)^T       of the blocked Cholesky
-//   MODE_TRAIL  + EPI_STORE : trailing update  T -= P P_j^T            (dpotrf, general_utils.py:178)
 //   MODE_GENERIC+ EPI_STORE : plain tiles (posterior covariance / Thompson sampling blocks)
 #pragma once
 #include "common.cuh"
@@ -27,7 +25,7 @@ constexpr int GEMM_SROW = GEMM_BK + 4;                    // padded smem row: 20
 constexpr int GEMM_STAGE_DOUBLES = 2 * TILE * GEMM_SROW;  // A slab + B slab
 constexpr size_t GEMM_SMEM_BYTES = (size_t)GEMM_STAGES * GEMM_STAGE_DOUBLES * sizeof(double);
 
-enum { MODE_SCORE = 0, MODE_PANEL = 1, MODE_TRAIL = 2, MODE_GENERIC = 3 };
+enum { MODE_SCORE = 0, MODE_GENERIC = 1 };
 enum { EPI_STORE = 0, EPI_SUMSQ = 1 };
 
 struct GemmArgs {
@@ -44,10 +42,6 @@ struct GemmArgs {
   int lower_only;                   // GENERIC: skip tiles with cb > rb
   int rb0;                          // GENERIC: global index of row block 0 (A / C / D already point at it): the
                                     //   triangular ranges and lower_only refer to rb0 + rb
-  int step, nb;                     // PANEL / TRAIL: factorisation step and #top row blocks
-  int skip_bottom;                  // PANEL / TRAIL: the L^-T rows are absent (LML-only build)
-  int tr_j0, tr_nc;                 // TRAIL: column blocks step+1+tr_j0 .. +tr_nc-1 only (tr_nc = 0: all of them) --
-                                    // the look-ahead schedule updates the next panel's column first
   int ksplit;                       // GENERIC: > 1 = split the k-range of every tile over `ksplit` CTAs; slice s writes
   double* part;                     //   alpha * (its partial sum) to part + s * (n_rb*128) * (n_cb*128) (compact tiles grid,
                                     //   ld = n_cb*128) and splitk_reduce_kernel adds the slices in a fixed order (+ C)
@@ -70,13 +64,6 @@ __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double
                : "d"(a), "d"(b));
 }
 
-// Row blocks of the tall factorisation matrix [A ; I ; y^T] that are structurally non-zero in
-// column block `step`: top rows below the diagonal, bottom (L^-T) rows 0..step, the y row block.
-__device__ __forceinline__ bool tall_row_active(int rbk, int step, int nb, int skip_bottom) {
-  return (rbk > step && rbk < nb) || (!skip_bottom && rbk >= nb && rbk <= nb + step) ||
-         (rbk == 2 * nb);
-}
-
 template <int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tn_kernel(const GemmArgs g) {
   extern __shared__ __align__(16) double smem[];
@@ -93,24 +80,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tn_kernel(const GemmArgs
     A = g.A + (int64_t)rb * TILE * g.lda;
     B = g.B + (int64_t)cb * TILE * g.ldb;
     k_hi = min(g.K, (rb + 1) * TILE);
-  } else if (g.mode == MODE_PANEL) {
-    const int rbk = g.step + 1 + bid;
-    if (!tall_row_active(rbk, g.step, g.nb, g.skip_bottom)) return;
-    A = g.A + (int64_t)rbk * TILE * g.lda + (int64_t)g.step * TILE;
-    B = g.B;
-    D = g.D + (int64_t)rbk * TILE * g.ldd + (int64_t)g.step * TILE;
-    k_hi = TILE;
-  } else if (g.mode == MODE_TRAIL) {
-    const int ncols = g.tr_nc > 0 ? g.tr_nc : g.nb - g.step - 1;
-    const int rbk = g.step + 1 + bid / ncols;
-    const int j = g.step + 1 + g.tr_j0 + bid % ncols;
-    if (!tall_row_active(rbk, g.step, g.nb, g.skip_bottom)) return;
-    if (rbk < g.nb && j > rbk) return;        // top part: lower triangle only
-    A = g.A + (int64_t)rbk * TILE * g.lda + (int64_t)g.step * TILE;
-    B = g.A + (int64_t)j * TILE * g.lda + (int64_t)g.step * TILE;
-    C = g.A + (int64_t)rbk * TILE * g.lda + (int64_t)j * TILE;
-    D = g.D + (int64_t)rbk * TILE * g.ldd + (int64_t)j * TILE;
-    k_hi = TILE;
   } else {
     const int ks = g.ksplit > 1 ? g.ksplit : 1;
     const int tile = bid / ks, slice = bid - tile * ks;
@@ -136,9 +105,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tn_kernel(const GemmArgs
       D = g.D + (int64_t)rb * TILE * g.ldd + (int64_t)cb * TILE;
     }
   }
-  const int64_t lda = g.lda;
-  const int64_t ldb = (g.mode == MODE_TRAIL) ? g.lda : g.ldb;
-  const int64_t ldc = (g.mode == MODE_TRAIL) ? g.lda : g.ldc;
+  const int64_t lda = g.lda, ldb = g.ldb, ldc = g.ldc;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp >> 2, wn = warp & 3;

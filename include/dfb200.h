@@ -456,6 +456,18 @@ int dfb_query(dfb_handle* h, const char* name, double* out);
 #define DFB_PROF_ACQ   2
 #define DFB_PROF_BUILD 3
 #define DFB_PROF_PRUNE 4
+/* The stages of dfb_build_posterior alone (tools/build_breakdown.py; dfb_extend_posterior and the Thompson-sampling
+ * blocks are not counted), each on the stream it runs on, one interval per launch or group of launches, units =
+ * intervals: 5 = K(X, X) and the tall matrix's initialisation, 6 = the diagonal-block Cholesky of every step, 7 = the
+ * panel solves and the look-ahead's next-column updates (the critical path), 8 = the remaining trailing updates (the
+ * bulk stream; all trailing updates in the single-stream schedule), 9 = the tail (W, alpha, the LML sums), 10 = the
+ * scoring state of the new posterior (the int8 digit planes of W when they are made, the fp64 TMA maps). */
+#define DFB_PROF_BUILD_KXX   5
+#define DFB_PROF_BUILD_CHOL  6
+#define DFB_PROF_BUILD_CHAIN 7
+#define DFB_PROF_BUILD_REST  8
+#define DFB_PROF_BUILD_TAIL  9
+#define DFB_PROF_BUILD_I8    10
 int dfb_profile_enable(dfb_handle* h, int on);
 int dfb_profile_read(dfb_handle* h, int cls, double* ms_total, int64_t* launches, double* units);
 
