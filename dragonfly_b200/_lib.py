@@ -91,6 +91,8 @@ PROTOTYPES = {
                                     C.POINTER(_I64), C.POINTER(_I64)]),
   'dfb_moo_score_argmax': (C.c_int, [_P, C.POINTER(MooDesc), C.POINTER(_P), C.POINTER(_P), _I64, _P,
                                      C.POINTER(_D), C.POINTER(_I64)]),
+  'dfb_moo_score_argmax_ts': (C.c_int, [_P, C.POINTER(MooDesc), C.POINTER(_P), C.POINTER(_P), _I64, _P, C.c_uint64,
+                                        _I64, _P, C.POINTER(_D), C.POINTER(_I64), C.POINTER(_I64)]),
   'dfb_kernel_matrix': (C.c_int, [_P, C.POINTER(KernelDesc), _P, _I64, _I32, _P, _I64, _I32, _P]),
   'dfb_ts_workspace_bytes': (C.c_size_t, [_I64, _I64]),
   'dfb_set_ts_workspace': (C.c_int, [_P, _P, C.c_size_t, _I64]),

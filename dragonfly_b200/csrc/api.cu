@@ -1506,6 +1506,35 @@ int dfb_moo_score_argmax(dfb_handle* h, const dfb_moo_desc* desc, const double* 
   return read_best(h, best_score_host, best_index_host);
 }
 
+int dfb_moo_score_argmax_ts(dfb_handle* h, const dfb_moo_desc* desc, const double* const* mu_dev,
+                            const double* const* sd_dev, int64_t m, const double* z_dev, uint64_t seed,
+                            int64_t row0, double* scores_dev, double* best_score_host,
+                            int64_t* best_index_host, int64_t* n_nonpos_host) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if (desc == nullptr || mu_dev == nullptr || sd_dev == nullptr || m < 1 || row0 < 0) {
+    set_error("bad moo_ts arguments (m = %lld, row0 = %lld)", (long long)m, (long long)row0);
+    return -1;
+  }
+  if (desc->kind != DFB_MOO_LIN_VAL && desc->kind != DFB_MOO_TCH_VAL) { set_error("scalarisation kind %d is not a VAL kind", desc->kind); return -1; }
+  if (desc->n_obj < 1 || desc->n_obj > DFB_MOO_MAX_OBJ) { set_error("n_obj = %d outside [1, %d]", desc->n_obj, DFB_MOO_MAX_OBJ); return -1; }
+  for (int k = 0; k < desc->n_obj; k++)
+    if (mu_dev[k] == nullptr || sd_dev[k] == nullptr) { set_error("objective %d: NULL vector", k); return -1; }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  DFB_TRY(launch_reset_best(h));
+  DFB_CUDA_OK(cudaMemsetAsync(h->ts_nonpos, 0, sizeof(int), h->stream));
+  TsZ tz;
+  memset(&tz, 0, sizeof(tz));
+  tz.z = z_dev; tz.seed = seed; tz.row0 = row0; tz.nonpos = h->ts_nonpos;
+  DFB_TRY(launch_moo(h, *desc, mu_dev, sd_dev, m, scores_dev, &tz));
+  if (n_nonpos_host != nullptr) {
+    int nonpos = 0;
+    DFB_CUDA_OK(cudaMemcpyAsync(&nonpos, h->ts_nonpos, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+    *n_nonpos_host = nonpos;
+  }
+  return read_best(h, best_score_host, best_index_host);
+}
+
 int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* X1_dev, int64_t n1,
                       int32_t d1, const double* X2_dev, int64_t n2, int32_t d2, double* K_dev) {
   DFB_TRY(need(h, true, false, false, false, false));

@@ -60,9 +60,11 @@ struct I8ErrModel {
 };
 constexpr int SHORTLIST_CAP = 4096;
 // The normals of DFB_ACQ_TS_MARGINAL for one chunk (dfb_score_argmax_ts).  z: this chunk's normals on the device, or
-// NULL for the counter-based ones, rng_normal(seed, row0 + the candidate's global index).  z_out (may be NULL): the
+// NULL for the counter-based ones, rng_normal(seed, row0 + the candidate's global index, 0).  z_out (may be NULL): the
 // z of every candidate is written there (the shortlist's source).  nonpos (may be NULL): counts the candidates whose
 // sigma^2 is not > 0.  In I8ErrModel, kind DFB_ACQ_TS_MARGINAL takes sens = |z_i| per candidate.
+// launch_moo (dfb_moo_score_argmax_ts) takes the same struct for all m candidates: z is m x n_obj row-major (or NULL for
+// rng_normal(seed, row0 + i, k)), z_out is not used.
 struct TsZ {
   const double* z;
   uint64_t seed;
@@ -100,8 +102,9 @@ int launch_ts_argmax(dfb_handle* h, const double* samples, int64_t ld, int S, in
                      double* best, int64_t* index);
 int launch_small_sumsq(dfb_handle* h, const double* W, int64_t ldw, const double* Ks, int64_t ldk, int64_t n_rows,
                        int m, double* part, int64_t ld_part, int* n_warps_out);
+// ts non-NULL: the VAL kinds over marginal posterior draws, a = mu_k and b = sd_k (TsZ above)
 int launch_moo(dfb_handle* h, const dfb_moo_desc& d, const double* const* a, const double* const* b, int64_t m,
-               double* scores);
+               double* scores, const TsZ* ts = nullptr);
 int launch_add_row_vector(dfb_handle* h, double* M, int64_t ld, int64_t rows, int64_t cols,
                           const double* v);
 int launch_diag_max(dfb_handle* h, const double* M, int64_t ld, int64_t n, double* out);

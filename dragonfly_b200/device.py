@@ -303,6 +303,36 @@ class DevicePosterior(object):
     """ dfb_moo_score_argmax: scalarise n_obj objectives' device vectors and take the arg-max.
         a_list / b_list: CUDA fp64 tensors (mu_k or sampled values; sd_k or None).
         Returns (best_score, best_index, scores tensor or None). """
+    d, m, a_ptrs, b_ptrs, keep = self._moo_operands(kind, a_list, b_list, weights, refs, beta)
+    sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
+    bs, bi = C.c_double(0.0), C.c_int64(-1)
+    _lib.check(self.lib.dfb_moo_score_argmax(
+        self.h, C.byref(d), a_ptrs, b_ptrs, m, C.c_void_p(sc.data_ptr()) if want_scores else None,
+        C.byref(bs), C.byref(bi)), 'dfb_moo_score_argmax')
+    del keep                      # the call has synchronised: the vectors may go
+    return bs.value, bi.value, sc
+
+  def moo_score_argmax_ts(self, kind, mu_list, sd_list, weights, refs=None, z=None, seed=0, row0=0, want_scores=False):
+    """ dfb_moo_score_argmax_ts: one marginal posterior draw per candidate and objective, fl(fl(sd_k z_k) + mu_k),
+        scalarised by kind (DFB_MOO_LIN_VAL / DFB_MOO_TCH_VAL), and its arg-max.  mu_list / sd_list: the objectives'
+        dfb_eval vectors (CUDA fp64 tensors); z: the (m, n_obj) normals (host or device), or None for the device's
+        counter-based normals of (seed, row0 + row, objective).  Returns (best_score, best_index, scores tensor or None,
+        the number of candidates with a variance that is not > 0). """
+    d, m, mu_ptrs, sd_ptrs, keep = self._moo_operands(kind, mu_list, sd_list, weights, refs, 0.0)
+    zd = None if z is None else _dev_f64(z, self.device)
+    assert zd is None or tuple(zd.shape) == (m, len(mu_list))
+    sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
+    bs, bi, nonpos = C.c_double(0.0), C.c_int64(-1), C.c_int64(0)
+    ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())
+    _lib.check(self.lib.dfb_moo_score_argmax_ts(
+        self.h, C.byref(d), mu_ptrs, sd_ptrs, m, ptr(zd), C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), int(row0),
+        ptr(sc), C.byref(bs), C.byref(bi), C.byref(nonpos)), 'dfb_moo_score_argmax_ts')
+    del keep
+    return bs.value, bi.value, sc, nonpos.value
+
+  def _moo_operands(self, kind, a_list, b_list, weights, refs, beta):
+    """ The dfb_moo_desc of n_obj = len(a_list) objectives and the C arrays of their device vectors: (desc, m, a pointers,
+        b pointers or None, the device tensors the pointers point into). """
     K = len(a_list)
     d = _lib.MooDesc()
     d.kind, d.n_obj, d.beta = int(kind), K, float(beta)
@@ -316,12 +346,7 @@ class DevicePosterior(object):
     PtrArr = C.c_void_p * K
     a_ptrs = PtrArr(*[t.data_ptr() for t in a_t])
     b_ptrs = PtrArr(*[t.data_ptr() for t in b_t]) if b_t is not None else None
-    sc = torch.empty((m,), dtype=torch.float64, device=self.device) if want_scores else None
-    bs, bi = C.c_double(0.0), C.c_int64(-1)
-    _lib.check(self.lib.dfb_moo_score_argmax(
-        self.h, C.byref(d), a_ptrs, b_ptrs, m, C.c_void_p(sc.data_ptr()) if want_scores else None,
-        C.byref(bs), C.byref(bi)), 'dfb_moo_score_argmax')
-    return bs.value, bi.value, sc
+    return d, m, a_ptrs, b_ptrs, (a_t, b_t)
 
   def fill_rng(self, seed, col0, S, m, what=_lib.DFB_RNG_NORMAL, out=None):
     """ dfb_fill_rng: the S x m matrix of counter-based normals / uniforms for global columns col0 .. col0+m-1. """

@@ -165,12 +165,17 @@ def _cp_device_layout(parts):
   return kinds, bounds, n_levels, luts
 
 
-def _cp_device_rows(sess, seed, r0, m, layout, out=None):
+def _cp_device_rows(post, seed, r0, m, layout, out=None):
   """ Rows r0 .. r0+m-1 of the device-generated CP candidates, category columns mapped from level index to their column
       value (a Hamming code or the level's number) on the device. """
-  import torch
   kinds, bounds, n_levels, luts = layout
-  pts = sess.post.fill_mixed_candidates(seed, r0, m, kinds, bounds, n_levels, out=out)
+  return _encode_levels(post.fill_mixed_candidates(seed, r0, m, kinds, bounds, n_levels, out=out), luts)
+
+
+def _encode_levels(pts, luts):
+  """ Maps, in place, the category columns of a tensor of CP candidate rows from level index to column value: column c
+      through luts[c] (_cp_device_layout), unless that is None or the identity. """
+  import torch
   for c, lut in enumerate(luts):
     if lut is not None and not np.array_equal(lut, np.arange(len(lut), dtype=np.float64)):
       lut_d = torch.as_tensor(lut, device=pts.device)
@@ -193,6 +198,27 @@ def _cp_point_from_device_row(parts, row):
   return pt
 
 
+def _cp_candidate_source(post, slab_rows, parts, M, mode, levels=False):
+  """ The M candidates of the `rand` maximiser on a CP domain as an _IndexedRows, and the seed of the device's candidates
+      (None in 'numpy' mode).  'numpy' draws the reference's points (draw_cp_candidates) in host slabs of
+      slab_rows(STREAM_SLAB_ROWS) rows; 'device' generates them with dfb_fill_mixed_candidates on `post`, keyed by (seed,
+      global row, column), in slabs of slab_rows(2 STREAM_SLAB_ROWS).  levels: category columns hold level indices
+      instead of the parts' column values (_encode_levels maps them). """
+  if mode == 'device':
+    seed = _device_seed()
+    kinds, bounds, n_levels, luts = _cp_device_layout(parts)
+    layout = (kinds, bounds, n_levels, [None] * len(luts) if levels else luts)
+    return _IndexedRows(
+        slab_rows(2 * STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: _cp_device_rows(post, seed, r0, m, layout, out),
+        lambda i: _cp_point_from_device_row(
+            parts, post.fill_mixed_candidates(seed, i, 1, kinds, bounds, n_levels).cpu().numpy()[0])), seed
+  rows, draws = draw_cp_candidates(parts, M)
+  if levels:
+    rows = np.ascontiguousarray(np.concatenate([np.asarray(d, dtype=np.float64) for d in draws], axis=1))
+  return _IndexedRows(slab_rows(STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: rows[r0:r0 + m],
+                      lambda i: point_from_draws(parts, draws, i)), None
+
+
 def _cp_fused_maximise(gp, anc_data, acq):
   """ maximise_acquisition on a CP domain with acq_opt_method 'rand' (_rand_maximise_vectorised_objective_in_cp_domain,
       exd_utils.py:247-274): the reference scores its sampled points one gp.eval at a time; here every candidate is
@@ -206,18 +232,7 @@ def _cp_fused_maximise(gp, anc_data, acq):
   mode = _candidate_rng(anc_data)
   M = int(anc_data.max_evals)
   with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
-    if mode == 'device':
-      seed = _device_seed()
-      layout = _cp_device_layout(parts)
-      kinds, bounds, n_levels, _ = layout
-      source = _IndexedRows(
-          sess.slab_rows(2 * STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: _cp_device_rows(sess, seed, r0, m, layout, out),
-          lambda i: _cp_point_from_device_row(
-              parts, sess.post.fill_mixed_candidates(seed, i, 1, kinds, bounds, n_levels).cpu().numpy()[0]))
-    else:
-      rows, draws = draw_cp_candidates(parts, M)
-      source = _IndexedRows(sess.slab_rows(STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: rows[r0:r0 + m],
-                            lambda i: point_from_draws(parts, draws, i))
+    source, seed = _cp_candidate_source(sess.post, sess.slab_rows, parts, M, mode)
     if acq is not None:
       return source.point(*_slab_argmax(source, lambda pts, r0: sess.score(pts)))
     z = np.random.normal(size=M) if mode == 'numpy' else None
@@ -229,11 +244,16 @@ def _cp_fused_maximise(gp, anc_data, acq):
       nonpos += int(res[3])
       return res
     best = _slab_argmax(source, score_ts)
-    if nonpos > 0:
-      raise ValueError('Could not compute Cholesky decomposition despite adding jitter to the diagonal: the posterior '
-                       'variance of %d candidate(s) is not positive. This is likely because the M is not positive '
-                       'semi-definite or has infinities/nans.' % (nonpos))
+    _check_nonpos(nonpos)
     return source.point(*best)
+
+
+def _check_nonpos(nonpos):
+  """ The reference's stable_cholesky raises for a 1 x 1 covariance that is not > 0 (general_utils.py:183-203). """
+  if nonpos > 0:
+    raise ValueError('Could not compute Cholesky decomposition despite adding jitter to the diagonal: the posterior '
+                     'variance of %d candidate(s) is not positive. This is likely because the M is not positive '
+                     'semi-definite or has infinities/nans.' % (nonpos))
 
 
 def _cp_other_maximiser(acq_fn, anc_data):

@@ -313,6 +313,24 @@ int dfb_moo_score_argmax(dfb_handle* h, const dfb_moo_desc* desc, const double* 
                          const double* const* b_dev, int64_t m, double* scores_dev,
                          double* best_score_host, int64_t* best_index_host);
 
+/* The multi-objective Thompson sampling acquisitions on Cartesian-product domains (mo_lin_asy_ts / mo_tch_asy_ts,
+ * multiobjective_gpb_acquisitions.py:19-68, with the `rand` maximiser of
+ * _rand_maximise_vectorised_objective_in_cp_domain, exd_utils.py:247-274): the reference calls every objective's
+ * gp.draw_samples(1, [x]) once per candidate, so candidate i gets one marginal posterior draw per objective k,
+ *     v_ik = fl(fl(sd_ik * z_ik) + mu_ik)          (no FMA contraction)
+ * which desc->kind (DFB_MOO_LIN_VAL or DFB_MOO_TCH_VAL only) then scalarises as dfb_moo_score_argmax does, followed by
+ * the arg-max in np.argmax order.  mu_dev / sd_dev: HOST arrays of n_obj device pointers (each m doubles, dfb_eval's mu
+ * and sd).  z_dev (device, m x n_obj row-major, may be NULL): the caller's normals, in the order the reference consumes
+ * them -- candidate-major, objective-minor, i.e. np.random.normal(size=(m, n_obj)).  z_dev = NULL: the kernel generates
+ * them, z_ik = element (k, row0 + i) of dfb_fill_rng(seed, ..., DFB_RNG_NORMAL); for n_obj = 1 that is the normal
+ * dfb_score_argmax_ts uses for the same (seed, row).  *n_nonpos_host (may be NULL) receives the number of candidates
+ * with any objective's sd not > 0, NaN included (sigma^2 not > 0: the reference's stable_cholesky raises there).
+ * scores_dev (m) may be NULL.  The handle supplies stream and scratch only, as for dfb_moo_score_argmax.  */
+int dfb_moo_score_argmax_ts(dfb_handle* h, const dfb_moo_desc* desc, const double* const* mu_dev,
+                            const double* const* sd_dev, int64_t m, const double* z_dev, uint64_t seed,
+                            int64_t row0, double* scores_dev, double* best_score_host,
+                            int64_t* best_index_host, int64_t* n_nonpos_host);
+
 /* Thompson sampling at scale (BASELINE config 5: 256 draws x 10^6 candidates).  The reference draws its normals
  * with np.random.normal on the host (general_utils.py:230), which dfb_ts_draws reproduces when the caller supplies
  * them; at 10^6 x 256 that is 2 GB of host RNG and copies per call.  dfb_fill_rng generates them on the device
