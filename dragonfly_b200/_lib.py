@@ -60,6 +60,19 @@ _P = C.c_void_p
 _D = C.c_double
 _I32 = C.c_int32
 _I64 = C.c_int64
+DFB_GA_MAX_COLS, DFB_GA_MAX_PARTS, DFB_GA_MAX_LUT = 32, 16, 256
+DFB_GA_PART_REAL, DFB_GA_PART_INTEGER, DFB_GA_PART_CATEGORICAL, DFB_GA_PART_NUMERIC = 0, 1, 2, 3
+
+
+class GaDesc(C.Structure):
+  _fields_ = [('d', C.c_int32), ('n_parts', C.c_int32), ('kind', C.c_int32 * DFB_GA_MAX_COLS),
+              ('n_levels', C.c_int32 * DFB_GA_MAX_COLS), ('lut_off', C.c_int32 * DFB_GA_MAX_COLS),
+              ('val_off', C.c_int32 * DFB_GA_MAX_COLS), ('part_kind', C.c_int32 * DFB_GA_MAX_PARTS),
+              ('part_c0', C.c_int32 * DFB_GA_MAX_PARTS), ('part_c1', C.c_int32 * DFB_GA_MAX_PARTS),
+              ('lo', C.c_double * DFB_GA_MAX_COLS), ('hi', C.c_double * DFB_GA_MAX_COLS),
+              ('lut', C.c_double * DFB_GA_MAX_LUT)]
+
+
 PROTOTYPES = {
   'dfb_version': (C.c_int, []),
   'dfb_last_error': (C.c_char_p, []),
@@ -93,6 +106,8 @@ PROTOTYPES = {
                                      C.POINTER(_D), C.POINTER(_I64)]),
   'dfb_moo_score_argmax_ts': (C.c_int, [_P, C.POINTER(MooDesc), C.POINTER(_P), C.POINTER(_P), _I64, _P, C.c_uint64,
                                         _I64, _P, C.POINTER(_D), C.POINTER(_I64), C.POINTER(_I64)]),
+  'dfb_ga_maximise': (C.c_int, [_P, C.POINTER(AcqDesc), _D, C.POINTER(GaDesc), C.c_uint64, _I64, _I64, _P, _P, _P,
+                                C.POINTER(_D), C.POINTER(_I64), C.POINTER(_D)]),
   'dfb_kernel_matrix': (C.c_int, [_P, C.POINTER(KernelDesc), _P, _I64, _I32, _P, _I64, _I32, _P]),
   'dfb_ts_workspace_bytes': (C.c_size_t, [_I64, _I64]),
   'dfb_set_ts_workspace': (C.c_int, [_P, _P, C.c_size_t, _I64]),

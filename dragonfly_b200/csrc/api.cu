@@ -1535,6 +1535,68 @@ int dfb_moo_score_argmax_ts(dfb_handle* h, const dfb_moo_desc* desc, const doubl
   return read_best(h, best_score_host, best_index_host);
 }
 
+int dfb_ga_maximise(dfb_handle* h, const dfb_acq_desc* acq, double mean_const, const dfb_ga_desc* desc, uint64_t seed,
+                    int64_t n_init, int64_t n_total, double* rows_dev, double* vals_dev, double* coded_dev,
+                    double* best_value_host, int64_t* best_index_host, double* best_row_host) {
+  DFB_TRY(need(h, true, true, true, true, true));
+  if (acq == nullptr || desc == nullptr || rows_dev == nullptr || vals_dev == nullptr || coded_dev == nullptr) {
+    set_error("ga_maximise: NULL argument"); return -1;
+  }
+  if (acq->kind < DFB_ACQ_UCB || acq->kind > DFB_ACQ_TTEI) { set_error("ga_maximise: acquisition kind %d", acq->kind); return -1; }
+  const dfb_ga_desc& g = *desc;
+  if (g.d < 1 || g.d > DFB_GA_MAX_COLS || g.n_parts < 1 || g.n_parts > DFB_GA_MAX_PARTS || n_init < 1 ||
+      n_total < n_init) {
+    set_error("bad ga_maximise arguments (d = %d, parts = %d, n_init = %lld, n_total = %lld)", g.d, g.n_parts,
+              (long long)n_init, (long long)n_total);
+    return -1;
+  }
+  int next = 0;
+  for (int p = 0; p < g.n_parts; p++) {
+    const int c0 = g.part_c0[p], c1 = g.part_c1[p], kind = g.part_kind[p];
+    if (c0 != next || c1 <= c0 || c1 > g.d || kind < DFB_GA_PART_REAL || kind > DFB_GA_PART_NUMERIC) {
+      set_error("ga_maximise: bad part %d", p); return -1;
+    }
+    next = c1;
+    for (int c = c0; c < c1; c++) {
+      const bool cat = kind >= DFB_GA_PART_CATEGORICAL;
+      if (g.kind[c] != (cat ? DFB_CAND_CATEGORICAL : (kind == DFB_GA_PART_REAL ? DFB_CAND_REAL : DFB_CAND_INTEGER)) ||
+          (!cat && !(g.lo[c] <= g.hi[c])) ||
+          (cat && (g.n_levels[c] < (kind == DFB_GA_PART_CATEGORICAL ? 2 : 1) || g.lut_off[c] < 0 ||
+                   g.lut_off[c] + g.n_levels[c] > DFB_GA_MAX_LUT)) ||
+          (kind == DFB_GA_PART_NUMERIC && (g.val_off[c] < 0 || g.val_off[c] + g.n_levels[c] > DFB_GA_MAX_LUT))) {
+        set_error("ga_maximise: bad column %d of part %d", c, p); return -1;
+      }
+    }
+  }
+  if (next != g.d) { set_error("ga_maximise: the parts cover %d of %d columns", next, g.d); return -1; }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  int64_t n_levels[DFB_GA_MAX_COLS];
+  for (int c = 0; c < g.d; c++) n_levels[c] = g.kind[c] == DFB_CAND_CATEGORICAL ? g.n_levels[c] : 0;
+  ChunkMode md;
+  md.want_std = true;
+  md.allow_small = h->small_eval != 0;
+  // the initial pool
+  DFB_TRY(launch_fill_mixed_candidates(h, seed, 0, n_init, g.d, g.kind, g.lo, g.hi, n_levels, rows_dev));
+  DFB_TRY(launch_ga_encode(h, g, rows_dev, n_init, coded_dev));
+  ChunkOut out = {nullptr, nullptr, vals_dev};
+  DFB_TRY(run_chunks(h, *acq, coded_dev, n_init, g.d, DFB_DEVICE, mean_const, out, md));
+  // epochs: no launch waits on the host
+  for (int64_t r0 = n_init; r0 < n_total; r0 += 5) {
+    const int c = (int)std::min<int64_t>(5, n_total - r0);
+    DFB_TRY(launch_ga_epoch(h, g, seed, r0, c, rows_dev, vals_dev, coded_dev));
+    ChunkOut oe = {nullptr, nullptr, vals_dev + r0};
+    DFB_TRY(run_chunks(h, *acq, coded_dev, c, g.d, DFB_DEVICE, mean_const, oe, md));
+  }
+  DFB_TRY(launch_ga_best(h, g, rows_dev, vals_dev, n_total, coded_dev));
+  double res[2 + DFB_GA_MAX_COLS];
+  DFB_CUDA_OK(cudaMemcpyAsync(res, coded_dev, sizeof(double) * (2 + g.d), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  if (best_value_host) *best_value_host = res[0];
+  if (best_index_host) *best_index_host = (int64_t)res[1];
+  if (best_row_host) for (int c = 0; c < g.d; c++) best_row_host[c] = res[2 + c];
+  return 0;
+}
+
 int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* X1_dev, int64_t n1,
                       int32_t d1, const double* X2_dev, int64_t n2, int32_t d2, double* K_dev) {
   DFB_TRY(need(h, true, false, false, false, false));

@@ -98,6 +98,12 @@ int launch_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m
                            const double* hi, double* out);
 int launch_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int d, const int32_t* kinds,
                                  const double* lo, const double* hi, const int64_t* n_levels, double* out);
+// the GA maximiser of Cartesian-product domains (dfb_ga_maximise)
+int launch_ga_encode(dfb_handle* h, const dfb_ga_desc& g, const double* rows, int64_t m, double* coded);
+int launch_ga_epoch(dfb_handle* h, const dfb_ga_desc& g, uint64_t seed, int64_t r0, int c, double* rows,
+                    const double* vals, double* coded);
+int launch_ga_best(dfb_handle* h, const dfb_ga_desc& g, const double* rows, const double* vals, int64_t n,
+                   double* out);
 int launch_ts_argmax(dfb_handle* h, const double* samples, int64_t ld, int S, int64_t m, int64_t idx_base, int reset,
                      double* best, int64_t* index);
 int launch_small_sumsq(dfb_handle* h, const double* W, int64_t ldw, const double* Ks, int64_t ldk, int64_t n_rows,

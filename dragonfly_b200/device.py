@@ -388,6 +388,20 @@ class DevicePosterior(object):
         C.c_void_p(out.data_ptr())), 'dfb_fill_mixed_candidates')
     return out
 
+  def ga_maximise(self, acq_desc, mean_const, ga_desc, seed, n_init, n_total):
+    """ dfb_ga_maximise: the whole GA search on the device.  Returns (best value, best index, best level row, the
+        n_total x d level rows, the n_total values), the last two CUDA tensors. """
+    d = int(ga_desc.d)
+    rows = torch.empty((int(n_total), d), dtype=torch.float64, device=self.device)
+    vals = torch.empty((int(n_total),), dtype=torch.float64, device=self.device)
+    coded = torch.empty((max(int(n_init), 5), d), dtype=torch.float64, device=self.device)
+    bv, bi, row = C.c_double(0.0), C.c_int64(-1), (C.c_double * d)()
+    _lib.check(self.lib.dfb_ga_maximise(
+        self.h, C.byref(acq_desc), float(mean_const), C.byref(ga_desc), C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF),
+        int(n_init), int(n_total), C.c_void_p(rows.data_ptr()), C.c_void_p(vals.data_ptr()),
+        C.c_void_p(coded.data_ptr()), C.byref(bv), C.byref(bi), row), 'dfb_ga_maximise')
+    return bv.value, bi.value, np.array(row[:], dtype=np.float64), rows, vals
+
   def ts_argmax(self, samples, idx_base, best, index, reset):
     """ dfb_ts_argmax: fold one block of draws (S x m CUDA tensor) into the running per-draw arg-max. """
     S, m = int(samples.shape[0]), int(samples.shape[1])

@@ -61,14 +61,15 @@ class _CPPart(object):
   __slots__ = ('type', 'dim', 'bounds', 'levels', 'codes')
 
 
-def _cp_parts(domain, kernel):
+def _cp_parts(domain, kernel=None):
   """ The parts of a CP domain in domain order; raises for what the device does not serve (constraints, NN and
-      discrete-Euclidean parts, nested CP domains). """
+      discrete-Euclidean parts, nested CP domains).  kernel None: the parts without Hamming tables (and without checking
+      the GP's kernel against the domain). """
   from .kernel import category_codes, _kind_of
   has_constraints = getattr(domain, 'has_constraints', None)
   if has_constraints is not None and has_constraints():
     raise NotImplementedError('Constrained Cartesian-product domains are outside the GPU hot-path scope.')
-  kernel_list = getattr(kernel, 'kernel_list', None)
+  kernel_list = getattr(kernel, 'kernel_list', None) if kernel is not None else [None] * len(domain.list_of_domains)
   if kernel_list is None or len(kernel_list) != len(domain.list_of_domains):
     raise NotImplementedError('A Cartesian-product domain needs a CPGP whose kernel has one factor per part.')
   parts = []
@@ -82,7 +83,9 @@ def _cp_parts(domain, kernel):
     elif p.type in _CP_DISCRETE:
       p.levels = [list(loi) for loi in dom.list_of_list_of_items]
       p.dim = len(p.levels)
-      if _kind_of(kern) == 'HammingKernel':
+      if kern is None:
+        pass
+      elif _kind_of(kern) == 'HammingKernel':
         p.codes = category_codes(kern)
       elif p.type != 'prod_discrete_numeric':
         raise NotImplementedError('A prod_discrete part needs a HammingKernel factor.')
@@ -256,11 +259,12 @@ def _check_nonpos(nonpos):
                      'semi-definite or has infinities/nans.' % (nonpos))
 
 
-def _cp_other_maximiser(acq_fn, anc_data):
+def _cp_other_maximiser(acq_fn, anc_data, gp=None, acq=None):
   """ The non-'rand' maximisers on a CP domain.  'direct' / 'pdoo' on a domain of Euclidean parts only: PDOO over the
       flattened bounds, the point regrouped into parts (maximise_with_method_on_product_euclidean_spaces,
-      exd_utils.py:219-244).  'ga' is the reference's own (a Dragonfly install is needed) with a one-point device
-      objective.  acq_fn takes a list of list-of-parts points. """
+      exd_utils.py:219-244).  'ga' and 'ga-<method>' run the reference's GA restated in ga.py, each batch it allows
+      scored in one call: with the device descriptor acq in one fused session on gp (evaluations in progress appended
+      once), else with acq_fn.  acq_fn takes a list of list-of-parts points. """
   method = str(anc_data.acq_opt_method).lower()
   if method.startswith(('direct', 'pdoo')):
     doms = anc_data.domain.list_of_domains
@@ -274,14 +278,17 @@ def _cp_other_maximiser(acq_fn, anc_data):
     flat_fn = lambda X: acq_fn([regroup(x) for x in np.asarray(X, dtype=np.float64)])
     return regroup(_delegate_to_reference_maximiser(flat_fn, flat))
   if method.startswith('ga'):
-    try:
-      from dragonfly.exd.exd_utils import maximise_with_method  # pylint: disable=import-error
-    except ImportError:
-      raise NotImplementedError("acq_opt_method '%s' on a Cartesian-product domain is the reference's GA and needs a "
-                                "Dragonfly install; 'rand' runs on the device." % (anc_data.acq_opt_method))
-    _, opt_pt = maximise_with_method(anc_data.acq_opt_method, lambda x: acq_fn([x]), anc_data.domain,
-                                     anc_data.max_evals)
-    return opt_pt
+    from . import ga
+    parts = _cp_parts(anc_data.domain, None if gp is None else gp.kernel)
+    if _shard_info()[1] > 1:
+      raise NotImplementedError('The GA maximiser of Cartesian-product domains is not sharded across ranks.')
+    if gp is None or acq is None:
+      return ga.maximise(acq_fn, parts, method, anc_data.max_evals)
+    seed = _device_seed() if _candidate_rng(anc_data) == 'device' else None
+    with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
+      search = None if seed is None else (lambda: ga.device_search(sess, parts, anc_data.max_evals, seed))
+      return ga.maximise(lambda pts: sess.score(pts, want_scores=True)[2], parts, method, anc_data.max_evals,
+                         search=search)
   raise NotImplementedError("acq_opt_method '%s' is not served on Cartesian-product domains; use 'rand'."
                             % (anc_data.acq_opt_method))
 
@@ -653,7 +660,7 @@ def _maximise_acq(gp, anc_data, acq, acq_fn):
   if _is_cp_domain(anc_data):
     if anc_data.acq_opt_method in ['rand']:
       return _cp_fused_maximise(gp, anc_data, acq)
-    return _cp_other_maximiser(acq_fn, anc_data)
+    return _cp_other_maximiser(acq_fn, anc_data, gp, acq)
   if _check_rand_euclidean(anc_data):
     return _fused_maximise(None, anc_data, session=lambda: gp._fused_session(acq, _halluc_points(anc_data)))
   return _delegate_to_reference_maximiser(acq_fn, anc_data)

@@ -365,6 +365,47 @@ int dfb_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, i
 int dfb_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int32_t d, const int32_t* kinds_host,
                               const double* lo_host, const double* hi_host, const int64_t* n_levels_host, double* out_dev);
 
+/* The GA acquisition maximiser of a Cartesian-product domain, resident on the device (the reference's CPGAOptimiser,
+ * cp_ga_optimiser.py / ga_optimiser.py, driven by Philox instead of MT19937).  Rows are in the level form of
+ * dfb_fill_mixed_candidates (categorical columns hold level indices); lut maps them to the column values the kernel
+ * descriptor scores (Hamming codes, or the levels of a prod_discrete_numeric part).  Parts:
+ *   DFB_GA_PART_REAL / _INTEGER  every column c: x + (hi - lo) / 10 * z, clipped to [lo, hi] (integer: then rounded half to
+ *                                even), z = element (c, row) of dfb_fill_rng(seed, ..., DFB_RNG_NORMAL)
+ *   DFB_GA_PART_CATEGORICAL      one coordinate q = c0 + floor(u1 (c1 - c0)) changes to a uniformly chosen OTHER level
+ *                                floor(u2 (L_q - 1)) (skipping the current one); u1, u2 = DFB_RNG_UNIFORM elements
+ *                                (1 + c0, row) and (1 + d + c0, row).  Every coordinate needs L_q >= 2.
+ *   DFB_GA_PART_NUMERIC          every coordinate c: np.random.choice(levels, p = 0.8 w / sum(w) + 0.2 / L) with
+ *                                w_l = exp(-|level_l - x|), levels at lut[val_off[c] ..], u = element (1 + c, row)
+ * Parents of the 5 rows of an epoch starting at row r0: row r0 + j takes the inverse CDF of
+ * exp((v_i - mean) / (2 (std + 1e-4))) over every value so far at u = element (0, r0 + j), uniform when a term or the sum
+ * is not finite.  */
+#define DFB_GA_MAX_COLS  32
+#define DFB_GA_MAX_PARTS 16
+#define DFB_GA_MAX_LUT   256
+#define DFB_GA_PART_REAL        0
+#define DFB_GA_PART_INTEGER     1
+#define DFB_GA_PART_CATEGORICAL 2
+#define DFB_GA_PART_NUMERIC     3
+typedef struct {
+  int32_t d, n_parts;
+  int32_t kind[DFB_GA_MAX_COLS];        /* DFB_CAND_* */
+  int32_t n_levels[DFB_GA_MAX_COLS];    /* categorical columns */
+  int32_t lut_off[DFB_GA_MAX_COLS];     /* categorical columns: column value of level l = lut[lut_off + l] */
+  int32_t val_off[DFB_GA_MAX_COLS];     /* DFB_GA_PART_NUMERIC columns: level l's number = lut[val_off + l] */
+  int32_t part_kind[DFB_GA_MAX_PARTS];  /* DFB_GA_PART_* */
+  int32_t part_c0[DFB_GA_MAX_PARTS], part_c1[DFB_GA_MAX_PARTS];   /* columns [c0, c1) */
+  double  lo[DFB_GA_MAX_COLS], hi[DFB_GA_MAX_COLS];
+  double  lut[DFB_GA_MAX_LUT];
+} dfb_ga_desc;
+/* The whole search on the handle's stream, one synchronisation at the end: rows 0 .. n_init-1 from
+ * dfb_fill_mixed_candidates(seed, 0, n_init), then epochs of 5 mutated rows (ga_epoch_kernel) until n_total rows, every
+ * row scored with acq (UCB / EI / PI / TTEI, fp64) into vals_dev[row].  Returns the first largest value (NaN never wins),
+ * its row index and its level row.  rows_dev: n_total x d, vals_dev: n_total, coded_dev: max(n_init, 5) x d, all device
+ * memory owned by the caller.  */
+int dfb_ga_maximise(dfb_handle* h, const dfb_acq_desc* acq, double mean_const, const dfb_ga_desc* desc, uint64_t seed,
+                    int64_t n_init, int64_t n_total, double* rows_dev, double* vals_dev, double* coded_dev,
+                    double* best_value_host, int64_t* best_index_host, double* best_row_host);
+
 /* Kernel.__call__(X1, X2) (kernel.py:72-83): the n1 x n2 Gram matrix, device pointers. */
 int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* X1_dev, int64_t n1,
                       int32_t d1, const double* X2_dev, int64_t n2, int32_t d2, double* K_dev);
