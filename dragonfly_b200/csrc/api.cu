@@ -1817,6 +1817,14 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
   else if (strcmp(name, "Ki8") == 0) { src = h->Ki8; size = 3 * 2 * chunk * npad; }
   else if (strcmp(name, "Ks") == 0) { src = h->Ks; size = (int64_t)sizeof(double) * chunk * npad; }
   else if (strcmp(name, "partial") == 0) { src = h->partial; size = (int64_t)sizeof(double) * (npad / TILE) * chunk; }
+  else if (strcmp(name, "kssv") == 0) { src = h->kssv; size = (int64_t)sizeof(double) * chunk; }
+  else if (strncmp(name, "ts_", 3) == 0) {
+    if (h->ts_ws == nullptr) { set_error("debug_copy '%s': no Thompson-sampling workspace is set", name); return -1; }
+    const int64_t mbp = h->ts_mb;
+    if (strcmp(name, "ts_Cov") == 0) { src = h->ts_Cov; size = (int64_t)sizeof(double) * mbp * mbp; }
+    else if (strcmp(name, "ts_T") == 0) { src = h->ts_T; size = (int64_t)sizeof(double) * (2 * mbp + TILE) * mbp; }
+    else { set_error("unknown debug_copy buffer '%s'", name); return -1; }
+  }
   else { set_error("unknown debug_copy buffer '%s'", name); return -1; }
   if (bytes != size) {
     set_error("debug_copy '%s': %lld bytes requested, the buffer has %lld", name, (long long)bytes, (long long)size);

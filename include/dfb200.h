@@ -437,7 +437,12 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
  * doubles), "Ki8" (the three K_* digit planes of the chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
  * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk),
  * "T" (the factorised tall matrix [L ; L^-T ; (L^-1 y_c)^T], (2 npad + 128) x npad: its padding, the y row), "alpha"
- * (npad doubles, padding included).
+ * (npad doubles, padding included), "kssv" (k(x*, x*) of the last scored chunk, chunk doubles).  With a Thompson-
+ * sampling workspace (dfb_set_ts_workspace; mbp = its mb rounded up to 128, and q = the last block's m rounded up to
+ * 128, whose data sits at the start of each buffer with leading dimension q): "ts_Cov" (mbp^2 doubles: the padded
+ * posterior covariance of the last dfb_eval_covar / dfb_ts_draws block, q x q; dfb_ts_draws writes its lower tiles
+ * only) and "ts_T" ((2 mbp + 128) mbp doubles: the tall matrix dfb_ts_draws factorised, (2 q + 128) x q, whose top is
+ * the factor of Cov + jitter I); without a TS workspace these two names are an error.
  * Synchronises. */
 int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
 /* Diagnostics (tests/test_gpu_prune_f32.py): the largest relative error of ex2.approx.ftz.f32 (which = 0) over every
