@@ -111,6 +111,8 @@ PROTOTYPES = {
   'dfb_kernel_matrix': (C.c_int, [_P, C.POINTER(KernelDesc), _P, _I64, _I32, _P, _I64, _I32, _P]),
   'dfb_ts_workspace_bytes': (C.c_size_t, [_I64, _I64]),
   'dfb_set_ts_workspace': (C.c_int, [_P, _P, C.c_size_t, _I64]),
+  'dfb_joint_workspace_bytes': (C.c_size_t, [_I64, _I64]),
+  'dfb_set_joint_workspace': (C.c_int, [_P, _P, C.c_size_t, _I64]),
   'dfb_ts_draws': (C.c_int, [_P, _P, _I64, _I32, _D, _P, _I32, _D, _P, _P, C.POINTER(_D)]),
   'dfb_fill_rng': (C.c_int, [_P, C.c_uint64, _I64, _I32, _I64, _I32, _P]),
   'dfb_ts_argmax': (C.c_int, [_P, _P, _I64, _I32, _I64, _I64, _I32, _P, _P]),

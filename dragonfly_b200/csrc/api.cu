@@ -142,6 +142,28 @@ static size_t carve_ts(dfb_handle* h, char* base, int64_t n_max, int64_t mb) {
   return c.off + 256;
 }
 
+// The joint form over up to m candidates: the covariance is factorised in place, so there is one Mpad x Mpad matrix
+// and no tall buffer.
+static size_t carve_joint(dfb_handle* h, char* base, int64_t n_max, int64_t m) {
+  const int64_t npad = round_up(n_max < 1 ? 1 : n_max, TILE);
+  const int64_t mp = round_up(m < 1 ? 1 : m, TILE);
+  Carver c(base);
+  double* Vt = c.take<double>((size_t)mp * npad);
+  double* cxs = c.take<double>((size_t)mp * DFB_MAX_SLOTS);
+  double* cnrm = c.take<double>((size_t)mp * DFB_MAX_FACTORS);
+  double* Cov = c.take<double>((size_t)mp * mp);
+  double* Ut = c.take<double>((size_t)256 * mp);
+  double* Sm = c.take<double>((size_t)256 * mp);
+  double* mu = c.take<double>((size_t)mp);
+  double* red = c.take<double>(8);
+  int* info = c.take<int>(4);
+  if (h != nullptr && base != nullptr) {
+    h->js_Vt = Vt; h->js_cxs = cxs; h->js_cnrm = cnrm; h->js_Cov = Cov; h->js_Ut = Ut; h->js_Sm = Sm; h->js_mu = mu;
+    h->js_red = red; h->js_info = info; h->js_mb = mp;
+  }
+  return c.off + 256;
+}
+
 static int check_desc(const dfb_kernel_desc* d) {
   if (d == nullptr) { set_error("kernel descriptor is NULL"); return -1; }
   if (d->n_terms < 1 || d->n_terms > DFB_MAX_TERMS || d->n_factors < 1 ||
@@ -346,15 +368,17 @@ static int factor_update(dfb_handle* h, const FactorMaps& m, const FactorArgs& g
   return prof_end(h, cls, 1.0);
 }
 
-// profile: time the stages in the DFB_PROF_BUILD_* classes (the posterior build; not the Thompson blocks)
+// profile: time the stages in the DFB_PROF_BUILD_* classes (the posterior build; not the Thompson blocks).
+// top_only: T is the npad x npad square alone, factorised in place (no L^-T rows, no y row; with_bottom is ignored).
+// The top's tiles see the same launches and arithmetic in both forms, so its L is bit for bit the tall form's.
 static int factorise_tall(dfb_handle* h, double* T, int64_t npad, double* Dinv, int* info,
-                          bool with_bottom, bool profile) {
+                          bool with_bottom, bool profile, bool top_only = false) {
   const int nb = (int)(npad / TILE);
   const int c_chol = profile ? DFB_PROF_BUILD_CHOL : -1, c_chain = profile ? DFB_PROF_BUILD_CHAIN : -1;
   const int c_rest = profile ? DFB_PROF_BUILD_REST : -1;
   const bool la = h->lookahead != 0 && nb >= 4;
   FactorMaps maps;
-  DFB_TRY(make_factor_maps(&maps, T, npad, Dinv));
+  DFB_TRY(make_factor_maps(&maps, T, top_only ? npad : 2 * npad + TILE, npad, Dinv));
   StreamSwap guard(h);
   if (la) {
     DFB_TRY(ensure_factor_streams(h));
@@ -371,6 +395,7 @@ static int factorise_tall(dfb_handle* h, double* T, int64_t npad, double* Dinv, 
     FactorArgs g;
     memset(&g, 0, sizeof(g));
     g.T = T; g.ld = npad; g.step = step; g.nb = nb; g.skip_bottom = with_bottom ? 0 : 1; g.info = info;
+    g.top_only = top_only ? 1 : 0;
     g.panel = 1;
     DFB_TRY(factor_update(h, maps, g, true, c_chain));
     if (step + 1 >= nb) continue;
@@ -584,7 +609,7 @@ static int replay_last_block(dfb_handle* h, int32_t flags, double* lml_out_host)
   // replay of factorisation step nb-1
   DFB_TRY(launch_chol_diag(h, h->T, npad, step, h->Dinv, h->info));
   FactorMaps maps;
-  DFB_TRY(make_factor_maps(&maps, h->T, npad, h->Dinv));
+  DFB_TRY(make_factor_maps(&maps, h->T, 2 * npad + TILE, npad, h->Dinv));
   FactorArgs fa;
   memset(&fa, 0, sizeof(fa));
   fa.T = h->T; fa.ld = npad; fa.step = step; fa.nb = nb; fa.panel = 1; fa.info = h->info;
@@ -1620,40 +1645,80 @@ int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* 
   return 0;
 }
 
-// mu and the padded posterior covariance (h->ts_Cov, ld = mbp) of one block of m candidates:
+// The buffers one posterior covariance is formed in: the block workspace's (ts_*, m <= its mb and the chunk) or the
+// joint workspace's (js_*, every candidate at once).
+struct CovBufs {
+  double* Vt; double* cxs; double* cnrm; double* Cov; double* mu;
+  bool joint;
+};
+
+// Block form when the TS workspace holds the m candidates within one scoring chunk, else the joint form when the joint
+// workspace holds them, else an error.  A caller that sets both picks the form by which workspace can hold m.
+static int cov_bufs(dfb_handle* h, int64_t m, CovBufs* b) {
+  const int64_t mbp = round_up(m, TILE);
+  if (m < 1) { set_error("posterior covariance of %lld candidates", (long long)m); return -1; }
+  if (h->ts_ws != nullptr && mbp <= h->ts_mb && mbp <= h->chunk) {
+    *b = CovBufs{h->ts_Vt, h->ts_cxs, h->ts_cnrm, h->ts_Cov, h->ts_mu, false};
+    return 0;
+  }
+  if (h->js_ws != nullptr && mbp <= h->js_mb) {
+    *b = CovBufs{h->js_Vt, h->js_cxs, h->js_cnrm, h->js_Cov, h->js_mu, true};
+    return 0;
+  }
+  if (h->ts_ws == nullptr && h->js_ws == nullptr) {
+    set_error("no Thompson-sampling workspace: call dfb_set_ts_workspace or dfb_set_joint_workspace first");
+    return -1;
+  }
+  set_error("%lld candidates exceed the TS workspace (%lld) / chunk (%lld) and the joint workspace (%lld)",
+            (long long)m, (long long)h->ts_mb, (long long)h->chunk, (long long)h->js_mb);
+  return -1;
+}
+
+// mu and the padded posterior covariance (b.Cov, ld = mbp) of m candidates:
 // K_* -> V^T = K_* W^T -> Cov = K** - V^T V    (gp_core.py:173-181)
-static int posterior_covariance(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc,
+// K_* and K** are formed in row slabs of at most one scoring chunk (the K_* buffer and the candidate staging hold one
+// chunk); a block (mbp <= chunk) is one slab.  Every tile of Cov is one DMMA contraction of depth npad over the same
+// V^T rows whatever the slab and the grid, so the leading q x q of a joint covariance is bit for bit the covariance of
+// its first q candidates.
+static int posterior_covariance(dfb_handle* h, const CovBufs& b, const double* Xc_dev, int64_t m, int32_t dc,
                                 double mean_const, int64_t* mbp_out, bool lower_only) {
   const ActiveKernel k = active_kernel(h);
-  if (h->ts_ws == nullptr) { set_error("no Thompson-sampling workspace: call dfb_set_ts_workspace first"); return -1; }
   if (dc != k.desc.cand_dim) { set_error("candidates have %d columns, the kernel descriptor expects %d", dc, k.desc.cand_dim); return -1; }
   const int64_t mbp = round_up(m, TILE);
-  if (m < 1 || mbp > h->ts_mb || mbp > h->chunk) { set_error("block of %lld candidates exceeds the TS workspace (%lld) / chunk (%lld)", (long long)m, (long long)h->ts_mb, (long long)h->chunk); return -1; }
   DFB_TRY(ensure_train_scaled(h));
   DFB_TRY(ensure_test_scaled(h));
   const int64_t npad = h->npad;
   const int nb = (int)(npad / TILE), mbb = (int)(mbp / TILE);
-  // K_* rows (zero rows beyond m) and mu
   KstarArgs ka{};
-  ka.desc = &k.desc; ka.d_desc = k.d_desc; ka.xsT = k.ss.xs; ka.nrmT = k.ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
-  ka.Xc = Xc_dev; ka.m = m; ka.dc = dc; ka.m_rows = mbp; ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
-  ka.mean_const = mean_const; ka.mu = h->ts_mu; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
-  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
-  // V^T[a][i] = sum_{k <= i} K_*[a][k] W[i][k]
   GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = h->Ks; g.lda = npad; g.B = h->W; g.ldb = npad; g.D = h->ts_Vt; g.ldd = npad; g.alpha = 1.0;
-  g.mode = MODE_GENERIC; g.n_rb = mbb; g.n_cb = nb; g.K = (int)npad; g.tri = 2;
-  DFB_TRY(launch_gemm(h, g, EPI_STORE, mbb * nb));
+  for (int64_t r0 = 0; r0 < mbp; r0 += h->chunk) {
+    const int64_t rows = std::min(h->chunk, mbp - r0);
+    // K_* rows (zero rows beyond m) and mu
+    ka = KstarArgs{};
+    ka.desc = &k.desc; ka.d_desc = k.d_desc; ka.xsT = k.ss.xs; ka.nrmT = k.ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
+    ka.Xc = Xc_dev + r0 * dc; ka.m = std::min(m - r0, rows); ka.dc = dc; ka.m_rows = rows; ka.n_valid = h->n;
+    ka.n_write = npad; ka.Ks = h->Ks; ka.ldk = npad;
+    ka.mean_const = mean_const; ka.mu = b.mu + r0; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
+    DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+    // V^T[a][i] = sum_{k <= i} K_*[a][k] W[i][k]
+    memset(&g, 0, sizeof(g));
+    g.A = h->Ks; g.lda = npad; g.B = h->W; g.ldb = npad; g.D = b.Vt + r0 * npad; g.ldd = npad; g.alpha = 1.0;
+    g.mode = MODE_GENERIC; g.n_rb = (int)(rows / TILE); g.n_cb = nb; g.K = (int)npad; g.tri = 2;
+    DFB_TRY(launch_gemm(h, g, EPI_STORE, g.n_rb * nb));
+  }
   // K** = kernel(X_test, X_test) (gp_core.py:179) with the candidates as both sides
-  DFB_TRY(launch_prep_scaled(h, k.d_desc, 0, Xc_dev, m, dc, h->ts_cxs, h->ts_cnrm, mbp));
-  ka.xsT = h->ts_cxs; ka.nrmT = h->ts_cnrm; ka.npad_tr = mbp; ka.alpha = nullptr; ka.n_valid = m; ka.n_write = mbp;
-  ka.Ks = h->ts_Cov; ka.ldk = mbp; ka.mean_const = 0.0; ka.mu = nullptr;
-  DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  DFB_TRY(launch_prep_scaled(h, k.d_desc, 0, Xc_dev, m, dc, b.cxs, b.cnrm, mbp));
+  for (int64_t r0 = 0; r0 < mbp; r0 += h->chunk) {
+    const int64_t rows = std::min(h->chunk, mbp - r0);
+    ka.Xc = Xc_dev + r0 * dc; ka.m = std::min(m - r0, rows); ka.m_rows = rows;
+    ka.xsT = b.cxs; ka.nrmT = b.cnrm; ka.npad_tr = mbp; ka.alpha = nullptr; ka.n_valid = m; ka.n_write = mbp;
+    ka.Ks = b.Cov + r0 * mbp; ka.ldk = mbp; ka.mean_const = 0.0; ka.mu = nullptr;
+    DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+  }
   // Cov = K** - V^T V
   memset(&g, 0, sizeof(g));
-  g.A = h->ts_Vt; g.lda = npad; g.B = h->ts_Vt; g.ldb = npad; g.C = h->ts_Cov; g.ldc = mbp;
-  g.D = h->ts_Cov; g.ldd = mbp; g.alpha = -1.0; g.mode = MODE_GENERIC; g.n_rb = mbb; g.n_cb = mbb;
+  g.A = b.Vt; g.lda = npad; g.B = b.Vt; g.ldb = npad; g.C = b.Cov; g.ldc = mbp;
+  g.D = b.Cov; g.ldd = mbp; g.alpha = -1.0; g.mode = MODE_GENERIC; g.n_rb = mbb; g.n_cb = mbb;
   g.K = (int)npad;
   g.lower_only = lower_only ? 1 : 0;     // the factorisation that follows reads the lower triangle only
   DFB_TRY(launch_gemm(h, g, EPI_STORE, mbb * mbb));
@@ -1674,16 +1739,66 @@ int dfb_set_ts_workspace(dfb_handle* h, void* workspace_dev, size_t bytes, int64
   return 0;
 }
 
+size_t dfb_joint_workspace_bytes(int64_t n_max, int64_t m) { return carve_joint(nullptr, nullptr, n_max, m); }
+
+int dfb_set_joint_workspace(dfb_handle* h, void* workspace_dev, size_t bytes, int64_t m) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if (workspace_dev == nullptr || m < 1) { set_error("bad joint workspace arguments"); return -1; }
+  const size_t want = carve_joint(nullptr, nullptr, h->n_max, m);
+  if (bytes < want) { set_error("joint workspace too small: %zu bytes given, %zu needed", bytes, want); return -1; }
+  if ((reinterpret_cast<uintptr_t>(workspace_dev) & 255) != 0) { set_error("joint workspace must be 256-byte aligned"); return -1; }
+  h->js_ws = static_cast<char*>(workspace_dev);
+  carve_joint(h, h->js_ws, h->n_max, m);
+  return 0;
+}
+
 int dfb_eval_covar(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, double mean_const,
                    double* mu_dev, double* covar_dev) {
   DFB_TRY(need(h, true, true, true, true, true));
   if (Xc_dev == nullptr || mu_dev == nullptr || covar_dev == nullptr) { set_error("bad eval_covar arguments"); return -1; }
+  CovBufs b;
+  DFB_TRY(cov_bufs(h, m, &b));
   DFB_CUDA_OK(cudaSetDevice(h->device));
   int64_t mbp = 0;
-  DFB_TRY(posterior_covariance(h, Xc_dev, m, dc, mean_const, &mbp, false));
-  DFB_TRY(launch_copy_pad(h, h->ts_mu, m, mu_dev, m));
-  DFB_TRY(launch_copy_rows(h, h->ts_Cov, mbp, covar_dev, m, m, m));
+  DFB_TRY(posterior_covariance(h, b, Xc_dev, m, dc, mean_const, &mbp, false));
+  DFB_TRY(launch_copy_pad(h, b.mu, m, mu_dev, m));
+  DFB_TRY(launch_copy_rows(h, b.Cov, mbp, covar_dev, m, m, m));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// The joint draw: Cov + jitter I (identity padding) factorised in place by the factor-only mode, then samples^T = L U
+// in passes of <= 256 draws over the one factor.
+static int joint_draws(dfb_handle* h, const CovBufs& b, const double* Xc_dev, int64_t m, int32_t dc, double mean_const,
+                       const double* Ut_dev, int32_t S, double jitter, double* samples_dev, int64_t* mbp_out) {
+  int64_t mbp = 0;
+  DFB_TRY(prof_begin(h, DFB_PROF_TS_COV));
+  DFB_TRY(posterior_covariance(h, b, Xc_dev, m, dc, mean_const, &mbp, true));
+  DFB_TRY(prof_end(h, DFB_PROF_TS_COV, 1.0));
+  DFB_TRY(launch_diag_max(h, b.Cov, mbp, m, h->js_red));
+  DFB_CUDA_OK(cudaMemsetAsync(h->js_info, 0, sizeof(int) * 4, h->stream));
+  DFB_TRY(launch_set_diag(h, b.Cov, mbp, 0, m, jitter, 1));
+  DFB_TRY(launch_set_diag(h, b.Cov, mbp, m, mbp, 1.0, 0));
+  DFB_TRY(prof_begin(h, DFB_PROF_TS_FACTOR));
+  DFB_TRY(factorise_tall(h, b.Cov, mbp, h->Dinv, h->js_info, false, false, true));
+  DFB_TRY(prof_end(h, DFB_PROF_TS_FACTOR, 1.0));
+  DFB_TRY(prof_begin(h, DFB_PROF_TS_PRODUCT));
+  for (int32_t s0 = 0; s0 < S; s0 += 256) {
+    const int32_t s = std::min(256, S - s0);
+    const int64_t Sp = round_up(s, TILE);
+    DFB_CUDA_OK(cudaMemsetAsync(h->js_Ut, 0, sizeof(double) * (size_t)Sp * mbp, h->stream));
+    DFB_TRY(launch_copy_rows(h, Ut_dev + (int64_t)s0 * m, m, h->js_Ut, mbp, s, m));
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.A = h->js_Ut; g.lda = mbp; g.B = b.Cov; g.ldb = mbp; g.D = h->js_Sm; g.ldd = mbp; g.alpha = 1.0;
+    g.mode = MODE_GENERIC; g.n_rb = (int)(Sp / TILE); g.n_cb = (int)(mbp / TILE); g.K = (int)mbp; g.tri = 2;
+    g.info = h->js_info;
+    DFB_TRY(launch_gemm(h, g, EPI_STORE, g.n_rb * g.n_cb));
+    DFB_TRY(launch_add_row_vector(h, h->js_Sm, mbp, s, m, b.mu));
+    DFB_TRY(launch_copy_rows(h, h->js_Sm, mbp, samples_dev + (int64_t)s0 * m, m, s, m));
+  }
+  DFB_TRY(prof_end(h, DFB_PROF_TS_PRODUCT, 1.0));
+  *mbp_out = mbp;
   return 0;
 }
 
@@ -1691,35 +1806,45 @@ int dfb_ts_draws(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, dou
                  const double* Ut_dev, int32_t S, double jitter, double* samples_dev, double* mu_dev,
                  double* max_diag_host) {
   DFB_TRY(need(h, true, true, true, true, true));
-  if (Xc_dev == nullptr || Ut_dev == nullptr || samples_dev == nullptr || S < 1 || S > 256) { set_error("bad ts_draws arguments (1 <= S <= 256)"); return -1; }
+  if (Xc_dev == nullptr || Ut_dev == nullptr || samples_dev == nullptr || S < 1) { set_error("bad ts_draws arguments"); return -1; }
+  CovBufs b;
+  DFB_TRY(cov_bufs(h, m, &b));
+  if (!b.joint && S > 256) { set_error("bad ts_draws arguments (a block takes 1 <= S <= 256)"); return -1; }
   DFB_CUDA_OK(cudaSetDevice(h->device));
   int64_t mbp = 0;
-  DFB_TRY(posterior_covariance(h, Xc_dev, m, dc, mean_const, &mbp, true));
-  DFB_TRY(launch_diag_max(h, h->ts_Cov, mbp, m, h->ts_red));
-  // stable_cholesky(K) (general_utils.py:224-229): factorise Cov + jitter I (identity padding)
-  DFB_CUDA_OK(cudaMemsetAsync(h->ts_info, 0, sizeof(int) * 4, h->stream));
-  DFB_CUDA_OK(cudaMemsetAsync(h->ts_T, 0, sizeof(double) * (size_t)(2 * mbp + TILE) * mbp, h->stream));
-  DFB_TRY(launch_copy_rows(h, h->ts_Cov, mbp, h->ts_T, mbp, mbp, mbp));
-  DFB_TRY(launch_set_diag(h, h->ts_T, mbp, 0, m, jitter, 1));
-  DFB_TRY(launch_set_diag(h, h->ts_T, mbp, m, mbp, 1.0, 0));
-  DFB_TRY(factorise_tall(h, h->ts_T, mbp, h->Dinv, h->ts_info, false, false));
-  // samples^T = L_post U: samples[s][a] = sum_{b <= a} U^T[s][b] L[a][b]
-  const int64_t Sp = round_up(S, TILE);
-  DFB_CUDA_OK(cudaMemsetAsync(h->ts_Ut, 0, sizeof(double) * (size_t)Sp * mbp, h->stream));
-  DFB_TRY(launch_copy_rows(h, Ut_dev, m, h->ts_Ut, mbp, S, m));
-  GemmArgs g;
-  memset(&g, 0, sizeof(g));
-  g.A = h->ts_Ut; g.lda = mbp; g.B = h->ts_T; g.ldb = mbp; g.D = h->ts_Sm; g.ldd = mbp; g.alpha = 1.0;
-  g.mode = MODE_GENERIC; g.n_rb = (int)(Sp / TILE); g.n_cb = (int)(mbp / TILE); g.K = (int)mbp; g.tri = 2;
-  g.info = h->ts_info;
-  DFB_TRY(launch_gemm(h, g, EPI_STORE, g.n_rb * g.n_cb));
-  DFB_TRY(launch_add_row_vector(h, h->ts_Sm, mbp, S, m, h->ts_mu));
-  DFB_TRY(launch_copy_rows(h, h->ts_Sm, mbp, samples_dev, m, S, m));
-  if (mu_dev != nullptr) DFB_TRY(launch_copy_pad(h, h->ts_mu, m, mu_dev, m));
+  const double* red = h->ts_red;
+  const int* dinfo = h->ts_info;
+  if (b.joint) {
+    DFB_TRY(joint_draws(h, b, Xc_dev, m, dc, mean_const, Ut_dev, S, jitter, samples_dev, &mbp));
+    red = h->js_red; dinfo = h->js_info;
+  } else {
+    DFB_TRY(posterior_covariance(h, b, Xc_dev, m, dc, mean_const, &mbp, true));
+    DFB_TRY(launch_diag_max(h, h->ts_Cov, mbp, m, h->ts_red));
+    // stable_cholesky(K) (general_utils.py:224-229): factorise Cov + jitter I (identity padding)
+    DFB_CUDA_OK(cudaMemsetAsync(h->ts_info, 0, sizeof(int) * 4, h->stream));
+    DFB_CUDA_OK(cudaMemsetAsync(h->ts_T, 0, sizeof(double) * (size_t)(2 * mbp + TILE) * mbp, h->stream));
+    DFB_TRY(launch_copy_rows(h, h->ts_Cov, mbp, h->ts_T, mbp, mbp, mbp));
+    DFB_TRY(launch_set_diag(h, h->ts_T, mbp, 0, m, jitter, 1));
+    DFB_TRY(launch_set_diag(h, h->ts_T, mbp, m, mbp, 1.0, 0));
+    DFB_TRY(factorise_tall(h, h->ts_T, mbp, h->Dinv, h->ts_info, false, false));
+    // samples^T = L_post U: samples[s][a] = sum_{b <= a} U^T[s][b] L[a][b]
+    const int64_t Sp = round_up(S, TILE);
+    DFB_CUDA_OK(cudaMemsetAsync(h->ts_Ut, 0, sizeof(double) * (size_t)Sp * mbp, h->stream));
+    DFB_TRY(launch_copy_rows(h, Ut_dev, m, h->ts_Ut, mbp, S, m));
+    GemmArgs g;
+    memset(&g, 0, sizeof(g));
+    g.A = h->ts_Ut; g.lda = mbp; g.B = h->ts_T; g.ldb = mbp; g.D = h->ts_Sm; g.ldd = mbp; g.alpha = 1.0;
+    g.mode = MODE_GENERIC; g.n_rb = (int)(Sp / TILE); g.n_cb = (int)(mbp / TILE); g.K = (int)mbp; g.tri = 2;
+    g.info = h->ts_info;
+    DFB_TRY(launch_gemm(h, g, EPI_STORE, g.n_rb * g.n_cb));
+    DFB_TRY(launch_add_row_vector(h, h->ts_Sm, mbp, S, m, h->ts_mu));
+    DFB_TRY(launch_copy_rows(h, h->ts_Sm, mbp, samples_dev, m, S, m));
+  }
+  if (mu_dev != nullptr) DFB_TRY(launch_copy_pad(h, b.mu, m, mu_dev, m));
   double mx = 0.0;
   int info = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(&mx, h->ts_red, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaMemcpyAsync(&info, h->ts_info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(&mx, red, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(&info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
   if (max_diag_host != nullptr) *max_diag_host = mx;
   if (info != 0) { set_error("posterior covariance is not positive definite at jitter %g (pivot %d)", jitter, info - 1); return info; }
@@ -1824,6 +1949,10 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
     if (strcmp(name, "ts_Cov") == 0) { src = h->ts_Cov; size = (int64_t)sizeof(double) * mbp * mbp; }
     else if (strcmp(name, "ts_T") == 0) { src = h->ts_T; size = (int64_t)sizeof(double) * (2 * mbp + TILE) * mbp; }
     else { set_error("unknown debug_copy buffer '%s'", name); return -1; }
+  }
+  else if (strcmp(name, "js_Cov") == 0) {
+    if (h->js_ws == nullptr) { set_error("debug_copy '%s': no joint workspace is set", name); return -1; }
+    src = h->js_Cov; size = (int64_t)sizeof(double) * h->js_mb * h->js_mb;
   }
   else { set_error("unknown debug_copy buffer '%s'", name); return -1; }
   if (bytes != size) {

@@ -50,7 +50,7 @@ struct ScaledSet {        // scaled training coordinates for one kernel descript
 }  // namespace dfb
 
 namespace dfb {
-constexpr int PROF_CLASSES = 11;
+constexpr int PROF_CLASSES = 14;
 constexpr int PROF_RING = 1024;
 struct ProfClass {
   cudaEvent_t start[PROF_RING];
@@ -121,6 +121,20 @@ struct dfb_handle {
   double* ts_mu = nullptr;    // mbp
   double* ts_red = nullptr;   // 4
   int* ts_info = nullptr;
+
+  // optional joint Thompson-sampling workspace (api.cu: carve_joint()): one covariance over all candidates, factorised
+  // in place
+  char* js_ws = nullptr;
+  int64_t js_mb = 0;          // padded candidate capacity Mpad
+  double* js_Vt = nullptr;    // Mpad x npad  (L^-1 K_*^T)^T
+  double* js_cxs = nullptr;   // slots x Mpad
+  double* js_cnrm = nullptr;  // factors x Mpad
+  double* js_Cov = nullptr;   // Mpad x Mpad  posterior covariance, then its Cholesky factor (lower tiles)
+  double* js_Ut = nullptr;    // 256 x Mpad
+  double* js_Sm = nullptr;    // 256 x Mpad
+  double* js_mu = nullptr;    // Mpad
+  double* js_red = nullptr;   // 4
+  int* js_info = nullptr;
 
   // TMA path of the scoring contraction (gemm_tma.cuh)
   int gemm_impl = 1;          // 0 = v1 cp.async ring, 1 = v2 TMA + mbarrier ring (default)

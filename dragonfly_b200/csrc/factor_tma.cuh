@@ -1,5 +1,6 @@
 // The panel solve and the trailing update of the blocked factorisation of the tall matrix [A ; I ; y^T]
-// (api.cu: factorise_tall), on Hopper's TMA and mbarriers:
+// (api.cu: factorise_tall) -- or, with top_only, of the square A alone (the joint Thompson draw) -- on Hopper's TMA and
+// mbarriers:
 //   panel     P <- P inv(L_kk)^T        in place, for every structurally non-zero row block of column block `step`
 //   trailing  T_rj <- T_rj - P_r P_j^T   for every structurally non-zero tile of column blocks [j0, j1)
 //
@@ -34,10 +35,16 @@ constexpr size_t fu_smem_bytes(int bm, int bn) {
   return (size_t)FU_STAGES * (bm + bn) * GEMM_BK * sizeof(double) + 1024 /*align*/ + 2 * FU_STAGES * 8 /*barriers*/;
 }
 
+// Row blocks below the top square that are full in column block `step` and in every trailing column: L^-T rows
+// nb .. nb+step (absent with skip_bottom) and the y row block; none with top_only.
+__host__ __device__ inline int fu_full_rows(const FactorArgs& g) {
+  return g.top_only ? 0 : (g.skip_bottom ? 0 : g.step + 1) + 1;
+}
+
 // Row blocks of the tall matrix that are structurally non-zero in column block `step`, in the order the panel
-// visits them: top rows step+1 .. nb-1, L^-T rows nb .. nb+step (absent with skip_bottom), the y row block 2 nb.
+// visits them: top rows step+1 .. nb-1, then the full rows (L^-T rows nb .. nb+step, the y row block 2 nb).
 __host__ __device__ inline int fu_panel_rows(const FactorArgs& g) {
-  return (g.nb - g.step - 1) + (g.skip_bottom ? 0 : g.step + 1) + 1;
+  return (g.nb - g.step - 1) + fu_full_rows(g);
 }
 __device__ __forceinline__ int fu_panel_row(const FactorArgs& g, int t) {
   const int top = g.nb - g.step - 1;
@@ -46,17 +53,16 @@ __device__ __forceinline__ int fu_panel_row(const FactorArgs& g, int t) {
   return (!g.skip_bottom && t <= g.step) ? g.nb + t : 2 * g.nb;
 }
 
-// Non-zero tiles of the trailing update of column blocks [j0, j1): the rows that are full in every column (L^-T
-// rows nb .. nb+step, the y row block) first, row by row, then the top's lower triangle (row blocks j .. nb-1 of
-// column j) column by column.
+// Non-zero tiles of the trailing update of column blocks [j0, j1): the full rows first, row by row, then the top's
+// lower triangle (row blocks j .. nb-1 of column j) column by column.
 __host__ __device__ inline int fu_trail_tiles(const FactorArgs& g) {
   const int nc = g.j1 - g.j0;
-  const int full = (g.skip_bottom ? 0 : g.step + 1) + 1;
+  const int full = fu_full_rows(g);
   return full * nc + nc * g.nb - (g.j0 + g.j1 - 1) * nc / 2;
 }
 __device__ __forceinline__ void fu_trail_tile(const FactorArgs& g, int t, int& rbk, int& j) {
   const int nc = g.j1 - g.j0;
-  const int full = (g.skip_bottom ? 0 : g.step + 1) + 1;
+  const int full = fu_full_rows(g);
   if (t < full * nc) {
     const int r = t / nc;
     j = g.j0 + (t - r * nc);

@@ -19,20 +19,23 @@ int make_tensor_map_2d_f64(CUtensorMap* out, const double* base, int64_t rows, i
 int launch_score_tma(dfb_handle* h, const CUtensorMap& tmW, const CUtensorMap& tmK,
                      const ScoreTmaArgs& g);
 
-// One launch of factor_update_kernel (factor_tma.cuh) on the tall matrix T (ld x (2 ld + 128)) of a factorisation.
+// One launch of factor_update_kernel (factor_tma.cuh) on the tall matrix T (ld x (2 ld + 128)) of a factorisation, or
+// with top_only on the square ld x ld alone.
 struct FactorArgs {
   double* T; int64_t ld;
   int step, nb;
   int skip_bottom;          // the L^-T rows are absent (LML-only build)
+  int top_only;             // factor only: neither the L^-T rows nor the y row exist (T is ld x ld)
   int panel;                // 1: panel solve of column block `step`; 0: trailing update of column blocks [j0, j1)
   int j0, j1;
   const int* info;          // nullable: do nothing if *info != 0 (failed factorisation)
 };
-// The tensor maps the launches of one factorisation read: T in boxes of 32, 64 and 128 rows, inv(L_kk)^T.
+// The tensor maps the launches of one factorisation read: T (rows x npad) in boxes of 32, 64 and 128 rows,
+// inv(L_kk)^T.
 struct FactorMaps {
   CUtensorMap t32, t64, t128, dinv;
 };
-int make_factor_maps(FactorMaps* out, const double* T, int64_t npad, const double* Dinv);
+int make_factor_maps(FactorMaps* out, const double* T, int64_t rows, int64_t npad, const double* Dinv);
 // chain = true: the 32 x 128 sub-tiles of the critical path (panel(k), next(k)); false: the 128 x 64 bulk shape.
 // Panel launches take the chain shape only.
 int launch_factor_update(dfb_handle* h, const FactorMaps& m, const FactorArgs& g, bool chain);

@@ -254,8 +254,37 @@ class DevicePosterior(object):
         'dfb_score_argmax_ts')
     return bs.value, bi.value, sc, nonpos.value
 
-  # -- joint posterior over one block: covariance and Thompson draws -----------------------------
+  # -- joint posterior over one block, or over all candidates: covariance and Thompson draws ---------
   TS_BLOCK = 4096
+  # Above TS_BLOCK and up to TS_JOINT_MAX candidates, the covariance and the draws are formed over all candidates at
+  # once in a joint workspace (about 8 Mpad^2 + 8 Mpad npad bytes: 2.9 GB at M = 16384, N = 5000), allocated on the
+  # first such call and grown when a larger M comes.  The form depends on M alone; a joint call that cannot get its
+  # workspace raises.
+  TS_JOINT_MAX = 16384
+
+  def _ensure_workspace_for(self, m):
+    if m <= self.TS_BLOCK:
+      self._ensure_ts_workspace(m)
+    elif m <= self.TS_JOINT_MAX:
+      self._ensure_joint_workspace(m)
+    else:
+      raise ValueError('%d candidates: the joint posterior takes at most %d (TS_JOINT_MAX).' % (m, self.TS_JOINT_MAX))
+
+  def _ensure_joint_workspace(self, m):
+    if getattr(self, '_js_m', 0) >= m:
+      return
+    mj = min(self.TS_JOINT_MAX, (int(m) + 1023) // 1024 * 1024)
+    # Give the old workspace back before taking a larger one.  The handle still points into it until
+    # dfb_set_joint_workspace succeeds, so no capacity is recorded meanwhile: if the allocation below raises, the next
+    # joint call allocates again instead of writing into memory the caching allocator may have handed on.
+    self._js_m = 0
+    self._js_workspace = None
+    nbytes = self.lib.dfb_joint_workspace_bytes(self.n_max, mj)
+    self._js_workspace = torch.empty(int(nbytes) + 256, dtype=torch.uint8, device=self.device)
+    ptr = (self._js_workspace.data_ptr() + 255) // 256 * 256
+    _lib.check(self.lib.dfb_set_joint_workspace(self.h, C.c_void_p(ptr), C.c_size_t(nbytes), mj),
+               'dfb_set_joint_workspace')
+    self._js_m = mj
 
   def _ensure_ts_workspace(self, m):
     mb = getattr(self, '_ts_mb', 0)
@@ -270,10 +299,11 @@ class DevicePosterior(object):
     self._ts_mb = mb
 
   def eval_covar(self, Xc, mean_const=0.0):
-    """ (mu, covar) of GP.eval(X, 'covar') for one block; host ndarray in -> host ndarrays out. """
+    """ (mu, covar) of GP.eval(X, 'covar') for up to TS_JOINT_MAX candidates (one block up to TS_BLOCK);
+        host ndarray in -> host ndarrays out. """
     Xd = _dev_f64(Xc, self.device)
     m, dc = int(Xd.shape[0]), int(Xd.shape[1])
-    self._ensure_ts_workspace(m)
+    self._ensure_workspace_for(m)
     mu = torch.empty((m,), dtype=torch.float64, device=self.device)
     cov = torch.empty((m, m), dtype=torch.float64, device=self.device)
     _lib.check(self.lib.dfb_eval_covar(self.h, C.c_void_p(Xd.data_ptr()), m, dc, float(mean_const),
@@ -284,13 +314,14 @@ class DevicePosterior(object):
     return mu.cpu().numpy(), cov.cpu().numpy()
 
   def ts_draws(self, Xc, Ut, mean_const=0.0, jitter=0.0):
-    """ One attempt of draw_gaussian_samples on a block: returns (info, samples (S, m), max_diag). """
+    """ One attempt of draw_gaussian_samples on a block (m <= TS_BLOCK, S <= 256), or jointly over all
+        m <= TS_JOINT_MAX candidates (any S, one factorisation): returns (info, samples (S, m), max_diag). """
     Xd = _dev_f64(Xc, self.device)
     Ud = _dev_f64(Ut, self.device)
     m, dc = int(Xd.shape[0]), int(Xd.shape[1])
     S = int(Ud.shape[0])
     assert int(Ud.shape[1]) == m
-    self._ensure_ts_workspace(m)
+    self._ensure_workspace_for(m)
     out = torch.empty((S, m), dtype=torch.float64, device=self.device)
     mx = C.c_double(0.0)
     info = _lib.check(self.lib.dfb_ts_draws(self.h, C.c_void_p(Xd.data_ptr()), m, dc, float(mean_const),

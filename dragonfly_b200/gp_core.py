@@ -102,6 +102,28 @@ def stable_cholesky_on_device(post, noise_var, add_to_diag_till_psd=True, flags=
                         'has infinities/nans.') % (diag_noise))
 
 
+def joint_draw_on_device(post, Xm, Ut, mean_const):
+  """ draw_gaussian_samples (general_utils.py:224-232) over all M candidates at once: stable_cholesky's ladder on
+      the joint device draw -- jitter 0, then 10^p * max(diag covariance) for p = -11, -10, ...; ValueError once p
+      reaches 5.  Each attempt forms the covariance again and factorises it once for all S draws.  Ut: the (S, M)
+      normals.  Returns (samples (S, M) ndarray, jitter power or None). """
+  info, smp, max_diag = post.ts_draws(Xm, Ut, mean_const=mean_const, jitter=0.0)
+  power = None
+  if info != 0:
+    power = -11
+    while True:
+      jitter = (10 ** power) * max_diag
+      info, smp, _ = post.ts_draws(Xm, Ut, mean_const=mean_const, jitter=jitter)
+      if info == 0:
+        break
+      power += 1
+      if power >= 5:
+        raise ValueError('Could not compute Cholesky decomposition despite adding %0.4f to '
+                         'the diagonal.' % (jitter))
+  smp = smp.cpu().numpy() if hasattr(smp, 'cpu') else np.asarray(smp)
+  return smp, power
+
+
 # What INTEGRATION.md's recipe copies onto the reference's own dragonfly.gp.gp_core.GP (setattr by name): the
 # public methods the device path replaces plus the private helpers they call.
 # Kept by the reference class: its constructor / set-up, data bookkeeping and printing.
@@ -465,12 +487,13 @@ class GP(object):
     return self._eval_on(self._post, X_test, uncert_form == 'std')
 
   def _eval_covar_on(self, post, X_test):
-    """ The full M x M posterior covariance (gp_core.py:179-185) -- one device block, so M is
-        bounded (DevicePosterior.TS_BLOCK); 'std' is the path for large M. """
+    """ The full M x M posterior covariance (gp_core.py:179-185) -- one device block up to
+        DevicePosterior.TS_BLOCK, the joint workspace up to TS_JOINT_MAX, so M is bounded; 'std' is the path
+        for large M. """
     Xm = self._test_matrix(X_test)
-    if len(Xm) > post.TS_BLOCK:
+    if len(Xm) > post.TS_JOINT_MAX:
       raise NotImplementedError('uncert_form="covar" materialises an M x M matrix; M = %d exceeds '
-                                'the device block of %d.' % (len(Xm), post.TS_BLOCK))
+                                'the device limit of %d.' % (len(Xm), post.TS_JOINT_MAX))
     mc = self._mean_const_for(X_test)
     if mc is not None:
       return post.eval_covar(Xm, mean_const=mc)
@@ -567,19 +590,23 @@ class GP(object):
 
   # -- sampling (gp_core.py:250-261) --------------------------------------------------------------------
   def _draw_samples_on(self, post, num_samples, X_test, cols=None):
-    """ draw_gaussian_samples (general_utils.py:224-232) per block of <= TS_BLOCK candidates:
-        L = stable_cholesky(covar) with the same jitter ladder, U = np.random.normal(size=(M, S))
-        drawn ONCE from the global RNG exactly like the reference, samples = (L U)^T + mu.
-        DEVIATION from the reference for M > TS_BLOCK (min(4096, the handle's scoring chunk)): blocks are
+    """ draw_gaussian_samples (general_utils.py:224-232): L = stable_cholesky(covar) with the same jitter
+        ladder, U = np.random.normal(size=(M, S)) drawn ONCE from the global RNG exactly like the reference,
+        samples = (L U)^T + mu.  Up to TS_JOINT_MAX (16384) candidates in ONE joint draw -- one block up to
+        TS_BLOCK (min(4096, the handle's scoring chunk)), the joint workspace above -- exact and seed-identical
+        to the reference.  DEVIATION from the reference for M > TS_JOINT_MAX: blocks of TS_BLOCK candidates are
         sampled INDEPENDENTLY of each other -- the reference's single joint draw needs the M x M covariance
         (8 TB at M = 10^6) -- so cross-block correlations are dropped and the sample matrix is not the one
-        the reference's RNG stream would give (DESIGN.md 7).  Exact, and seed-identical, for M <= TS_BLOCK. """
+        the reference's RNG stream would give (DESIGN.md 7).  `cols` (whole blocks of one rank) applies to
+        that block form only. """
     Xm = self._test_matrix(X_test)
     mean_c = self._mean_const_for(X_test)
     if mean_c is None:
       raise NotImplementedError('Thompson sampling on device needs a constant mean function.')
     M = len(Xm)
     U = np.random.normal(size=(M, int(num_samples)))
+    if post.TS_BLOCK < M <= post.TS_JOINT_MAX:
+      return joint_draw_on_device(post, Xm, np.ascontiguousarray(U.T), mean_c)[0]
     out = np.empty((int(num_samples), M))
     if cols is not None:
       # multi-GPU sharding by whole blocks (gpb_acquisitions._draw_one_sample): foreign blocks stay -inf

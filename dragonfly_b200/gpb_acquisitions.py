@@ -837,27 +837,33 @@ def _cp_ts(gp, anc_data):
   return _cp_fused_maximise(gp, anc_data, None)
 
 
-def _ts_block(gp):
+def _ts_limits(gp):
+  """ (TS_BLOCK, TS_JOINT_MAX) of the GP's device posterior. """
   post = getattr(gp, '_post', None) or getattr(getattr(gp, 'mfgp', None), '_post', None)
-  return int(getattr(post, 'TS_BLOCK', 4096))
+  return int(getattr(post, 'TS_BLOCK', 4096)), int(getattr(post, 'TS_JOINT_MAX', 16384))
 
 
 def _ts_cols(gp, n_rows):
-  """ This rank's share [lo, hi) of the candidate rows, in whole TS blocks; None when not distributed. """
+  """ This rank's share [lo, hi) of the candidate rows, in whole TS blocks; None when not distributed, and when
+      the candidates take one joint draw (TS_BLOCK < n_rows <= TS_JOINT_MAX): every rank then computes the whole
+      draw. """
   rank, world, _ = _shard_info()
   if world == 1:
     return None
+  blk, joint_max = _ts_limits(gp)
+  if blk < n_rows <= joint_max:
+    return None
   from . import dist as dfb_dist
-  blk = _ts_block(gp)
   b_lo, b_hi = dfb_dist.shard_bounds((n_rows + blk - 1) // blk, rank, world)
   return (min(b_lo * blk, n_rows), min(b_hi * blk, n_rows))
 
 
 def _draw_one_sample(gp, rand_pts, halluc):
-  """ One joint posterior draw over the candidates (gp_core.py:250-261).  Under torch.distributed each rank
-      computes only its share of the independent 4096-candidate blocks (DESIGN.md 7) -- the normals are still
-      drawn for ALL candidates so that every rank consumes the global RNG like the single-process run -- and
-      the entries of the other ranks' blocks are -inf. """
+  """ One joint posterior draw over the candidates (gp_core.py:250-261).  Up to TS_JOINT_MAX candidates every rank
+      computes the whole joint draw.  Above it, under torch.distributed, each rank computes only its share of the
+      independent 4096-candidate blocks (DESIGN.md 7) -- the normals are still drawn for ALL candidates so that every
+      rank consumes the global RNG like the single-process run -- and the entries of the other ranks' blocks are
+      -inf. """
   cols = _ts_cols(gp, len(rand_pts))
   kw = {} if cols is None else {'cols': cols}
   if len(halluc) > 0:

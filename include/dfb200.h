@@ -273,9 +273,17 @@ int dfb_mu_upper_bound(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, i
  * of up to `mb` candidates at a time (mb <= the scoring chunk).  */
 size_t dfb_ts_workspace_bytes(int64_t n_max, int64_t mb);
 int    dfb_set_ts_workspace(dfb_handle* h, void* workspace_dev, size_t bytes, int64_t mb);
+/* Optional workspace for the JOINT posterior over up to m candidates at once (dfb_eval_covar, dfb_ts_draws for more
+ * candidates than the TS workspace or the scoring chunk holds): about 8 Mpad^2 + 8 Mpad npad bytes plus 4 KB per
+ * candidate (Mpad = m rounded up to 128, npad = n_max rounded up to 128; ~2.9 GB at m = 16384, n_max = 5000).
+ * Caller-owned device memory, 256-byte aligned.  The covariance is factorised in place, so no second M x M matrix. */
+size_t dfb_joint_workspace_bytes(int64_t n_max, int64_t m);
+int    dfb_set_joint_workspace(dfb_handle* h, void* workspace_dev, size_t bytes, int64_t m);
 
 /* GP.eval(X_test, 'covar') (gp_core.py:165-187): mu (m) and the full m x m posterior covariance
- * K** - V^T V, V = L^-1 K_*^T (device pointers; m <= mb).  Used by draw_samples (gp_core.py:250-254). */
+ * K** - V^T V, V = L^-1 K_*^T (device pointers).  Block form when the TS workspace holds m within one scoring
+ * chunk, else the joint form when the joint workspace holds m; the leading q x q of a joint covariance is bit for bit
+ * the block covariance of the first q candidates.  Used by draw_samples (gp_core.py:250-254). */
 int dfb_eval_covar(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, double mean_const,
                    double* mu_dev, double* covar_dev);
 
@@ -412,11 +420,13 @@ int dfb_kernel_matrix(dfb_handle* h, const dfb_kernel_desc* desc, const double* 
 
 /* Thompson sampling (asy_ts, gpb_acquisitions.py:119-127; GP.draw_samples, gp_core.py:250-254;
  * draw_gaussian_samples, general_utils.py:224-232): samples = (L_post U)^T + mu with
- * L_post = chol(K** - V^T V + jitter I) for ONE block of m <= mb candidates.  Ut_dev is U^T, the
- * S x m matrix of standard normals (drawn on the host with np.random.normal for parity),
- * samples_dev is S x m, mu_dev (m) may be NULL.  max_diag_host receives max(diag covariance), the
- * scale of stable_cholesky's jitter ladder.  Returns info > 0 if the covariance is not PD at this
- * jitter (the host then walks the ladder, general_utils.py:183-203).  S <= 256 per call.  */
+ * L_post = chol(K** - V^T V + jitter I) for ONE block of m <= mb candidates (TS workspace, S <= 256 per call), or
+ * jointly over all m candidates when only the joint workspace holds them (dfb_set_joint_workspace; any S, one
+ * factorisation per call, the product in passes of 256 draws).  Ut_dev is U^T, the S x m matrix of standard normals
+ * (drawn on the host with np.random.normal for parity), samples_dev is S x m, mu_dev (m) may be NULL.  max_diag_host
+ * receives max(diag covariance), the scale of stable_cholesky's jitter ladder.  Returns info > 0 if the covariance
+ * is not PD at this jitter (the host then walks the ladder, general_utils.py:183-203; each attempt forms the
+ * covariance again).  */
 int dfb_ts_draws(dfb_handle* h, const double* Xc_dev, int64_t m, int32_t dc, double mean_const,
                  const double* Ut_dev, int32_t S, double jitter, double* samples_dev, double* mu_dev,
                  double* max_diag_host);
@@ -442,7 +452,10 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
  * 128, whose data sits at the start of each buffer with leading dimension q): "ts_Cov" (mbp^2 doubles: the padded
  * posterior covariance of the last dfb_eval_covar / dfb_ts_draws block, q x q; dfb_ts_draws writes its lower tiles
  * only) and "ts_T" ((2 mbp + 128) mbp doubles: the tall matrix dfb_ts_draws factorised, (2 q + 128) x q, whose top is
- * the factor of Cov + jitter I); without a TS workspace these two names are an error.
+ * the factor of Cov + jitter I); without a TS workspace these two names are an error.  With a joint workspace
+ * (Mpad = its m rounded up to 128, q = the last joint call's m rounded up to 128, ld q): "js_Cov" (Mpad^2 doubles:
+ * after dfb_eval_covar the q x q covariance, after dfb_ts_draws its Cholesky factor in the lower tiles, zero above the
+ * diagonal inside the diagonal tiles, the covariance's K** part in the upper tiles).
  * Synchronises. */
 int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes);
 /* Diagnostics (tests/test_gpu_prune_f32.py): the largest relative error of ex2.approx.ftz.f32 (which = 0) over every
@@ -532,6 +545,12 @@ int dfb_query(dfb_handle* h, const char* name, double* out);
 #define DFB_PROF_BUILD_REST  8
 #define DFB_PROF_BUILD_TAIL  9
 #define DFB_PROF_BUILD_I8    10
+/* The stages of a joint dfb_ts_draws (more candidates than one block; tools/bench_ts_joint.py), one interval per call
+ * on the handle's stream, units = intervals: 11 = the covariance (K_*, V^T, K**, Sigma = K** - V^T V), 12 = the
+ * factor-only factorisation of Sigma + jitter I, 13 = the L U product passes with mu and the copy-out. */
+#define DFB_PROF_TS_COV      11
+#define DFB_PROF_TS_FACTOR   12
+#define DFB_PROF_TS_PRODUCT  13
 int dfb_profile_enable(dfb_handle* h, int on);
 int dfb_profile_read(dfb_handle* h, int cls, double* ms_total, int64_t* launches, double* units);
 
