@@ -38,7 +38,11 @@ distance, gamma_k = k u / (1 - k u).
     the fused constant of kstar_seg and its product: at most 5 roundings) and c_v = 24 for Matern (exp; the
     constants Gamma(p+1)/Gamma(2p+1), norm_constant and the scale product, 4 roundings; the polynomial in
     mm = sqrt(8 nu) r: 8 u relative for p <= 2 since every coefficient is a positive integer; the products with the
-    exponential and the scales, or kstar_seg's fused constant, 5 roundings).  The exponent argument of Matern,
+    exponential and the scales, or kstar_seg's fused constant, 5 roundings).  Matern-7/2 (p = 3, only the descriptor
+    interpreter evaluates it) forms mm ** 3 with pow: mm carries 2 roundings (fl(sqrt(8 nu)) and the product), pow
+    adds at most 2 ulp = 4 u (CUDA documents 2 ulp; NumPy's libm pow is within 1 ulp), so mm ** 3 is within 10 u,
+    its coefficient product 11 u, and the three adds of positive terms make the polynomial 14 u instead of 8 u:
+    c_v = 24 + 6 = 30, taken as 32.  The exponent argument of Matern,
     -fl(sqrt(2 nu)) r^, carries 2u of relative error, which multiplies K by at most exp(2.0001 u sqrt(2 nu) r_hi).
     An absolute 1e-290 |s| covers the exponential's flush to zero below -707 and subnormal intermediates.
 
@@ -52,8 +56,19 @@ import numpy as np
 
 U = 2.0 ** -53
 LD = np.longdouble
+# the kinds of the plain K_* producers (and of the bound pass built on them): Matern p <= 2
 KINDS = {'se': ('se', 0), 'matern12': ('matern', 0), 'matern32': ('matern', 1), 'matern52': ('matern', 2)}
+# the kinds the descriptor interpreter evaluates as well: Matern-7/2 (p = 3) too
+INTERP_KINDS = dict(KINDS, matern72=('matern', 3))
 C_V = {'se': 8.0, 'matern': 24.0}
+C_V_MATERN_POW = 32.0          # Matern with p >= 3: the polynomial's leading power comes from pow
+
+
+def c_v(kind, p):
+  """ The multiple of u |K| of step 4 (module docstring). """
+  if kind == 'matern' and p >= 3:
+    return C_V_MATERN_POW
+  return C_V[kind]
 
 
 def gamma_d(d):
@@ -65,16 +80,23 @@ def _scaled(Z, bw):
   return np.asarray(Z, dtype=np.float64).astype(LD) / np.asarray(bw, dtype=np.float64).astype(LD)
 
 
-def _d2_and_s(Xc, X, bw):
-  """ Exact (longdouble) D^2 from the scaled differences and S = |a|^2 + |b|^2, both (m, n). """
+def pair(a, b, diag=False):
+  """ Column vectors a (m,) and b (n,) as operands of an entrywise operation: (m, n) outer form, or (m,) entries
+      (a_i, b_i) when diag (m = n: the diagonal of the (m, n) form without the rest). """
+  if diag:
+    return a, b
+  return a[:, None], b[None, :]
+
+
+def _d2_and_s(Xc, X, bw, diag=False):
+  """ Exact (longdouble) D^2 from the scaled differences and S = |a|^2 + |b|^2, both (m, n) (or (m,) when diag). """
   A, B = _scaled(Xc, bw), _scaled(X, bw)
-  m, n = A.shape[0], B.shape[0]
-  d2 = np.zeros((m, n), dtype=LD)
+  d2 = LD(0)
   for q in range(A.shape[1]):
-    diff = A[:, q][:, None] - B[:, q][None, :]
-    d2 += diff * diff
-  s = (A * A).sum(axis=1)[:, None] + (B * B).sum(axis=1)[None, :]
-  return d2, s
+    a, b = pair(A[:, q], B[:, q], diag)
+    diff = a - b
+    d2 = d2 + diff * diff
+  return d2, sum(pair((A * A).sum(axis=1), (B * B).sum(axis=1), diag))
 
 
 def _matern_consts(p):
@@ -101,18 +123,20 @@ def _se_of_d2(scale, d2):
   return LD(scale) * np.exp(-d2 / LD(2))
 
 
-def kernel_exact(kind, p, scale, bw, Xc, X):
-  """ k(Xc_i, X_j) in longdouble, (m, n).  kind 'se' or 'matern' (nu = p + 1/2); scale = k(x, x), the product of
-      every scale factor of the kernel (for a Matern kernel, hyperparams['scale']); bw the d bandwidths. """
-  d2, _ = _d2_and_s(Xc, X, bw)
+def kernel_exact(kind, p, scale, bw, Xc, X, diag=False):
+  """ k(Xc_i, X_j) in longdouble, (m, n) (or k(Xc_i, X_i), (m,), when diag).  kind 'se' or 'matern' (nu = p + 1/2);
+      scale = k(x, x), the product of every scale factor of the kernel (for a Matern kernel, hyperparams['scale']); bw
+      the d bandwidths. """
+  d2, _ = _d2_and_s(Xc, X, bw, diag)
   if kind == 'se':
     return _se_of_d2(scale, d2)
   return _matern_of_r(p, scale, np.sqrt(d2))
 
 
-def kstar_bound(kind, p, scale, bw, Xc, X):
-  """ Per-entry bound on |K^ - K| for any fp64 evaluation of the kernels' form (module docstring), (m, n) float64. """
-  d2, s = _d2_and_s(Xc, X, bw)
+def kstar_bound(kind, p, scale, bw, Xc, X, diag=False):
+  """ Per-entry bound on |K^ - K| for any fp64 evaluation of the kernels' form (module docstring), (m, n) float64
+      (or (m,) when diag). """
+  d2, s = _d2_and_s(Xc, X, bw, diag)
   d = np.shape(bw)[0] if np.ndim(bw) else np.shape(Xc)[1]
   delta = LD(gamma_d(d)) * s
   u2 = LD(2 * U)
@@ -120,7 +144,7 @@ def kstar_bound(kind, p, scale, bw, Xc, X):
     k = _se_of_d2(scale, d2)
     k_lo, k_hi = _se_of_d2(scale, d2 - delta), _se_of_d2(scale, d2 + delta)
     prop = np.maximum(np.abs(k_lo - k), np.abs(k - k_hi))
-    eval_err = LD(C_V['se'] * U) * np.abs(k_lo)
+    eval_err = LD(c_v(kind, p) * U) * np.abs(k_lo)
   else:
     r = np.sqrt(d2)
     r_lo = np.sqrt(np.maximum(d2 - delta, LD(0))) * (LD(1) - u2)
@@ -130,7 +154,7 @@ def kstar_bound(kind, p, scale, bw, Xc, X):
     prop = np.maximum(np.abs(k_lo - k), np.abs(k - k_hi))
     s2 = _matern_consts(p)[3]
     arg = np.expm1(LD(2.0001 * U) * s2 * r_hi)
-    eval_err = (LD(C_V['matern'] * U) + arg) * np.abs(k_lo)
+    eval_err = (LD(c_v(kind, p) * U) + arg) * np.abs(k_lo)
   # longdouble rounding of the reference itself (2^-60 |K|) and the absolute floor
   b = prop + eval_err + LD(2.0 ** -60) * np.abs(k_lo) + LD(1e-290) * abs(LD(scale))
   return b.astype(np.float64)
