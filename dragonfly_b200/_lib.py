@@ -22,6 +22,7 @@ DFB_ACQ_MEAN, DFB_ACQ_UCB, DFB_ACQ_EI, DFB_ACQ_PI, DFB_ACQ_TTEI, DFB_ACQ_TS_MARG
 DFB_BUILD_FULL, DFB_BUILD_LML_ONLY, DFB_BUILD_NO_ALPHA = 0, 1, 2
 DFB_EXTEND_SAVE = 16
 DFB_MOO_MAX_OBJ = 8
+DFB_MAX_GROUPS = 48
 DFB_RNG_NORMAL, DFB_RNG_UNIFORM = 0, 1
 DFB_PEAK_I8, DFB_PEAK_DMMA_F64 = 0, 1
 DFB_MOO_LIN_UCB, DFB_MOO_TCH_UCB, DFB_MOO_LIN_VAL, DFB_MOO_TCH_VAL = 0, 1, 2, 3
@@ -100,6 +101,8 @@ PROTOTYPES = {
   'dfb_eval_covar': (C.c_int, [_P, _P, _I64, _I32, _D, _P, _P]),
   'dfb_score_argmax': (C.c_int, [_P, C.POINTER(AcqDesc), _P, _I64, _I32, _I32, _D, _P,
                                  C.POINTER(_D), C.POINTER(_I64)]),
+  'dfb_score_groups': (C.c_int, [_P, C.POINTER(KernelDesc), C.POINTER(_D), _I32, _P, _I64, _I32, C.POINTER(_I32),
+                                 _P]),
   'dfb_score_argmax_ts': (C.c_int, [_P, _P, _I64, _I32, _I32, _D, _P, C.c_uint64, _I64, _P, C.POINTER(_D),
                                     C.POINTER(_I64), C.POINTER(_I64)]),
   'dfb_moo_score_argmax': (C.c_int, [_P, C.POINTER(MooDesc), C.POINTER(_P), C.POINTER(_P), _I64, _P,

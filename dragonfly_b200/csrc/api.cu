@@ -97,6 +97,7 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   dfb_kernel_desc* d0 = c.take<dfb_kernel_desc>(1);
   dfb_kernel_desc* d1 = c.take<dfb_kernel_desc>(1);
   dfb_kernel_desc* d2 = c.take<dfb_kernel_desc>(1);
+  dfb_kernel_desc* d_grp = c.take<dfb_kernel_desc>(DFB_MAX_GROUPS);
   // dfb_extend_posterior's snapshot of what it overwrites: the last row block of L, the last block
   // column of L^-T, that block of the y row, alpha
   double* ext_save = c.take<double>((size_t)(2 * TILE + 1) * npad + TILE);
@@ -115,7 +116,7 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
     h->surv_cap = surv_cap; h->surv_idx = surv_idx; h->surv_X = surv_X; h->surv_count = surv_count;
     h->keep_words = keep_words; h->keep_cap = keep_cap;
     h->best_index = best_index; h->red = red; h->info = info;
-    h->d_desc_tr = d0; h->d_desc_te = d1; h->d_desc_tmp = d2;
+    h->d_desc_tr = d0; h->d_desc_te = d1; h->d_desc_tmp = d2; h->d_desc_grp = d_grp;
     h->n_max = n_max; h->npad_max = npad; h->chunk = chunk;
   }
   return c.off + 256;
@@ -728,6 +729,30 @@ struct CandidateStage {
   }
 };
 
+// The fp64 tile contraction of the G stage: per 128-row block of W, the partial |L^-1 k_*|^2 of the first m_rows rows
+// of h->Ks into h->partial (leading dimension: the chunk).
+static int contract_tiles_f64(dfb_handle* h, int64_t m_rows) {
+  const int64_t npad = h->npad;
+  GemmArgs g;
+  memset(&g, 0, sizeof(g));
+  g.A = h->W; g.lda = npad; g.B = h->Ks; g.ldb = npad; g.mode = MODE_SCORE;
+  g.n_rb = (int)(npad / TILE); g.n_cb = (int)(m_rows / TILE); g.K = (int)npad;
+  g.partial = h->partial; g.ld_partial = h->chunk;
+  if (h->gemm_impl == 1 && h->tma_ready) {
+    ScoreTmaArgs ta;
+    ta.n_rb = g.n_rb; ta.n_cb = g.n_cb; ta.K = g.K; ta.partial = g.partial; ta.ld_partial = g.ld_partial;
+    ta.cb_group = h->tma_cb_group;
+    return launch_score_tma(h, h->tmW, h->tmK, ta);
+  }
+  return launch_gemm(h, g, EPI_SUMSQ, g.n_rb * g.n_cb);
+}
+
+// The row-streaming contraction of dfb_eval applies to m <= SMALL_EVAL_M rows when option small_eval is on and the
+// per-warp partials fit h->partial.
+static bool small_eval_fits(const dfb_handle* h) {
+  return h->small_eval != 0 && (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)(h->npad / TILE) * h->chunk;
+}
+
 // Per chunk two stages, back to back on the handle's stream:
 //   K: K_* rows / digit planes + mu + k(x*,x*)                                      fp64 pipe
 //   G: the contraction |L^-1 k_*|^2 -> sd / acquisition / arg-max / shortlist       tensor pipe (int8) or DMMA
@@ -743,8 +768,7 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   CandidateStage st;
   DFB_TRY(st.open(h, Xc, m, dc, space));
   const int* abort_count = md.collect ? h->list_count : nullptr;
-  const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M &&
-                     (int64_t)((h->n + 7) / 8 * 8) * SMALL_EVAL_M <= (int64_t)nb * Mc;
+  const bool small = want_std && md.allow_small && !md.use_i8 && m <= SMALL_EVAL_M && small_eval_fits(h);
   // K_* arguments of every chunk; the candidates, their count and mu are set per chunk
   KstarArgs ka{};
   ka.desc = &k.desc; ka.d_desc = k.d_desc; ka.xsT = k.ss.xs; ka.nrmT = k.ss.nrm; ka.npad_tr = npad; ka.alpha = h->alpha;
@@ -784,24 +808,14 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
       DFB_TRY(launch_small_sumsq(h, h->W, npad, h->Ks, npad, h->n, (int)mc, h->partial, SMALL_EVAL_M, &small_warps));
       DFB_TRY(prof_end(h, DFB_PROF_GEMM, (double)mc));
     } else if (want_std) {
-      GemmArgs g;
-      memset(&g, 0, sizeof(g));
-      g.A = h->W; g.lda = npad; g.B = h->Ks; g.ldb = npad; g.mode = MODE_SCORE;
-      g.n_rb = nb; g.n_cb = (int)(m_rows / TILE); g.K = (int)npad;
-      g.partial = h->partial; g.ld_partial = Mc;
       DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
       if (md.use_i8) {
         const double colscale = i8_colscale(k.desc);
         DFB_TRY(launch_score_i8_args(h, h->i8_radix256 != 0, h->tmWi8, h->tmKi8, nb,
                                      (int)(m_rows / i8_tile_n(h->i8_radix256)), (int)npad, h->partial, Mc,
                                      h->rowscale, colscale, abort_count));
-      } else if (h->gemm_impl == 1 && h->tma_ready) {
-        ScoreTmaArgs ta;
-        ta.n_rb = g.n_rb; ta.n_cb = g.n_cb; ta.K = g.K; ta.partial = g.partial; ta.ld_partial = g.ld_partial;
-        ta.cb_group = h->tma_cb_group;
-        DFB_TRY(launch_score_tma(h, h->tmW, h->tmK, ta));
       } else {
-        DFB_TRY(launch_gemm(h, g, EPI_SUMSQ, g.n_rb * g.n_cb));
+        DFB_TRY(contract_tiles_f64(h, m_rows));
       }
       DFB_TRY(prof_end(h, DFB_PROF_GEMM, (double)mc));
     }
@@ -1296,6 +1310,129 @@ int dfb_eval(dfb_handle* h, const double* Xc, int64_t m, int32_t dc, int32_t spa
   h->last_used_i8 = md.use_i8 ? 1 : 0;
   DFB_TRY(run_chunks(h, acq, Xc, m, dc, space, mean_const, out, md));
   DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// dfb_score_groups.  The groups' descriptors go to h->d_desc_grp and their scaled training sets side by side into the
+// test-kernel set h->te (group g from slot / factor offset sum_{g' < g} n_slots / n_factors), which is re-prepared when
+// a test kernel is next used.  Rows are put in group order, staged packed (each group's rows with its own column count),
+// and scored SMALL_EVAL_M at a time: per group present in a pass, one K_* launch writes its rows' K_*, mu and k(x*, x*)
+// at their place in the pass; one contraction covers the pass; per group, one acquisition launch with its beta.
+int dfb_score_groups(dfb_handle* h, const dfb_kernel_desc* descs, const double* betas, int32_t n_groups,
+                     const double* X_host, int64_t m, int32_t ldx, const int32_t* group_host, double* scores_host) {
+  DFB_TRY(need(h, true, true, true, true, true));
+  if (descs == nullptr || betas == nullptr || n_groups < 1 || n_groups > DFB_MAX_GROUPS) {
+    set_error("score_groups: n_groups = %d outside [1, %d] or NULL descriptors", n_groups, DFB_MAX_GROUPS);
+    return -1;
+  }
+  if (ldx < 1 || ldx > DFB_MAX_SLOTS) {
+    set_error("score_groups: ldx = %d outside [1, %d]", ldx, DFB_MAX_SLOTS);
+    return -1;
+  }
+  if (m < 0 || (m > 0 && (X_host == nullptr || group_host == nullptr || scores_host == nullptr))) {
+    set_error("bad score_groups arguments (m = %lld)", (long long)m);
+    return -1;
+  }
+  std::vector<int> slot_off(n_groups + 1, 0), fac_off(n_groups + 1, 0);
+  for (int g = 0; g < n_groups; g++) {
+    DFB_TRY(check_desc(&descs[g]));
+    slot_off[g + 1] = slot_off[g] + descs[g].n_slots;
+    fac_off[g + 1] = fac_off[g] + descs[g].n_factors;
+  }
+  if (slot_off[n_groups] > DFB_MAX_SLOTS || fac_off[n_groups] > DFB_MAX_FACTORS) {
+    set_error("score_groups: the groups use %d slots and %d factors (at most %d and %d)", slot_off[n_groups],
+              fac_off[n_groups], DFB_MAX_SLOTS, DFB_MAX_FACTORS);
+    return -1;
+  }
+  for (int64_t r = 0; r < m; r++) {
+    if (group_host[r] < 0 || group_host[r] >= n_groups) {
+      set_error("score_groups: row %lld has group %d", (long long)r, group_host[r]);
+      return -1;
+    }
+    if (descs[group_host[r]].cand_dim > ldx) {
+      set_error("score_groups: group %d has %d columns, the rows %d", group_host[r], descs[group_host[r]].cand_dim, ldx);
+      return -1;
+    }
+  }
+  if (m == 0) return 0;
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  DFB_TRY(ensure_train_scaled(h));
+  const int64_t npad = h->npad;
+  DFB_CUDA_OK(cudaMemcpyAsync(h->d_desc_grp, descs, sizeof(dfb_kernel_desc) * n_groups, cudaMemcpyHostToDevice,
+                              h->stream));
+  h->te_prepped = false;
+  for (int g = 0; g < n_groups; g++)
+    DFB_TRY(launch_prep_scaled(h, h->d_desc_grp + g, 1, h->X, h->n, h->d, h->te.xs + slot_off[g] * npad,
+                               h->te.nrm + fac_off[g] * npad, npad));
+
+  // rows in group order (stable), packed
+  std::vector<int64_t> order(m);
+  for (int64_t r = 0; r < m; r++) order[r] = r;
+  std::stable_sort(order.begin(), order.end(), [&](int64_t a, int64_t b) { return group_host[a] < group_host[b]; });
+  const bool small = small_eval_fits(h);
+  // a batch: as many whole passes as the staging buffer (chunk x DFB_MAX_SLOTS) and h->score (chunk) hold
+  const int64_t batch = std::min(h->chunk, h->chunk * DFB_MAX_SLOTS / ldx) / SMALL_EVAL_M * SMALL_EVAL_M;
+  std::vector<double> packed, sorted_scores(m);
+  for (int64_t b0 = 0; b0 < m; b0 += batch) {
+    const int64_t bm = std::min(batch, m - b0);
+    packed.clear();
+    std::vector<int64_t> col0(bm);                        // offset of each row's coordinates in `packed`
+    for (int64_t i = 0; i < bm; i++) {
+      const int64_t r = order[b0 + i];
+      const int dc = descs[group_host[r]].cand_dim;
+      col0[i] = (int64_t)packed.size();
+      packed.insert(packed.end(), X_host + r * ldx, X_host + r * ldx + dc);
+    }
+    DFB_CUDA_OK(cudaMemcpyAsync(h->stage, packed.data(), sizeof(double) * packed.size(), cudaMemcpyHostToDevice,
+                                h->stream));
+    for (int64_t p0 = 0; p0 < bm; p0 += SMALL_EVAL_M) {
+      const int64_t pm = std::min<int64_t>(SMALL_EVAL_M, bm - p0);
+      // segments [s0, s1) of one group within the pass
+      std::vector<int64_t> seg;
+      for (int64_t i = 0; i < pm; i++)
+        if (i == 0 || group_host[order[b0 + p0 + i]] != group_host[order[b0 + p0 + i - 1]]) seg.push_back(i);
+      seg.push_back(pm);
+      DFB_TRY(prof_begin(h, DFB_PROF_KSTAR));
+      for (size_t s = 0; s + 1 < seg.size(); s++) {
+        const int64_t s0 = seg[s], cnt = seg[s + 1] - s0;
+        const int g = group_host[order[b0 + p0 + s0]];
+        KstarArgs ka{};
+        ka.desc = &descs[g]; ka.d_desc = h->d_desc_grp + g;
+        ka.xsT = h->te.xs + slot_off[g] * npad; ka.nrmT = h->te.nrm + fac_off[g] * npad; ka.npad_tr = npad;
+        ka.alpha = h->alpha; ka.Xc = h->stage + col0[p0 + s0]; ka.m = cnt; ka.dc = descs[g].cand_dim;
+        ka.m_rows = (cnt + 1) / 2 * 2;                   // rows past cnt are overwritten by the next group's launch
+        ka.n_valid = h->n; ka.n_write = npad; ka.Ks = h->Ks + s0 * npad; ka.ldk = npad; ka.mean_const = 0.0;
+        ka.mu = h->mu + s0; ka.kss_out = h->kssv + s0; ka.cprep = h->cprep; ka.mu_part = h->mu_part;
+        DFB_TRY(launch_kstar(h, ka, route_kstar(h, ka, KstarWant::ROWS)));
+      }
+      DFB_TRY(prof_end(h, DFB_PROF_KSTAR, (double)pm));
+      DFB_TRY(prof_begin(h, DFB_PROF_GEMM));
+      int n_part = (int)(npad / TILE);
+      int64_t ld_part = h->chunk;
+      if (small) {
+        DFB_TRY(launch_small_sumsq(h, h->W, npad, h->Ks, npad, h->n, (int)pm, h->partial, SMALL_EVAL_M, &n_part));
+        ld_part = SMALL_EVAL_M;
+      } else {
+        DFB_TRY(contract_tiles_f64(h, round_up(pm, TILE)));
+      }
+      DFB_TRY(prof_end(h, DFB_PROF_GEMM, (double)pm));
+      DFB_TRY(prof_begin(h, DFB_PROF_ACQ));
+      for (size_t s = 0; s + 1 < seg.size(); s++) {
+        const int64_t s0 = seg[s], cnt = seg[s + 1] - s0;
+        dfb_acq_desc acq;
+        memset(&acq, 0, sizeof(acq));
+        acq.kind = DFB_ACQ_UCB;
+        acq.beta = betas[group_host[order[b0 + p0 + s0]]];
+        DFB_TRY(launch_acq(h, acq, h->mu + s0, h->partial + s0, ld_part, n_part, h->kssv + s0, cnt, 0, 1, nullptr,
+                           h->score + p0 + s0, false));
+      }
+      DFB_TRY(prof_end(h, DFB_PROF_ACQ, (double)pm));
+    }
+    DFB_CUDA_OK(cudaMemcpyAsync(sorted_scores.data() + b0, h->score, sizeof(double) * bm, cudaMemcpyDeviceToHost,
+                                h->stream));
+    DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  }
+  for (int64_t i = 0; i < m; i++) scores_host[order[i]] = sorted_scores[i];
   return 0;
 }
 

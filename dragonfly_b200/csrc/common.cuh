@@ -107,6 +107,7 @@ struct dfb_handle {
   dfb_kernel_desc* d_desc_tr = nullptr;
   dfb_kernel_desc* d_desc_te = nullptr;
   dfb_kernel_desc* d_desc_tmp = nullptr;
+  dfb_kernel_desc* d_desc_grp = nullptr;   // DFB_MAX_GROUPS descriptors of dfb_score_groups
 
   // optional Thompson-sampling workspace (api.cu: carve_ts())
   char* ts_ws = nullptr;

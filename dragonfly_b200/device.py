@@ -254,6 +254,23 @@ class DevicePosterior(object):
         'dfb_score_argmax_ts')
     return bs.value, bi.value, sc, nonpos.value
 
+  def score_groups(self, descs, betas, X, groups):
+    """ dfb_score_groups: Add-UCB's per-group objective of every row, mu + beta_g sd under row r's group descriptor
+        descs[groups[r]] (mean 0).  X: host (m, ldx) rows, group g's coordinates in its first descs[g].cand_dim
+        columns.  Returns the m scores (host ndarray). """
+    G = len(descs)
+    arr = (_lib.KernelDesc * G)(*descs)
+    b = np.ascontiguousarray(betas, dtype=np.float64)
+    X = np.ascontiguousarray(np.asarray(X, dtype=np.float64))
+    g = np.ascontiguousarray(groups, dtype=np.int32)
+    assert len(b) == G and X.ndim == 2 and len(g) == len(X)
+    out = np.empty((len(X),), dtype=np.float64)
+    _lib.check(self.lib.dfb_score_groups(self.h, arr, b.ctypes.data_as(C.POINTER(C.c_double)), G,
+                                         X.ctypes.data_as(C.c_void_p), int(X.shape[0]), int(X.shape[1]),
+                                         g.ctypes.data_as(C.POINTER(C.c_int32)),
+                                         out.ctypes.data_as(C.c_void_p)), 'dfb_score_groups')
+    return out
+
   # -- joint posterior over one block, or over all candidates: covariance and Thompson draws ---------
   TS_BLOCK = 4096
   # Above TS_BLOCK and up to TS_JOINT_MAX candidates, the covariance and the draws are formed over all candidates at

@@ -83,21 +83,29 @@ class PDOOSearch(object):
     return self.state.cache
 
   # -- objective values of a group of cells: value table first, the rest in batched calls ---------------------------------
-  def _eval_cells(self, cells, group=None):
+  def _fetch(self, cells, group=None):
+    """ The values of `cells`: yields the cells missing from the value table, `group` at a time (all at once when None),
+        receives their values and files them.  A non-deterministic objective gets every cell, every time. """
     if not self.deterministic:
-      pts = np.array([[(lo + hi) / 2.0 for (lo, hi) in c] for c in cells])
+      got = yield list(cells)
       self.num_device_calls += 1
-      return [float(v) for v in np.asarray(self.batch_obj(pts), dtype=np.float64).reshape(-1)]
+      return [float(v) for v in np.asarray(got, dtype=np.float64).reshape(-1)]
     miss = [c for c in dict.fromkeys(cells) if c not in self.values]
     step = len(miss) if not group else group
     for s0 in range(0, len(miss), max(step, 1)):
       part = miss[s0:s0 + step]
-      pts = np.array([[(lo + hi) / 2.0 for (lo, hi) in c] for c in part])
-      got = np.asarray(self.batch_obj(pts), dtype=np.float64).reshape(-1)
+      got = np.asarray((yield part), dtype=np.float64).reshape(-1)
       self.num_device_calls += 1
       for c, v in zip(part, got):
         self.values[c] = float(v)
     return [self.values[c] for c in cells]
+
+  def _score(self, cells):
+    """ batch_obj at the midpoints of the cells. """
+    return self.batch_obj(np.array([[(lo + hi) / 2.0 for (lo, hi) in c] for c in cells]))
+
+  def _eval_cells(self, cells, group=None):
+    return self._drive(self._fetch(cells, group), self._score)
 
   @staticmethod
   def _drive(gen, evaluate):
@@ -205,7 +213,7 @@ class PDOOSearch(object):
     while wants:
       cells = [c for i in sorted(wants) for c in wants[i]]
       before = len(self.values)
-      self._eval_cells(cells, group=self.PREFETCH_GROUP)
+      yield from self._fetch(cells, group=self.PREFETCH_GROUP)
       self.num_prefetched += len(self.values) - before
       nxt = {}
       for i in sorted(wants):
@@ -215,20 +223,62 @@ class PDOOSearch(object):
           pass
       wants = nxt
 
+  def _exact_pass(self, budget, rho):
+    """ One DOO pass on the shared state, its requests answered from the value table (misses fetched on demand). """
+    gen = self._doo_pass(self.state, budget, self.nu_max, rho)
+    try:
+      need = next(gen)
+      while True:
+        need = gen.send((yield from self._fetch(need)))
+    except StopIteration as stop:
+      return stop.value
+
   # -- the sweep over rho (doo.py:232-251) ------------------------------------------------------------------------------
-  def run(self, mult=0.5):
+  def steps(self, mult=0.5):
+    """ The whole search as a generator: yields lists of cells whose objective values it needs (never more than
+        PREFETCH_GROUP in the prefetch), receives their values, and returns (passes, index of the chosen pass). """
     Dm = int(np.log(self.K) / np.log(1 / self.rho_max))
     n = self.total_budget / 1.0
     N = int(mult * Dm * np.log(n / np.log(n)))
     budget = self.total_budget / float(N)
     rhos = [(self.rho_max) ** (float(N) / (N - i)) for i in range(N)]
     if self.prefetch and N > 1:
-      self._prefetch_all(budget, rhos)
+      yield from self._prefetch_all(budget, rhos)
     passes = []
     for rho in rhos:
-      passes.append(self._drive(self._doo_pass(self.state, budget, self.nu_max, rho), self._eval_cells))
+      passes.append((yield from self._exact_pass(budget, rho)))
     adjusted = [p[0] - self.state.C * (1 - p[1]) for p in passes]
     return passes, int(np.argmax(adjusted))
+
+  def run(self, mult=0.5):
+    return self._drive(self.steps(mult), self._score)
+
+
+def run_lockstep(searches, score, mult=0.5):
+  """ Runs several searches together: every round, the cells that all unfinished searches request go to ONE call
+      score([(i, cells_i), ...]) -> [values_i, ...] (i = the search's index, in increasing order).  Each search sees only
+      its own values, so it visits the cells it visits when run alone, in the same order, and returns the same result.
+      Returns ([search.run()'s result per search], the number of rounds). """
+  gens = [s.steps(mult) for s in searches]
+  results, wants = [None] * len(gens), {}
+  for i, gen in enumerate(gens):
+    try:
+      wants[i] = next(gen)
+    except StopIteration as stop:
+      results[i] = stop.value
+  rounds = 0
+  while wants:
+    order = sorted(wants)
+    got = score([(i, wants[i]) for i in order])
+    rounds += 1
+    nxt = {}
+    for i, vals in zip(order, got):
+      try:
+        nxt[i] = gens[i].send(vals)
+      except StopIteration as stop:
+        results[i] = stop.value
+    wants = nxt
+  return results, rounds
 
 
 def pdoo_maximise(obj, bounds, max_evals, vectorised=True, deterministic=True):
@@ -252,3 +302,27 @@ def pdoo_maximise(obj, bounds, max_evals, vectorised=True, deterministic=True):
 
 
 pdoo_maximise.last_search = None
+
+
+def pdoo_maximise_lockstep(score, list_of_bounds, max_evals):
+  """ pdoo_maximise over each of several boxes with the same budget, the searches run in lock-step (run_lockstep):
+      score([(i, X_i), ...]) -> [values_i, ...] gets, per round, the points X_i in box i's ORIGINAL coordinates that
+      search i needs.  Returns [(max_val, max_pt) per box]; pdoo_maximise_lockstep.last_searches and .last_rounds keep the
+      searches (query sequences) and the number of score calls. """
+  boxes = [np.array(b, dtype=np.float64) for b in list_of_bounds]
+  searches = [PDOOSearch(None, len(b), float(max_evals), nu_max=1.0, rho_max=0.9, K=2, C_init=0.8, tol=1e-3)
+              for b in boxes]
+
+  def score_cells(requests):
+    pts = [(i, np.array([[(lo + hi) / 2.0 for (lo, hi) in c] for c in cells]) * (boxes[i][:, 1] - boxes[i][:, 0])
+            + boxes[i][:, 0]) for i, cells in requests]
+    return score(pts)
+  results, rounds = run_lockstep(searches, score_cells, 0.5)
+  pdoo_maximise_lockstep.last_searches, pdoo_maximise_lockstep.last_rounds = searches, rounds
+  out = []
+  for b, (passes, index) in zip(boxes, results):
+    out.append((passes[index][0], passes[index][2] * (b[:, 1] - b[:, 0]) + b[:, 0]))
+  return out
+
+
+pdoo_maximise_lockstep.last_searches, pdoo_maximise_lockstep.last_rounds = None, 0

@@ -560,14 +560,20 @@ def _reference_fortran_direct_available():
   return getattr(ref_oper, 'direct_ft_wrap', None) is not None
 
 
+def _uses_device_pdoo(anc_data):
+  """ True when maximise_acquisition ends in PDOO: 'pdoo', or 'direct' without the reference's Fortran DIRECT
+      (oper_utils.py:121-137). """
+  method = str(anc_data.acq_opt_method).lower()
+  return method.startswith('pdoo') or (method.startswith('direct') and not _reference_fortran_direct_available())
+
+
 def _delegate_to_reference_maximiser(acq_fn, anc_data, deterministic=True):
   """ The non-vectorised maximisers of maximise_acquisition (:29-37).  `acq_fn` takes a (k, d) array.
       'pdoo' -- and 'direct' wherever the reference itself would fall back to PDOO because its Fortran DIRECT is
       not built (oper_utils.py:121-137) -- run the batched PDOO of dragonfly_b200/doo.py: the same search as
       dragonfly/utils/doo.py with the two children of every split scored in one device call.  Fortran DIRECT
       itself stays the reference's (a sequential host code driving the device-backed objective point by point). """
-  method = str(anc_data.acq_opt_method).lower()
-  if method.startswith('pdoo') or (method.startswith('direct') and not _reference_fortran_direct_available()):
+  if _uses_device_pdoo(anc_data):
     from .doo import pdoo_maximise
     if deterministic:
       _, opt_pt, _ = pdoo_maximise(lambda X: acq_fn(np.asarray(X, dtype=np.float64)), anc_data.domain.bounds,
@@ -753,24 +759,88 @@ def _get_add_ucb_beta_th(dim, time_step):
   return np.sqrt(0.2 * dim * np.log(2 * dim * time_step + 1))
 
 
-def _add_ucb_groups(anc_data, groupings, maximise_group):
+def _add_ucb_groups(anc_data, groupings, maximise_group, score_groups):
   """ The group loop of Add-UCB (:139-189, :334-388): group j's UCB, with the beta of its d_j coordinates, is maximised
-      over the d_j-dimensional sub-box with max_evals // (number of groups) candidates by
-      maximise_group(j, acq_desc, anc_data_j) -> point_j, and the group points are put back into one point. """
-  if not _check_rand_euclidean(anc_data):
-    raise NotImplementedError("Add-UCB on device needs acq_opt_method == 'rand'.")
+      over the d_j-dimensional sub-box with max_evals // (number of groups) evaluations, and the group points are put back
+      into one point.  'rand': maximise_group(j, acq_desc, anc_data_j) -> point_j, group by group.  PDOO: one search per
+      group, all driven in lock-step so that each round's points of every group are scored in one
+      score_groups([(j, X_j), ...], betas) -> [values_j, ...] call.  Other methods (Fortran DIRECT): the reference's
+      maximiser per group on the one-point objective score_groups([(j, x)], betas). """
+  rand = _check_rand_euclidean(anc_data)
   domain_bounds = np.asarray(anc_data.domain_bounds)
-  group_points = []
-  for j, group_j in enumerate(groupings):
+  betas = [_get_add_ucb_beta_th(len(group_j), anc_data.t) for group_j in groupings]
+  anc_datas = []
+  for group_j in groupings:
     anc_data_j = copy(anc_data)
     anc_data_j.max_evals = anc_data.max_evals // len(groupings)
     anc_data_j.domain = EuclideanDomain(domain_bounds[group_j])
-    acq = make_acq_desc('ucb', beta=_get_add_ucb_beta_th(len(group_j), anc_data.t))
-    group_points.append(maximise_group(j, acq, anc_data_j))
+    anc_datas.append(anc_data_j)
+  if rand:
+    group_points = [maximise_group(j, make_acq_desc('ucb', beta=betas[j]), anc_data_j)
+                    for j, anc_data_j in enumerate(anc_datas)]
+  elif _uses_device_pdoo(anc_data):
+    from .doo import pdoo_maximise_lockstep
+    found = pdoo_maximise_lockstep(lambda requests: score_groups(requests, betas),
+                                   [domain_bounds[group_j] for group_j in groupings], anc_datas[0].max_evals)
+    group_points = [pt for _, pt in found]
+  else:
+    group_points = [_delegate_to_reference_maximiser(
+        lambda X, j=j: score_groups([(j, np.asarray(X, dtype=np.float64))], betas)[0], anc_data_j)
+                    for j, anc_data_j in enumerate(anc_datas)]
   ret = np.zeros((sum(len(point_j) for point_j in group_points),))
   for point_j, group_j in zip(group_points, groupings):
     ret[group_j] = point_j
   return ret
+
+
+def _group_calls(descs, groups):
+  """ The groups of one round split into dfb_score_groups calls, in order: each call holds at most DFB_MAX_GROUPS
+      groups whose descriptors together use at most DFB_MAX_SLOTS slots and DFB_MAX_FACTORS factors. """
+  from . import _lib
+  calls, cur, slots, factors = [], [], 0, 0
+  for j in groups:
+    s, f = int(descs[j].n_slots), int(descs[j].n_factors)
+    if cur and (len(cur) == _lib.DFB_MAX_GROUPS or slots + s > _lib.DFB_MAX_SLOTS or
+                factors + f > _lib.DFB_MAX_FACTORS):
+      calls.append(cur)
+      cur, slots, factors = [], 0, 0
+    cur.append(j)
+    slots, factors = slots + s, factors + f
+  if cur:
+    calls.append(cur)
+  return calls
+
+
+def _group_scorer(post, descs, prefix=None):
+  """ score_groups of _add_ucb_groups on a device posterior: the rows of all requests -- each group's points, after
+      `prefix` (a fixed leading block of coordinates) when given -- in dfb_score_groups calls that pass only the groups
+      of the round (one call unless they exceed the entry's limits on groups, slots and factors, _group_calls). """
+  def score_one_call(requests, betas):
+    rows = [np.asarray(X, dtype=np.float64).reshape(len(X), -1) for _, X in requests]
+    if prefix is not None:
+      rows = [np.concatenate((np.repeat(prefix.reshape(1, -1), len(R), axis=0), R), axis=1) for R in rows]
+    present = list(dict.fromkeys(j for j, _ in requests))
+    local = {j: k for k, j in enumerate(present)}
+    X = np.zeros((sum(len(R) for R in rows), max(R.shape[1] for R in rows)))
+    groups = np.empty((len(X),), dtype=np.int32)
+    r0, bounds = 0, []
+    for (j, _), R in zip(requests, rows):
+      X[r0:r0 + len(R), :R.shape[1]] = R
+      groups[r0:r0 + len(R)] = local[j]
+      bounds.append((r0, r0 + len(R)))
+      r0 += len(R)
+    scores = post.score_groups([descs[j] for j in present], [betas[j] for j in present], X, groups)
+    return [scores[a:b] for a, b in bounds]
+
+  def score_groups(requests, betas):
+    out = {}
+    for call in _group_calls(descs, list(dict.fromkeys(j for j, _ in requests))):
+      members = set(call)
+      part = [(k, r) for k, r in enumerate(requests) if r[0] in members]
+      for (k, _), vals in zip(part, score_one_call([r for _, r in part], betas)):
+        out[k] = vals
+    return [out[k] for k in range(len(requests))]
+  return score_groups
 
 
 def _add_ucb(gp, add_kernel, mean_funcs, anc_data):
@@ -781,12 +851,14 @@ def _add_ucb(gp, add_kernel, mean_funcs, anc_data):
                               '(asy_add_ucb passes None).')
   groupings = add_kernel.groupings
   train_dim = gp._train_matrix().shape[1]
+  descs = [gp._group_test_descriptor(add_kernel, add_kernel.kernel_list[j], groupings[j], train_dim)
+           for j in range(len(groupings))]
 
   def maximise_group(j, acq, anc_data_j):
-    desc_j = gp._group_test_descriptor(add_kernel, add_kernel.kernel_list[j], groupings[j], train_dim)
-    return _fused_maximise(None, anc_data_j, session=lambda: gp._fused_session(acq, [], test_desc=desc_j,
+    return _fused_maximise(None, anc_data_j, session=lambda: gp._fused_session(acq, [], test_desc=descs[j],
                                                                                mean_const=0.0))
-  return _add_ucb_groups(anc_data, groupings, maximise_group)
+
+  return _add_ucb_groups(anc_data, groupings, maximise_group, _group_scorer(gp._device_posterior(), descs))
 
 
 def asy_add_ucb(gp, anc_data):
@@ -992,21 +1064,24 @@ def _add_ucb_for_boca(mfgp, fidel_to_opt, mean_funcs, anc_data):
   f2o = np.asarray(fidel_to_opt, dtype=np.float64).reshape(-1)
   dz = len(f2o)
   train_dim = mfgp._train_matrix().shape[1]
-
-  def maximise_group(j, acq, anc_data_j):
-    group_j = groupings[j]
+  descs = []
+  for j, group_j in enumerate(groupings):
     d_j = len(group_j)
     prod_j = CoordinateProductKernel(dz + d_j, kern_scale, [mfgp.fidel_kernel, mfgp.domain_kernel.kernel_list[j]],
                                      [list(range(dz)), list(range(dz, dz + d_j))])
     train_coords = [mfgp.fidel_coords[i] for i in range(dz)] + \
                    [mfgp.domain_coords[int(g)] for g in group_j]
-    desc_j = build_descriptor(prod_j, train_dim=train_dim, cand_dim=dz + d_j,
-                              train_coords=train_coords, cand_coords=list(range(dz + d_j)))
+    descs.append(build_descriptor(prod_j, train_dim=train_dim, cand_dim=dz + d_j,
+                                  train_coords=train_coords, cand_coords=list(range(dz + d_j))))
+
+  def maximise_group(j, acq, anc_data_j):
     def scorer(pts):
       zx = np.concatenate((np.repeat(f2o.reshape(1, -1), len(pts), axis=0), pts), axis=1)
-      return mfgp._fused_score(acq, zx, [], test_desc=desc_j, mean_const=0.0)
+      return mfgp._fused_score(acq, zx, [], test_desc=descs[j], mean_const=0.0)
     return _fused_maximise(scorer, anc_data_j)
-  return _add_ucb_groups(anc_data, groupings, maximise_group)
+
+  return _add_ucb_groups(anc_data, groupings, maximise_group,
+                         _group_scorer(mfgp._device_posterior(), descs, prefix=f2o))
 
 
 def asy_add_ucb_for_boca(mfgp, fidel_to_opt, anc_data):

@@ -295,6 +295,23 @@ int dfb_score_argmax(dfb_handle* h, const dfb_acq_desc* acq, const double* Xc, i
                      int32_t dc, int32_t space, double mean_const, double* scores,
                      double* best_score_host, int64_t* best_index_host);
 
+/* Add-UCB's per-group objectives (_add_ucb, gpb_acquisitions.py:139-189) for the rows of several groups in one call,
+ * as the sequential maximisers evaluate them (one point at a time, mean 0):
+ *     score_r = fl(mu_r + fl(betas[g] * sd_r)),  g = group_host[r],
+ * where (mu_r, sd_r) is what dfb_eval returns for row r alone, mean_const 0, with descs[g] bound by
+ * dfb_set_test_kernel and option "score_impl" 0 or 2 (dfb_eval in fp64).  The contraction here is always fp64: with
+ * "score_impl" 1, dfb_eval's int8 sigma may differ from it within its error bound.  Row r holds group g's
+ * descs[g].cand_dim coordinates in the first columns of a host row-major matrix with ldx columns,
+ * 1 <= ldx <= DFB_MAX_SLOTS.  Each group's K_* rows come from the K_* producer dfb_eval picks for its descriptor;
+ * then up to 32 rows, of any groups, share one row-streaming contraction over W (the tile contraction when the workspace
+ * cannot hold the streaming partials, as in dfb_eval), so m rows take ceil(m / 32) such passes.  A row's score does
+ * not depend on the other rows of the call.  At most DFB_MAX_GROUPS groups, whose descriptors together use at most
+ * DFB_MAX_SLOTS slots and DFB_MAX_FACTORS factors.  A test kernel bound with dfb_set_test_kernel stays bound.  Host
+ * memory in and out; scores_host holds m values.  */
+#define DFB_MAX_GROUPS 48
+int dfb_score_groups(dfb_handle* h, const dfb_kernel_desc* descs, const double* betas, int32_t n_groups,
+                     const double* X_host, int64_t m, int32_t ldx, const int32_t* group_host, double* scores_host);
+
 /* Thompson sampling on Cartesian-product domains (asy_ts, gpb_acquisitions.py:119-127, with the `rand` maximiser of
  * _rand_maximise_vectorised_objective_in_cp_domain, exd_utils.py:247-274): the reference calls gp.draw_samples(1, [x])
  * (gp_core.py:250-254; draw_gaussian_samples, general_utils.py:224-232) once per candidate -- a 1 x 1 covariance, its
