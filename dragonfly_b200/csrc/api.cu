@@ -29,6 +29,7 @@ static int64_t default_chunk(int64_t npad) {
 }
 
 constexpr int PRUNE_MAX_DC = 8;       // candidate columns the survivor list of the bound pass holds
+constexpr int PRUNE_SEED_MAX = 4096;  // largest option prune_seed_rows
 
 struct Carver {
   char* base;
@@ -90,6 +91,14 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
   // one screen launch covers a host staging batch (up to chunk x DFB_MAX_SLOTS rows) or ~10^6 device rows
   const int64_t keep_cap = round_up(chunk * DFB_MAX_SLOTS > ((int64_t)1 << 20) ? chunk * DFB_MAX_SLOTS : (int64_t)1 << 20, 32);
   uint32_t* keep_words = c.take<uint32_t>((size_t)keep_cap / 32);
+  double* prune_ub = c.take<double>((size_t)keep_cap);
+  uint32_t* seed_words = c.take<uint32_t>((size_t)keep_cap / 32);
+  uint32_t* seed_hist = c.take<uint32_t>((size_t)2 << 16);
+  uint64_t* seed_sel = c.take<uint64_t>(4);
+  const int64_t seed_cap = 2 * PRUNE_SEED_MAX;
+  int64_t* seed_idx = c.take<int64_t>((size_t)seed_cap);
+  double* seed_X = c.take<double>((size_t)seed_cap * PRUNE_MAX_DC);
+  int* seed_count = c.take<int>(4);
   double* best_score = c.take<double>(1);
   int64_t* best_index = c.take<int64_t>(1);
   double* red = c.take<double>(8);
@@ -115,6 +124,8 @@ static size_t carve(dfb_handle* h, char* base, int64_t n_max, int64_t chunk) {
     h->blk_score = blk_score; h->blk_index = blk_index; h->best_score = best_score;
     h->surv_cap = surv_cap; h->surv_idx = surv_idx; h->surv_X = surv_X; h->surv_count = surv_count;
     h->keep_words = keep_words; h->keep_cap = keep_cap;
+    h->prune_ub = prune_ub; h->seed_words = seed_words; h->seed_hist = seed_hist; h->seed_sel = seed_sel;
+    h->seed_cap = seed_cap; h->seed_idx = seed_idx; h->seed_X = seed_X; h->seed_count = seed_count;
     h->best_index = best_index; h->red = red; h->info = info;
     h->d_desc_tr = d0; h->d_desc_te = d1; h->d_desc_tmp = d2; h->d_desc_grp = d_grp;
     h->n_max = n_max; h->npad_max = npad; h->chunk = chunk;
@@ -857,12 +868,24 @@ static int run_chunks(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, 
   return 0;
 }
 
+// The seeds of the bound pass (run_chunks_pruned): md, the int8 pass's mode; rows below split (chunk 0) are not counted
+// by last_survivors / last_pruned_candidates.  run_bound_pass fills in the seed counts.
+struct SeedStage {
+  const ChunkMode* md;
+  int64_t split;
+  int seeds = 0, seeds_head = 0;
+};
+
 // The bound pass of dfb_score_argmax (see bound_pass_applies): no K_* rows, no contraction, but one screen per step of
 // keep_cap device rows or one staging batch of host rows, which appends the candidates whose acquisition bound reaches
 // best_lb - pad to the survivor list (global index idx_base + row).  With mu_out it writes mu_bar there instead, a chunk
 // per step (dfb_mu_upper_bound).  Void once *abort_count (the seed's shortlist; may be NULL) has overflowed.
+// With seeds, the first step stores every row's bound instead, contracts the rows with the largest bounds (option
+// prune_seed_rows; this resets best, best_lb and the shortlist) and then screens the other rows of the step against
+// the seeds' best_lb -- all before the step's staging buffer may be refilled.
 static int run_bound_pass(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc, int32_t space,
-                          double mean_const, double pad, int64_t idx_base, const int* abort_count, double* mu_out) {
+                          double mean_const, double pad, int64_t idx_base, const int* abort_count, double* mu_out,
+                          SeedStage* seeds = nullptr) {
   const ActiveKernel k = active_kernel(h);
   DFB_TRY(prepare_candidates(h, k, dc, space));
   CandidateStage st;
@@ -873,6 +896,26 @@ static int run_bound_pass(dfb_handle* h, const dfb_acq_desc& acq, const double* 
     const double* xc_dev;
     DFB_TRY(st.rows(c0, &xc_dev));
     double* mu_dev = mu_out == nullptr ? nullptr : space == DFB_DEVICE ? mu_out + c0 : h->mu;
+    if (seeds != nullptr && c0 == 0) {
+      DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
+      DFB_TRY(launch_prune(h, acq, k.desc, k.d_desc, k.ss.xs, xc_dev, mc, dc, mean_const, pad, idx_base, nullptr,
+                           nullptr, h->prune_ub));
+      DFB_TRY(launch_seed_select(h, mc, h->prune_seed_rows, idx_base, xc_dev, dc, seeds->split));
+      DFB_TRY(prof_end(h, DFB_PROF_PRUNE, (double)mc));
+      int cnt[2] = {0, 0};
+      DFB_CUDA_OK(cudaMemcpyAsync(cnt, h->seed_count, sizeof(cnt), cudaMemcpyDeviceToHost, h->stream));
+      DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+      seeds->seeds = cnt[0]; seeds->seeds_head = cnt[1];
+      ChunkMode sm = *seeds->md;
+      sm.idx_map = h->seed_idx;
+      const ChunkOut none = {nullptr, nullptr, nullptr};
+      DFB_TRY(run_chunks(h, acq, h->seed_X, cnt[0], dc, DFB_DEVICE, mean_const, none, sm));
+      DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
+      DFB_TRY(launch_ub_screen(h, mc, pad, idx_base, xc_dev, dc, seeds->split, abort_count));
+      DFB_TRY(prof_end(h, DFB_PROF_PRUNE, 0.0));
+      DFB_TRY(st.done(c0, mc));
+      continue;
+    }
     DFB_TRY(prof_begin(h, DFB_PROF_PRUNE));
     DFB_TRY(launch_prune(h, acq, k.desc, k.d_desc, k.ss.xs, xc_dev, mc, dc, mean_const, pad, idx_base + c0, abort_count,
                          mu_dev));
@@ -1480,12 +1523,15 @@ int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host) {
 // arg-max over it -- index and score -- is the one the full pass returns, bit for bit.
 // (3) No dropped candidate can be a NaN winner (a negative fp64 variance gives a NaN score, and np.argmax takes the
 //     first NaN): see bound_pass_applies.
-// Order: (a) chunk 0 scored as today (collect mode) seeds best, best_lb and the shortlist; (b) the bound pass over
-// rows chunk.. (run_bound_pass: one screen + gather per step) fills the survivor list; (c) one read-back of the
-// survivor count; (d) the survivors are scored like any
-// other chunk (collect mode, indices mapped back), continuing the arg-max of (a); the caller then re-scores the
-// shortlist in fp64 and runs the self-check unchanged.  A survivor list that overflows (4 chunks) voids the screen:
-// chunks 1.. are then scored as today, still continuing the seed's state.
+// Any seed set works: best_lb comes from contracted candidates only, and every other candidate is screened against it.
+// Order (run_bound_pass with a SeedStage): (a) the first step's rows (up to keep_cap device rows or one staging batch,
+// chunk 0 included) get their bound ub stored; (b) the rows with the K largest ub (option prune_seed_rows) are
+// selected and gathered, one read-back of their count; (c) the seeds are scored (collect mode, indices mapped back),
+// which seeds best, best_lb and the shortlist; (d) the first step's other rows are screened against best_lb - pad from
+// the stored ub; (e) later steps run the usual screen; then one read-back of the survivor count, and (f) the survivors
+// are scored like any other chunk, continuing the arg-max of (c); the caller then re-scores the shortlist in fp64 and
+// runs the self-check unchanged.  A survivor list that overflows (4 chunks) voids the screen: every candidate is then
+// scored afresh, as with option prune 0.
 static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, int64_t m,
                                int32_t dc, double b2) {
   if (!h->prune || h->have_test_kernel || m <= h->chunk || dc > PRUNE_MAX_DC || !kstar_plain(desc)) return false;
@@ -1503,29 +1549,34 @@ static bool bound_pass_applies(const dfb_handle* h, const dfb_acq_desc& acq, con
   return floor > b2 && floor > (double)h->n * DBL_EPSILON * kss;
 }
 
+// last_survivors and last_pruned_candidates count rows chunk.. only: each is contracted (a seed or a survivor) or pruned.
 static int run_chunks_pruned(dfb_handle* h, const dfb_acq_desc& acq, const double* Xc, int64_t m, int32_t dc,
                              int32_t space, double mean_const, const ChunkMode& md) {
   const int64_t Mc = h->chunk;
   const ChunkOut none = {nullptr, nullptr, nullptr};
-  const double* rest = Xc + Mc * dc;
-  DFB_TRY(run_chunks(h, acq, Xc, Mc, dc, space, mean_const, none, md));                 // (a)
-  DFB_CUDA_OK(cudaMemsetAsync(h->surv_count, 0, sizeof(int), h->stream));
-  DFB_TRY(run_bound_pass(h, acq, rest, m - Mc, dc, space, mean_const, md.pad, Mc, h->list_count, nullptr));  // (b)
-  int surv = 0;
-  DFB_CUDA_OK(cudaMemcpyAsync(&surv, h->surv_count, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));                                        // (c)
-  h->last_survivors = surv;
+  DFB_CUDA_OK(cudaMemsetAsync(h->surv_count, 0, sizeof(int) * 2, h->stream));
+  SeedStage seeds;
+  seeds.md = &md; seeds.split = Mc;
+  DFB_TRY(run_bound_pass(h, acq, Xc, m, dc, space, mean_const, md.pad, 0, h->list_count, nullptr, &seeds));  // (a)-(e)
+  int surv[2] = {0, 0};
+  DFB_CUDA_OK(cudaMemcpyAsync(surv, h->surv_count, sizeof(surv), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  h->last_seed_rows = seeds.seeds;
+  if (surv[0] > h->surv_cap) {                      // overflow: every candidate is contracted, the seeds' state reset
+    h->last_survivors = surv[0];
+    h->last_pruned = 0;
+    h->last_contracted = seeds.seeds + m;
+    DFB_CUDA_OK(cudaMemsetAsync(h->list_count, 0, sizeof(int) * 4, h->stream));
+    return run_chunks(h, acq, Xc, m, dc, space, mean_const, none, md);
+  }
+  h->last_survivors = (seeds.seeds - seeds.seeds_head) + (surv[0] - surv[1]);
+  h->last_pruned = m - Mc - h->last_survivors;
+  h->last_contracted = seeds.seeds + surv[0];
+  if (surv[0] == 0) return 0;
   ChunkMode cont = md;
   cont.keep_best = true;
-  if (surv > h->surv_cap) {                         // overflow: every candidate of chunks 1.. is contracted
-    h->last_pruned = 0;
-    cont.idx_base = Mc;
-    return run_chunks(h, acq, rest, m - Mc, dc, space, mean_const, none, cont);
-  }
-  h->last_pruned = m - Mc - surv;
-  if (surv == 0) return 0;
   cont.idx_map = h->surv_idx;
-  return run_chunks(h, acq, h->surv_X, surv, dc, DFB_DEVICE, mean_const, none, cont);   // (d)
+  return run_chunks(h, acq, h->surv_X, surv[0], dc, DFB_DEVICE, mean_const, none, cont);   // (f)
 }
 
 // The running arg-max (score, index) of the handle, read back
@@ -1562,6 +1613,8 @@ static int score_argmax_impl(dfb_handle* h, const dfb_acq_desc* acq, const doubl
   h->last_selfcheck_ratio = 0.0;
   h->last_survivors = 0;
   h->last_pruned = 0;
+  h->last_seed_rows = 0;
+  h->last_contracted = 0;
   bool need_exact_pass = !fast;
   if (fast) {
     // Pass 1: int8-slice scoring of everything, collecting the shortlist of candidates whose fp64 score could be
@@ -2080,6 +2133,8 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
   else if (strcmp(name, "Ks") == 0) { src = h->Ks; size = (int64_t)sizeof(double) * chunk * npad; }
   else if (strcmp(name, "partial") == 0) { src = h->partial; size = (int64_t)sizeof(double) * (npad / TILE) * chunk; }
   else if (strcmp(name, "kssv") == 0) { src = h->kssv; size = (int64_t)sizeof(double) * chunk; }
+  else if (strcmp(name, "prune_ub") == 0) { src = h->prune_ub; size = (int64_t)sizeof(double) * h->keep_cap; }
+  else if (strcmp(name, "seed_idx") == 0) { src = h->seed_idx; size = (int64_t)sizeof(int64_t) * h->seed_cap; }
   else if (strncmp(name, "ts_", 3) == 0) {
     if (h->ts_ws == nullptr) { set_error("debug_copy '%s': no Thompson-sampling workspace is set", name); return -1; }
     const int64_t mbp = h->ts_mb;
@@ -2114,6 +2169,10 @@ int dfb_query(dfb_handle* h, const char* name, double* out) {
   if (strcmp(name, "last_selfcheck_ratio") == 0) { *out = h->last_selfcheck_ratio; return 0; }
   if (strcmp(name, "last_survivors") == 0) { *out = (double)h->last_survivors; return 0; }
   if (strcmp(name, "last_pruned_candidates") == 0) { *out = (double)h->last_pruned; return 0; }
+  if (strcmp(name, "last_seed_rows") == 0) { *out = (double)h->last_seed_rows; return 0; }
+  if (strcmp(name, "last_contracted_rows") == 0) { *out = (double)h->last_contracted; return 0; }
+  if (strcmp(name, "keep_cap") == 0) { *out = (double)h->keep_cap; return 0; }
+  if (strcmp(name, "seed_cap") == 0) { *out = (double)h->seed_cap; return 0; }
   if (strcmp(name, "chunk") == 0) { *out = (double)h->chunk; return 0; }
   if (strcmp(name, "npad") == 0) { *out = (double)h->npad; return 0; }
   if (strcmp(name, "last_c2_group") == 0) { *out = (double)h->last_c2_group; return 0; }
@@ -2141,6 +2200,11 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value) {
   if (strcmp(name, "kstar_seg") == 0) { h->kstar_seg = value ? 1 : 0; return 0; }
   if (strcmp(name, "kstar_rows64") == 0) { h->kstar_rows64 = value ? 1 : 0; return 0; }
   if (strcmp(name, "prune") == 0) { h->prune = value ? 1 : 0; return 0; }
+  if (strcmp(name, "prune_seed_rows") == 0) {
+    if (value < 1 || value > PRUNE_SEED_MAX) { set_error("prune_seed_rows must be in 1..%d", PRUNE_SEED_MAX); return -1; }
+    h->prune_seed_rows = (int)value;
+    return 0;
+  }
   if (strcmp(name, "i8_unguarded") == 0) { h->i8_unguarded = value ? 1 : 0; return 0; }
   if (strcmp(name, "i8_radix") == 0) {
     if (value < -1 || value > 1) { set_error("i8_radix must be -1 (auto), 0 (radix 128) or 1 (radix 256)"); return -1; }

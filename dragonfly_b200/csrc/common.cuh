@@ -169,7 +169,17 @@ struct dfb_handle {
   int* surv_count = nullptr;      // [0] survivors wanted (> surv_cap = overflow)
   uint32_t* keep_words = nullptr; // keep_cap / 32 ballot words of one screen launch
   int64_t keep_cap = 0;           // rows one screen launch may cover
-  int64_t last_survivors = 0, last_pruned = 0;
+  // seeds of the bound pass: the first screen launch's rows with the largest bounds, contracted before the screen
+  int prune_seed_rows = 256;      // option "prune_seed_rows": K
+  double* prune_ub = nullptr;     // keep_cap bounds ub of the first screen launch
+  uint32_t* seed_words = nullptr; // keep_cap / 32 words: bit set = seed
+  uint32_t* seed_hist = nullptr;  // two 2^16-bin histograms of the bounds' key prefixes
+  uint64_t* seed_sel = nullptr;   // [4]: the selection's thresholds and counts (kernels.cu: seed_threshold_kernel)
+  int64_t seed_cap = 0;           // 2 x the largest K
+  int64_t* seed_idx = nullptr;    // seed_cap global indices
+  double* seed_X = nullptr;       // seed_cap x PRUNE_MAX_DC candidate rows
+  int* seed_count = nullptr;      // [0] seeds, [1] seeds below row chunk
+  int64_t last_survivors = 0, last_pruned = 0, last_seed_rows = 0, last_contracted = 0;
   int64_t last_selfcheck_violations = 0;
   double last_selfcheck_ratio = 0.0;   // max |s_int8 - s_fp64| / E_i over the last shortlist
   int64_t last_shortlist = 0;     // diagnostics: size of the last shortlist, -1 = overflow -> exact pass

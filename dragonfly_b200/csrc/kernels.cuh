@@ -83,10 +83,21 @@ int launch_collect_shortlist(dfb_handle* h, const double* score, const double* s
 // bound pass of dfb_score_argmax (plain kernels): keeps the m candidates Xc (device) whose acquisition at
 // (mu_bar, sqrt(k**)) reaches *best_lb - pad, mu_bar a certified upper bound of mu, and appends them (x rows, global
 // index idx_base + row) to the survivor list in row order; m <= h->keep_cap.  mu_ub non-NULL: writes mu_bar instead
-// (no screen).  No-op once *abort_count > SHORTLIST_CAP (abort_count may be NULL).
+// (no screen).  ub_out non-NULL: writes the bound ub = acq(mu_bar, sqrt(k**)) of every row there instead (+inf for a PI
+// row without one), the input of launch_seed_select and launch_ub_screen (ub_out = h->prune_ub).  No-op once
+// *abort_count > SHORTLIST_CAP (abort_count may be NULL).
 int launch_prune(dfb_handle* h, const dfb_acq_desc& acq, const dfb_kernel_desc& desc, const dfb_kernel_desc* d_desc,
                  const double* xsT, const double* Xc, int64_t m, int dc, double mean_const, double pad, int64_t idx_base,
-                 const int* abort_count, double* mu_ub);
+                 const int* abort_count, double* mu_ub, double* ub_out = nullptr);
+// Seeds of the bound pass: of the m rows' bounds in h->prune_ub, the K largest (kernels.cu: seed_key for the order;
+// between K and 2K rows, exact ties at the threshold in row order), gathered in row order -- x rows of Xc (device, dc
+// columns) into h->seed_X, global index idx_base + row into h->seed_idx -- and marked in h->seed_words.
+// h->seed_count[0] = seeds, [1] = seeds whose row is below split.  m <= h->keep_cap, 2K <= h->seed_cap.
+int launch_seed_select(dfb_handle* h, int64_t m, int64_t K, int64_t idx_base, const double* Xc, int dc, int64_t split);
+// The screen of the same m rows against *best_lb - pad, seeds excluded: the rows kept are appended to the survivor
+// list like launch_prune's; h->surv_count[1] gains those below row split.
+int launch_ub_screen(dfb_handle* h, int64_t m, double pad, int64_t idx_base, const double* Xc, int dc, int64_t split,
+                     const int* abort_count);
 // largest relative error of ex2.approx.ftz.f32 (which = 0) or rsqrt.approx.ftz.f32 (1) over the inputs the bound pass
 // gives them, as the bit pattern of a double in *out_bits (device)
 int launch_approx_err(dfb_handle* h, int which, unsigned long long* out_bits);

@@ -464,7 +464,10 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
  * doubles), "Ki8" (the three K_* digit planes of the chunk buffer, 6 chunk npad bytes), "Ks" (fp64 K_* rows,
  * chunk x npad, written only when the digits are not emitted by the K_* kernel), "partial" ((npad / 128) x chunk),
  * "T" (the factorised tall matrix [L ; L^-T ; (L^-1 y_c)^T], (2 npad + 128) x npad: its padding, the y row), "alpha"
- * (npad doubles, padding included), "kssv" (k(x*, x*) of the last scored chunk, chunk doubles).  With a Thompson-
+ * (npad doubles, padding included), "kssv" (k(x*, x*) of the last scored chunk, chunk doubles), "prune_ub" (query
+ * "keep_cap" doubles: the bounds acq(mu_ub, sqrt(k**)) of the first screen launch of the last bound pass, one per row
+ * of its first step, +inf for a PI row without one), "seed_idx" (query "seed_cap" int64: the global indices of the
+ * last bound pass's seeds in row order, query "last_seed_rows" of them).  With a Thompson-
  * sampling workspace (dfb_set_ts_workspace; mbp = its mb rounded up to 128, and q = the last block's m rounded up to
  * 128, whose data sits at the start of each buffer with leading dimension q): "ts_Cov" (mbp^2 doubles: the padded
  * posterior covariance of the last dfb_eval_covar / dfb_ts_draws block, q x q; dfb_ts_draws writes its lower tiles
@@ -520,14 +523,20 @@ int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host);
  *                 tiles that share one load of the W digits, so an odd group is rounded up by one tile; query
  *                 "last_c2_group" gives the group in effect.
  *  "prune"      : 1 (default) = dfb_score_argmax's int8 path contracts only the candidates whose acquisition can reach
- *                 the arg-max.  After chunk 0 is scored, every further candidate gets a certified upper bound mu_ub of
- *                 its mean (single precision, dfb_mu_upper_bound) and is dropped when acq(mu_ub, sqrt(k(x*, x*))) -- an
- *                 upper bound of its score, sigma^2 <= k(x*, x*) -- lies below a certain lower bound of the fp64
- *                 maximum; the survivors are scored as usual.  Index and score are those of the full pass, bit for
- *                 bit.  Applies to EI, PI and UCB with beta >= 0, plain SE / Matern (p <= 2) kernels on <= 8 dims, no
+ *                 the arg-max.  Every candidate gets a certified upper bound mu_ub of its mean (single precision,
+ *                 dfb_mu_upper_bound) and so an upper bound ub = acq(mu_ub, sqrt(k(x*, x*))) of its score (sigma^2 <=
+ *                 k(x*, x*)).  The candidates with the largest ub (the seeds, option "prune_seed_rows") are scored
+ *                 first and give a certain lower bound of the fp64 maximum; every other candidate is dropped when its
+ *                 ub lies below it, and the survivors are scored as usual.  Index and score are those of the full
+ *                 pass, bit for bit.  Applies to EI, PI and UCB with beta >= 0, plain SE / Matern (p <= 2) kernels on <= 8 dims, no
  *                 test kernel, m > chunk, no score vector, and when the posterior's variance
  *                 floor k** s / (n k** + s) (s = noise + jitter) exceeds the int8 error bound.  0 = contract every
  *                 candidate.
+ *  "prune_seed_rows": K, 1..4096 (default 256): the seeds of option "prune" are the rows with the K largest bounds ub
+ *                 among the first screen launch's rows (up to 2^20 device rows, or one staging batch of host rows):
+ *                 every row above a threshold and the exact ties at it in row order, K to 2K rows in all (fewer when
+ *                 there are fewer rows).  Any seed set gives the same result; K only sets how many rows are
+ *                 contracted before the screen.
  *  "kstar_fast" : 1 (default) = plain SE / Matern kernels on <= 8 dims get specialised K_* kernels; 0 = they go through
  *                 the descriptor interpreter (kstar_kernel).  Which K_* kernel runs: kernels.cu, route_kstar.
  *  "tma_cb_group": scheduling knob of the fp64 TMA contraction. */
@@ -536,8 +545,11 @@ int dfb_set_option(dfb_handle* h, const char* name, int64_t value);
  * "last_used_i8", "last_shortlist" (-1 = overflow -> fp64 pass), "last_selfcheck_violations" (> 0: the int8 screen
  * was voided and the call redone in fp64), "last_selfcheck_ratio" (max |s_int8 - s_fp64| / allowance over the last
  * shortlist; the model's margin is its inverse), "chunk", "npad", "last_c2_group"; "i8_impl" is always 2 (bench.py
- * reports it); "last_survivors" (candidates the bound pass of option "prune" kept; > 4 chunks = overflow, the screen
- * was voided; 0 when it did not run), "last_pruned_candidates" (candidates contracted in no pass). */
+ * reports it); "last_survivors" (candidates of rows chunk.. that the bound pass of option "prune" contracted, as
+ * seeds or as survivors of the screen; > 4 chunks = overflow, the screen was voided; 0 when it did not run),
+ * "last_pruned_candidates" (candidates of rows chunk.. contracted in no pass; with "last_survivors" they add up to
+ * m - chunk), "last_seed_rows" (the bound pass's seeds, all rows), "last_contracted_rows" (rows of all m the bound
+ * pass's int8 scoring contracted: seeds + survivors; after an overflow, seeds + m), "keep_cap", "seed_cap". */
 int dfb_query(dfb_handle* h, const char* name, double* out);
 
 /* Per-kernel-class device timing with CUDA events on the handle's stream (bench.py's roofline):

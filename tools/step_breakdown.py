@@ -1,7 +1,8 @@
 """Wall-clock / device-time breakdown of one bench.py step (build + fused score of 10^6 candidates).
 
-The device line splits the score into the contracted chunks (kstar, gemm, acq: the seed chunk and the survivors of
-the bound pass) and the bound pass itself (a certified upper bound of mu and the screen, for every other candidate)."""
+The device line splits the score into the contracted rows (kstar, gemm, acq: the seeds and the survivors of the bound
+pass) and the bound pass itself (a certified upper bound of mu for every candidate, the seed selection and the
+screen)."""
 import os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -16,6 +17,15 @@ mean = gp_core.ConstantMean(w['mean_const'])
 acq = device.make_acq_desc('ei', best=float(w['Y'].max()))
 cd = torch.rand((n_cand, 6), dtype=torch.float64, device='cuda')
 sync = torch.cuda.synchronize
+
+
+def query(post, name):
+  try:
+    return int(post.query(name))
+  except Exception:           # an older library (DFB200_LIB) without this query
+    return -1
+
+
 for prof in (False, False, False, True):
   sync(); t0 = time.perf_counter()
   gp = gp_core.GP(w['X'], w['Y'], kern, mean, w['noise_var'], device=0)
@@ -26,13 +36,14 @@ for prof in (False, False, False, True):
   line = 'build %.2f ms  score %.2f ms  total %.2f ms' % (1e3 * (t1 - t0), 1e3 * (t2 - t1), 1e3 * (t2 - t0))
   if prof:
     r = [gp._post.profile_read(c) for c in (0, 1, 2, 4)]
-    # kstar / gemm / acq: the chunks that were contracted (the seed chunk and the survivors of the bound pass);
-    # bound: the upper bound of mu + screen over every other candidate
+    # kstar / gemm / acq: the rows that were contracted (the seeds and the survivors of the bound pass);
+    # bound: the upper bound of mu over every candidate, the seed selection and the screen
     line += ' | device: kstar %.2f (%d) gemm %.2f (%d, %d cand) acq %.2f (%d) bound %.2f (%d) sum %.2f' % (
         r[0][0], r[0][1], r[1][0], r[1][1], r[1][2], r[2][0], r[2][1], r[3][0], r[3][1], sum(x[0] for x in r))
-    line += ' | shortlist %d survivors %d pruned %d' % (int(gp._post.query('last_shortlist')),
-                                                        int(gp._post.query('last_survivors')),
-                                                        int(gp._post.query('last_pruned_candidates')))
+    q = lambda name: query(gp._post, name)
+    line += ' | shortlist %d seeds %d survivors %d pruned %d contracted %d' % (
+        q('last_shortlist'), q('last_seed_rows'), q('last_survivors'), q('last_pruned_candidates'),
+        q('last_contracted_rows'))
   print(line)
   del gp
 
