@@ -127,6 +127,7 @@ PROTOTYPES = {
   'dfb_debug_score_i8': (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _P, _D, _P, _P, _I64]),
   'dfb_debug_copy': (C.c_int, [_P, C.c_char_p, _P, _I64]),
   'dfb_debug_approx_error': (C.c_int, [_P, _I32, C.POINTER(_D)]),
+  'dfb_debug_chol_diag': (C.c_int, [_P, _I32, _P, _I64, _P, _P, C.POINTER(_I32)]),
   'dfb_set_option': (C.c_int, [_P, C.c_char_p, _I64]),
   'dfb_query': (C.c_int, [_P, C.c_char_p, C.POINTER(_D)]),
   'dfb_profile_enable': (C.c_int, [_P, C.c_int]),

@@ -1509,6 +1509,27 @@ int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host) {
   return 0;
 }
 
+int dfb_debug_chol_diag(dfb_handle* h, int32_t which, const double* blk_dev, int64_t ld, double* out_blk_dev,
+                        double* out_dinv_dev, int32_t* info_host) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if ((which != 0 && which != 1) || blk_dev == nullptr || out_blk_dev == nullptr || out_dinv_dev == nullptr ||
+      info_host == nullptr || ld < TILE) {
+    set_error("bad debug_chol_diag arguments");
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  int* info = reinterpret_cast<int*>(h->red);
+  DFB_CUDA_OK(cudaMemsetAsync(info, 0, sizeof(int), h->stream));
+  DFB_CUDA_OK(cudaMemcpy2DAsync(out_blk_dev, TILE * sizeof(double), blk_dev, (size_t)ld * sizeof(double),
+                                TILE * sizeof(double), TILE, cudaMemcpyDeviceToDevice, h->stream));
+  DFB_TRY(launch_chol_diag_debug(h, which, out_blk_dev, out_dinv_dev, info));
+  int v = 0;
+  DFB_CUDA_OK(cudaMemcpyAsync(&v, info, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  *info_host = v;
+  return 0;
+}
+
 // ---- bound pass of dfb_score_argmax ---------------------------------------------------------------------------------
 // Most candidates of a large random batch cannot reach the arg-max, and proving so needs an upper bound of mu alone:
 //   (1) ub = acq(mu_bar, sqrt(k**)) >= the fp64 score of the exact pass.  mu_bar (kernels.cu: prune_bound_kernel, in

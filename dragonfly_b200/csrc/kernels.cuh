@@ -42,6 +42,9 @@ int launch_kstar(dfb_handle* h, const KstarArgs& a, KstarRoute route);
 int launch_init_tall(dfb_handle* h, double* T, int64_t n, int64_t npad, double diag_add,
                      const double* yc, int with_bottom);
 int launch_chol_diag(dfb_handle* h, double* T, int64_t ld, int step, double* Dinv, int* info);
+// One 128 x 128 block (leading dimension 128) factorised in place by chol_diag_block (which = 0) or chol_diag_kernel (1);
+// *info (device) must be 0 and receives the 1-based index of the first failing pivot
+int launch_chol_diag_debug(dfb_handle* h, int which, double* blk, double* Dinv, int* info);
 int launch_transpose(dfb_handle* h, const double* src, double* dst, int64_t n);
 int launch_alpha(dfb_handle* h, const double* Wt, const double* v, double* alpha, int64_t n,
                  int64_t npad);

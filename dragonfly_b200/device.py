@@ -460,6 +460,20 @@ class DevicePosterior(object):
   def launch_count(self):
     return int(self.lib.dfb_launch_count(self.h))
 
+  def debug_chol_diag(self, which, blk):
+    """ dfb_debug_chol_diag (a test hook): factorise a copy of one 128 x 128 block (CUDA float64 tensor) with the
+    batched-LML elimination (which = 0) or the posterior build's diagonal-block kernel (1).  Returns (info, blk, Dinv);
+    the two outputs are filled with NaN beforehand, so on failure blk is the copy and Dinv untouched. """
+    assert blk.dtype == torch.float64 and blk.is_cuda and tuple(blk.shape) == (128, 128) and blk.stride(1) == 1
+    out = torch.full((128, 128), float('nan'), dtype=torch.float64, device=blk.device)
+    dinv = torch.full((128, 128), float('nan'), dtype=torch.float64, device=blk.device)
+    info = C.c_int32(0)
+    torch.cuda.synchronize(blk.device)
+    _lib.check(self.lib.dfb_debug_chol_diag(self.h, int(which), C.c_void_p(blk.data_ptr()), int(blk.stride(0)),
+                                            C.c_void_p(out.data_ptr()), C.c_void_p(dinv.data_ptr()), C.byref(info)),
+               'dfb_debug_chol_diag')
+    return info.value, out, dinv
+
   def set_option(self, name, value):
     _lib.check(self.lib.dfb_set_option(self.h, name.encode('utf-8'), int(value)), 'dfb_set_option')
 

@@ -482,6 +482,13 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
  * float in [-126, 0], or of rsqrt.approx.ftz.f32 (which = 1) over every float in [2^-120, 2^126), against fp64
  * references -- the inputs the bound pass of dfb_score_argmax gives them.  Synchronises. */
 int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host);
+/* Diagnostics (tests/test_gpu_chol_diag.py), not on the product path: copies the 128 x 128 block at blk_dev (leading
+ * dimension ld >= 128) to out_blk_dev (leading dimension 128) and factorises the copy in place with the diagonal-block
+ * elimination of the batched LML builds (which = 0) or with the posterior build's chol_diag_kernel (which = 1): L in
+ * the lower triangle, zeros above, d_j on the diagonal, L^-1 (lower) in out_dinv_dev (128 x 128).  *info_host: 0, or
+ * the 1-based index of the first pivot that is not > 0, in which case nothing but the copy is written.  Synchronises. */
+int dfb_debug_chol_diag(dfb_handle* h, int32_t which, const double* blk_dev, int64_t ld, double* out_blk_dev,
+                        double* out_dinv_dev, int32_t* info_host);
 
 /* Tuning switches.
  *  "gemm_impl"  : 0 = cp.async-ring DMMA kernel, 1 = TMA + mbarrier warp-specialised DMMA kernel for the
