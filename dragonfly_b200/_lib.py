@@ -128,6 +128,9 @@ PROTOTYPES = {
   'dfb_debug_copy': (C.c_int, [_P, C.c_char_p, _P, _I64]),
   'dfb_debug_approx_error': (C.c_int, [_P, _I32, C.POINTER(_D)]),
   'dfb_debug_chol_diag': (C.c_int, [_P, _I32, _P, _I64, _P, _P, C.POINTER(_I32)]),
+  'dfb_debug_acq': (C.c_int, [_P, C.POINTER(AcqDesc), _P, _P, _I64, _I32, _P, _I64, _P, C.c_uint64, _D, _D, _D, _D,
+                              _P, _P, C.POINTER(_D), C.POINTER(_I64), C.POINTER(_D), C.POINTER(_I32)]),
+  'dfb_debug_selfcheck': (C.c_int, [_P, _P, _P, _P, _I32, C.POINTER(_I32)]),
   'dfb_set_option': (C.c_int, [_P, C.c_char_p, _I64]),
   'dfb_query': (C.c_int, [_P, C.c_char_p, C.POINTER(_D)]),
   'dfb_profile_enable': (C.c_int, [_P, C.c_int]),

@@ -1530,6 +1530,73 @@ int dfb_debug_chol_diag(dfb_handle* h, int32_t which, const double* blk_dev, int
   return 0;
 }
 
+// The acquisition epilogue of run_chunks on caller vectors (tests/test_gpu_acq_exact.py): per chunk of the handle, the
+// acquisition with the block arg-max and the lower-bound tracking of an int8 pass, the merge into the running
+// (score, index, best_lb), then the shortlist of that chunk -- the launches and arguments of a collecting pass.
+static int read_best(dfb_handle* h, double* best_score_host, int64_t* best_index_host);
+// The sensitivity of the int8 pass's allowance (kernels.cu: i8_score_err): |beta| (UCB), sup phi = 1/sqrt(2 pi) < 0.4
+// (EI, TTEI), sup |z phi(z)| = phi(1) < 0.25 (PI); TS takes |z_i| per candidate inside the kernels.
+static double i8_score_sens(const dfb_acq_desc& acq) {
+  return (acq.kind == DFB_ACQ_UCB) ? fabs(acq.beta) : (acq.kind == DFB_ACQ_PI ? 0.25 : 0.4);
+}
+int dfb_debug_acq(dfb_handle* h, const dfb_acq_desc* acq, const double* mu_dev, const double* partial_dev,
+                  int64_t ld_partial, int32_t nrb, const double* kss_dev, int64_t m, const double* z_dev, uint64_t seed,
+                  double b2, double sens, double pad, double best_lb, double* sd_dev, double* scores_dev,
+                  double* best_score_host, int64_t* best_index_host, double* best_lb_host, int32_t* count_host) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if (acq == nullptr || acq->kind < DFB_ACQ_UCB || acq->kind > DFB_ACQ_TS_MARGINAL || mu_dev == nullptr ||
+      kss_dev == nullptr || sd_dev == nullptr || scores_dev == nullptr || m < 1 || nrb < 0 ||
+      (nrb > 0 && (partial_dev == nullptr || ld_partial < m)) || !(b2 >= 0.0) || best_score_host == nullptr ||
+      best_index_host == nullptr || best_lb_host == nullptr || count_host == nullptr) {
+    set_error("bad debug_acq arguments (m = %lld, nrb = %d)", (long long)m, nrb);
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  const bool ts = acq->kind == DFB_ACQ_TS_MARGINAL;
+  I8ErrModel em;
+  em.b2 = b2; em.sens = sens < 0.0 ? i8_score_sens(*acq) : sens; em.kind = acq->kind;
+  DFB_CUDA_OK(cudaMemsetAsync(h->list_count, 0, sizeof(int) * 4, h->stream));
+  DFB_TRY(launch_reset_best(h));
+  DFB_CUDA_OK(cudaMemcpyAsync(h->best_lb, &best_lb, sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  for (int64_t c0 = 0; c0 < m; c0 += h->chunk) {
+    const int64_t mc = std::min(m - c0, h->chunk);
+    TsZ tz;
+    memset(&tz, 0, sizeof(tz));
+    tz.z = z_dev != nullptr ? z_dev + c0 : nullptr;
+    tz.seed = seed;
+    tz.z_out = z_dev != nullptr ? nullptr : h->ts_z;
+    DFB_TRY(launch_acq(h, *acq, mu_dev + c0, nrb > 0 ? partial_dev + c0 : nullptr, ld_partial, nrb, kss_dev + c0, mc, c0,
+                       1, sd_dev + c0, scores_dev + c0, true, nullptr, &em, ts ? &tz : nullptr));
+    DFB_TRY(launch_collect_shortlist(h, scores_dev + c0, sd_dev + c0, mc, c0, nullptr, em, pad, nullptr, 0,
+                                     ts ? (tz.z != nullptr ? tz.z : h->ts_z) : nullptr));
+  }
+  int count = 0;
+  DFB_CUDA_OK(cudaMemcpyAsync(&count, h->list_count, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaMemcpyAsync(best_lb_host, h->best_lb, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  DFB_TRY(read_best(h, best_score_host, best_index_host));
+  *count_host = count;
+  return 0;
+}
+
+int dfb_debug_selfcheck(dfb_handle* h, const double* s8_dev, const double* err_dev, const double* s64_dev, int32_t count,
+                        int32_t* out_host) {
+  DFB_TRY(need(h, true, false, false, false, false));
+  if (s8_dev == nullptr || err_dev == nullptr || s64_dev == nullptr || count < 0 || out_host == nullptr) {
+    set_error("bad debug_selfcheck arguments");
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  int* out = reinterpret_cast<int*>(h->red);
+  DFB_CUDA_OK(cudaMemsetAsync(out, 0, sizeof(int) * 2, h->stream));
+  DFB_TRY(launch_selfcheck(h, s8_dev, err_dev, s64_dev, count, out));
+  int v[2] = {0, 0};
+  DFB_CUDA_OK(cudaMemcpyAsync(v, out, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
+  out_host[0] = v[0];
+  out_host[1] = v[1];
+  return 0;
+}
+
 // ---- bound pass of dfb_score_argmax ---------------------------------------------------------------------------------
 // Most candidates of a large random batch cannot reach the arg-max, and proving so needs an upper bound of mu alone:
 //   (1) ub = acq(mu_bar, sqrt(k**)) >= the fp64 score of the exact pass.  mu_bar (kernels.cu: prune_bound_kernel, in
@@ -1645,11 +1712,14 @@ static int score_argmax_impl(dfb_handle* h, const dfb_acq_desc* acq, const doubl
     double scale = sk;                    // natural score scale, for the slack only
     if (acq->kind == DFB_ACQ_UCB) scale = (1.0 + fabs(acq->beta)) * sk + fabs(mean_const);
     else if (acq->kind == DFB_ACQ_PI) scale = 1.0;
+    // EI ~ max(mu - best, 0) where the mean function lies far from the incumbent: one ulp of such a score would
+    // outgrow a pad of 1e-9 sqrt(k**) (tests/test_acq_ref.py: the bound pass's ub + pad >= score)
+    else if (acq->kind == DFB_ACQ_EI) scale = sk + fabs(mean_const) + fabs(acq->best);
     else if (ts) scale = 9.0 * sk + fabs(mean_const);     // UCB's with |z| <= 8 (Box-Muller's on 53-bit uniforms: 8.6)
     md.collect = true;
     md.em.b2 = i8_sigma2_bound(h, desc);
     md.em.kind = acq->kind;
-    md.em.sens = (acq->kind == DFB_ACQ_UCB) ? fabs(acq->beta) : (acq->kind == DFB_ACQ_PI ? 0.25 : 0.4);   // TS: |z_i|
+    md.em.sens = i8_score_sens(*acq);
     md.pad = 1e-9 * scale;
     DFB_CUDA_OK(cudaMemsetAsync(h->list_count, 0, sizeof(int) * 4, h->stream));
     if (scores == nullptr && bound_pass_applies(h, *acq, desc, m, dc, md.em.b2))
@@ -1674,7 +1744,7 @@ static int score_argmax_impl(dfb_handle* h, const dfb_acq_desc* acq, const doubl
       }
       ChunkOut none = {nullptr, nullptr, nullptr};
       DFB_TRY(run_chunks(h, *acq, h->list_X, count, dc, DFB_DEVICE, mean_const, none, ex));
-      DFB_TRY(launch_selfcheck(h, h->score, count));
+      DFB_TRY(launch_selfcheck(h, h->list_s8, h->list_err, h->score, count, h->list_count + 1));
       int chk[2] = {0, 0};
       DFB_CUDA_OK(cudaMemcpyAsync(chk, h->list_count + 1, sizeof(chk), cudaMemcpyDeviceToHost, h->stream));
       DFB_CUDA_OK(cudaStreamSynchronize(h->stream));
@@ -2156,6 +2226,9 @@ int dfb_debug_copy(dfb_handle* h, const char* name, void* dst_dev, int64_t bytes
   else if (strcmp(name, "kssv") == 0) { src = h->kssv; size = (int64_t)sizeof(double) * chunk; }
   else if (strcmp(name, "prune_ub") == 0) { src = h->prune_ub; size = (int64_t)sizeof(double) * h->keep_cap; }
   else if (strcmp(name, "seed_idx") == 0) { src = h->seed_idx; size = (int64_t)sizeof(int64_t) * h->seed_cap; }
+  else if (strcmp(name, "list_idx") == 0) { src = h->list_idx; size = (int64_t)sizeof(int64_t) * SHORTLIST_CAP; }
+  else if (strcmp(name, "list_s8") == 0) { src = h->list_s8; size = (int64_t)sizeof(double) * SHORTLIST_CAP; }
+  else if (strcmp(name, "list_err") == 0) { src = h->list_err; size = (int64_t)sizeof(double) * SHORTLIST_CAP; }
   else if (strncmp(name, "ts_", 3) == 0) {
     if (h->ts_ws == nullptr) { set_error("debug_copy '%s': no Thompson-sampling workspace is set", name); return -1; }
     const int64_t mbp = h->ts_mb;

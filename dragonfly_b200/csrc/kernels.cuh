@@ -104,7 +104,7 @@ int launch_ub_screen(dfb_handle* h, int64_t m, double pad, int64_t idx_base, con
 // largest relative error of ex2.approx.ftz.f32 (which = 0) or rsqrt.approx.ftz.f32 (1) over the inputs the bound pass
 // gives them, as the bit pattern of a double in *out_bits (device)
 int launch_approx_err(dfb_handle* h, int which, unsigned long long* out_bits);
-int launch_selfcheck(dfb_handle* h, const double* s64, int count);
+int launch_selfcheck(dfb_handle* h, const double* s8, const double* err, const double* s64, int count, int* out);
 int launch_vec_max(dfb_handle* h, const double* v, int64_t n, double* out);
 int launch_reset_best(dfb_handle* h);
 int launch_fill_rng(dfb_handle* h, uint64_t seed, int64_t col0, int S, int64_t m, int what, double* out);

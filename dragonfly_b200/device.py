@@ -4,6 +4,7 @@ torch-owned workspace it computes in.  PyTorch appears here only as the allocato
 and the owner of CUDA streams; every numeric result comes from libdfb200's CUDA kernels.
 """
 import ctypes as C
+import types
 import weakref
 
 import numpy as np
@@ -473,6 +474,51 @@ class DevicePosterior(object):
                                             C.c_void_p(out.data_ptr()), C.c_void_p(dinv.data_ptr()), C.byref(info)),
                'dfb_debug_chol_diag')
     return info.value, out, dinv
+
+  def debug_acq(self, acq_desc, mu, partial, kss, z=None, seed=0, b2=0.0, sens=-1.0, pad=0.0,
+                best_lb=float('-inf')):
+    """ dfb_debug_acq (a test hook): the acquisition, arg-max and shortlist launches of an int8 pass on CUDA float64
+    vectors mu (m), partial (nrb x m, or None) and kss (m); z (m) the normals of DFB_ACQ_TS_MARGINAL or None; sens < 0:
+    the allowance sensitivity dfb_score_argmax uses.  sd and
+    the scores are filled with NaN beforehand.  Returns a namespace of sd, scores, score, index, best_lb and count. """
+    m = int(mu.shape[0])
+    for t in (mu, kss) + ((z,) if z is not None else ()):
+      assert t.dtype == torch.float64 and t.is_cuda and t.is_contiguous() and int(t.shape[0]) == m
+    nrb, ld = 0, m
+    if partial is not None:
+      assert partial.dtype == torch.float64 and partial.is_cuda and partial.stride(1) == 1 and int(partial.shape[1]) == m
+      nrb, ld = int(partial.shape[0]), int(partial.stride(0))
+    sd = torch.full((m,), float('nan'), dtype=torch.float64, device=mu.device)
+    scores = torch.full((m,), float('nan'), dtype=torch.float64, device=mu.device)
+    bs, bi, bl, cnt = C.c_double(0.0), C.c_int64(-1), C.c_double(0.0), C.c_int32(0)
+    torch.cuda.synchronize(mu.device)
+    _lib.check(self.lib.dfb_debug_acq(
+        self.h, C.byref(acq_desc), C.c_void_p(mu.data_ptr()), C.c_void_p(partial.data_ptr() if nrb else 0), ld, nrb,
+        C.c_void_p(kss.data_ptr()), m, C.c_void_p(z.data_ptr() if z is not None else 0),
+        C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), float(b2), float(sens), float(pad), float(best_lb),
+        C.c_void_p(sd.data_ptr()), C.c_void_p(scores.data_ptr()), C.byref(bs), C.byref(bi), C.byref(bl),
+        C.byref(cnt)), 'dfb_debug_acq')
+    return types.SimpleNamespace(sd=sd, scores=scores, score=bs.value, index=bi.value, best_lb=bl.value, count=cnt.value)
+
+  def debug_selfcheck(self, s8, err, s64):
+    """ dfb_debug_selfcheck (a test hook): (violations, scaled ratio) of the int8 pass's self-check on CUDA float64
+    vectors of equal length. """
+    n = int(s8.shape[0])
+    for t in (s8, err, s64):
+      assert t.dtype == torch.float64 and t.is_cuda and t.is_contiguous() and int(t.shape[0]) == n
+    out = (C.c_int32 * 2)()
+    torch.cuda.synchronize(s8.device)
+    _lib.check(self.lib.dfb_debug_selfcheck(self.h, C.c_void_p(s8.data_ptr()), C.c_void_p(err.data_ptr()),
+                                            C.c_void_p(s64.data_ptr()), n, out), 'dfb_debug_selfcheck')
+    return int(out[0]), int(out[1])
+
+  def debug_buffer(self, name, dtype, count):
+    """ dfb_debug_copy (a test hook): the internal buffer `name` of count elements of dtype, as a CUDA tensor. """
+    out = torch.empty((int(count),), dtype=dtype, device=self.device)
+    torch.cuda.synchronize(self.device)
+    _lib.check(self.lib.dfb_debug_copy(self.h, name.encode('utf-8'), C.c_void_p(out.data_ptr()),
+                                       int(out.numel() * out.element_size())), 'dfb_debug_copy')
+    return out
 
   def set_option(self, name, value):
     _lib.check(self.lib.dfb_set_option(self.h, name.encode('utf-8'), int(value)), 'dfb_set_option')

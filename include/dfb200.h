@@ -467,7 +467,9 @@ int dfb_debug_score_i8(dfb_handle* h, int32_t radix256, const void* a_planes_dev
  * (npad doubles, padding included), "kssv" (k(x*, x*) of the last scored chunk, chunk doubles), "prune_ub" (query
  * "keep_cap" doubles: the bounds acq(mu_ub, sqrt(k**)) of the first screen launch of the last bound pass, one per row
  * of its first step, +inf for a PI row without one), "seed_idx" (query "seed_cap" int64: the global indices of the
- * last bound pass's seeds in row order, query "last_seed_rows" of them).  With a Thompson-
+ * last bound pass's seeds in row order, query "last_seed_rows" of them), "list_idx" (4096 int64), "list_s8" and
+ * "list_err" (4096 doubles each): the shortlist of the last int8 pass or dfb_debug_acq -- global index, int8 score and
+ * allowance (-1: always kept) of its first min(count, 4096) entries in append order.  With a Thompson-
  * sampling workspace (dfb_set_ts_workspace; mbp = its mb rounded up to 128, and q = the last block's m rounded up to
  * 128, whose data sits at the start of each buffer with leading dimension q): "ts_Cov" (mbp^2 doubles: the padded
  * posterior covariance of the last dfb_eval_covar / dfb_ts_draws block, q x q; dfb_ts_draws writes its lower tiles
@@ -489,6 +491,27 @@ int dfb_debug_approx_error(dfb_handle* h, int32_t which, double* out_host);
  * the 1-based index of the first pivot that is not > 0, in which case nothing but the copy is written.  Synchronises. */
 int dfb_debug_chol_diag(dfb_handle* h, int32_t which, const double* blk_dev, int64_t ld, double* out_blk_dev,
                         double* out_dinv_dev, int32_t* info_host);
+/* Diagnostics (tests/test_gpu_acq_exact.py), not on the product path: the acquisition epilogue of dfb_score_argmax's
+ * int8 pass on caller vectors, chunk by chunk of the handle's chunk size.  Per chunk: the acquisition kernel (acq->kind
+ * UCB, EI, PI, TTEI or DFB_ACQ_TS_MARGINAL) with sd_i = sqrt(kss_i - ((partial[0][i] + partial[1][i]) + ...)) over
+ * nrb rows of partial_dev (leading dimension ld_partial >= m; nrb = 0: sd_i = sqrt(kss_i)), the block arg-max and,
+ * when b2 > 0, the running best_lb = max(best_lb, s_i - E_i) with the allowance E_i of the error model (b2, sens;
+ * sens < 0: the sensitivity dfb_score_argmax uses for acq->kind; TS: sens = |z_i| whatever is passed); the merge into the running (score, index, best_lb); then the shortlist of the chunk against that
+ * best_lb with slack pad (read back with dfb_debug_copy "list_idx", "list_s8", "list_err").  z_dev (TS, m values) may
+ * be NULL: then z_i = element (0, i) of dfb_fill_rng(seed, ...).  best_lb is the initial value of the running bound.
+ * sd_dev and scores_dev (m each) receive sd and the scores; a chunk after the shortlist overflowed (count > 4096)
+ * writes nothing, as in dfb_score_argmax.  Returns the running (score, index), best_lb and the shortlist count.
+ * Synchronises. */
+int dfb_debug_acq(dfb_handle* h, const dfb_acq_desc* acq, const double* mu_dev, const double* partial_dev,
+                  int64_t ld_partial, int32_t nrb, const double* kss_dev, int64_t m, const double* z_dev, uint64_t seed,
+                  double b2, double sens, double pad, double best_lb, double* sd_dev, double* scores_dev,
+                  double* best_score_host, int64_t* best_index_host, double* best_lb_host, int32_t* count_host);
+/* Diagnostics: the self-check of dfb_score_argmax's int8 pass on caller vectors of count entries -- int8 scores s8,
+ * allowances err (< 0: not checked) and exact scores s64.  out_host[0] = the violations it counts, out_host[1] = the
+ * largest |s8 - s64| / err, scaled by 1e6 and capped at 1e9 (query "last_selfcheck_ratio" before scaling).
+ * Synchronises. */
+int dfb_debug_selfcheck(dfb_handle* h, const double* s8_dev, const double* err_dev, const double* s64_dev, int32_t count,
+                        int32_t* out_host);
 
 /* Tuning switches.
  *  "gemm_impl"  : 0 = cp.async-ring DMMA kernel, 1 = TMA + mbarrier warp-specialised DMMA kernel for the
