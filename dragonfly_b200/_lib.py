@@ -74,6 +74,17 @@ class GaDesc(C.Structure):
               ('lut', C.c_double * DFB_GA_MAX_LUT)]
 
 
+DFB_CONS_MAX_OPS, DFB_CONS_MAX_STACK, DFB_CONS_MAX_TAB, DFB_CONS_MAX_VEC = 128, 16, 64, 16
+DFB_CONS_REJECT, DFB_CONS_ACCEPT, DFB_CONS_UNDECIDED = 0, 1, 2
+
+
+class ConsProg(C.Structure):
+  _fields_ = [('n_ops', C.c_int32), ('n_tab', C.c_int32), ('n_cols', C.c_int32), ('reserved', C.c_int32),
+              ('op', C.c_int32 * DFB_CONS_MAX_OPS), ('arg', C.c_int32 * DFB_CONS_MAX_OPS),
+              ('arg2', C.c_int32 * DFB_CONS_MAX_OPS), ('val', C.c_double * DFB_CONS_MAX_OPS),
+              ('tab_key', C.c_double * DFB_CONS_MAX_TAB), ('tab_val', C.c_double * DFB_CONS_MAX_TAB)]
+
+
 PROTOTYPES = {
   'dfb_version': (C.c_int, []),
   'dfb_last_error': (C.c_char_p, []),
@@ -122,6 +133,8 @@ PROTOTYPES = {
   'dfb_fill_candidates': (C.c_int, [_P, C.c_uint64, _I64, _I64, _I32, C.POINTER(_D), C.POINTER(_D), _P]),
   'dfb_fill_mixed_candidates': (C.c_int, [_P, C.c_uint64, _I64, _I64, _I32, C.POINTER(_I32), C.POINTER(_D),
                                           C.POINTER(_D), C.POINTER(_I64), _P]),
+  'dfb_constraint_status': (C.c_int, [_P, C.POINTER(ConsProg), _P, _I64, _I64, _P, C.POINTER(_I64)]),
+  'dfb_compact_rows': (C.c_int, [_P, _P, _I64, _I32, _I64, _P, _I32, _I64, _P, _P, C.POINTER(_I64)]),
   'dfb_measure_peak': (C.c_int, [C.c_int, C.c_int, C.POINTER(_D)]),
   'dfb_launch_count': (_I64, [_P]),
   'dfb_debug_score_i8': (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _P, _D, _P, _P, _I64]),

@@ -2171,6 +2171,72 @@ int dfb_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_
   return launch_fill_mixed_candidates(h, seed, row0, m, d, kinds_host, lo_host, hi_host, n_levels_host, out_dev);
 }
 
+// The program's shape, checked on the host: every op reads columns and table entries in range and keeps the stack within
+// DFB_CONS_MAX_STACK; booleans and numbers are not told apart here (the compiler types them).
+static bool cons_prog_ok(const dfb_cons_prog* p, int64_t ld) {
+  if (p->n_ops < 0 || p->n_ops > DFB_CONS_MAX_OPS || p->n_tab < 0 || p->n_tab > DFB_CONS_MAX_TAB || p->n_cols < 1 ||
+      p->n_cols > ld)
+    return false;
+  int sp = 0;
+  for (int k = 0; k < p->n_ops; k++) {
+    const int op = p->op[k], arg = p->arg[k];
+    int pop = 2, push = 1;
+    switch (op) {
+      case DFB_CONS_OP_COL:
+      case DFB_CONS_OP_LOOKUP:
+        if (arg < 0 || arg >= p->n_cols) return false;
+        if (op == DFB_CONS_OP_LOOKUP) {
+          const double n = p->val[k];
+          if (!(n >= 1.0 && n <= DFB_CONS_MAX_TAB) || n != (double)(int)n || p->arg2[k] < 0 ||
+              p->arg2[k] + (int)n > p->n_tab)
+            return false;
+        }
+        pop = 0; break;
+      case DFB_CONS_OP_CONST: pop = 0; break;
+      case DFB_CONS_OP_NEG: case DFB_CONS_OP_ABS: case DFB_CONS_OP_SQRT: case DFB_CONS_OP_EXP: case DFB_CONS_OP_LOG:
+      case DFB_CONS_OP_NOT:
+        pop = 1; break;
+      case DFB_CONS_OP_POW: if (arg < 0 || arg > 8) return false; pop = 1; break;
+      case DFB_CONS_OP_NPSUM: case DFB_CONS_OP_NORM:
+        if (arg < 1 || arg > DFB_CONS_MAX_VEC) return false;
+        pop = arg; break;
+      case DFB_CONS_OP_ACCEPT: pop = 1; push = 0; break;
+      default:
+        if (op < 0 || op >= DFB_CONS_N_OPS) return false;
+        break;                                                        // binary ops
+    }
+    if (sp < pop) return false;
+    sp += push - pop;
+    if (sp > DFB_CONS_MAX_STACK) return false;
+  }
+  return sp == 0;
+}
+
+int dfb_constraint_status(dfb_handle* h, const dfb_cons_prog* prog, const double* rows_dev, int64_t m, int64_t ld,
+                          uint8_t* status_dev, int64_t* counts_host) {
+  DFB_TRY(need(h, false, false, false, false, false));
+  if (prog == nullptr || counts_host == nullptr || m < 0 || (m > 0 && (rows_dev == nullptr || status_dev == nullptr)) ||
+      !cons_prog_ok(prog, ld)) {
+    set_error("bad constraint_status arguments (m = %lld, ld = %lld, or a malformed program)", (long long)m,
+              (long long)ld);
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  return launch_constraint_status(h, *prog, rows_dev, m, ld, status_dev, counts_host);
+}
+
+int dfb_compact_rows(dfb_handle* h, const double* rows_dev, int64_t m, int32_t d, int64_t ld, const uint8_t* status_dev,
+                     int32_t keep, int64_t idx_base, double* out_rows_dev, int64_t* out_idx_dev, int64_t* count_host) {
+  DFB_TRY(need(h, false, false, false, false, false));
+  if (count_host == nullptr || m < 0 || d < 1 || ld < d || idx_base < 0 || keep < 0 || keep > 255 ||
+      (m > 0 && (rows_dev == nullptr || status_dev == nullptr || out_rows_dev == nullptr || out_idx_dev == nullptr))) {
+    set_error("bad compact_rows arguments (m = %lld, d = %d, ld = %lld)", (long long)m, d, (long long)ld);
+    return -1;
+  }
+  DFB_CUDA_OK(cudaSetDevice(h->device));
+  return launch_compact_rows(h, rows_dev, m, d, ld, status_dev, keep, idx_base, out_rows_dev, out_idx_dev, count_host);
+}
+
 int dfb_ts_argmax(dfb_handle* h, const double* samples_dev, int64_t ld, int32_t S, int64_t m, int64_t idx_base,
                   int32_t reset, double* best_dev, int64_t* index_dev) {
   DFB_TRY(need(h, false, false, false, false, false));

@@ -151,4 +151,11 @@ int64_t lml_batch_item_doubles(int64_t npad, int ns, int nf);
 // hamming: launch the instantiation that evaluates HAMMING factors (dfb_lml_batch_mixed); without, the Euclidean one
 int launch_lml_batch(dfb_handle* h, const LmlBatchArgs& g, int B, bool hamming);
 
+// certified constraint filter of Cartesian-product candidates (dfb_constraint_status) and the order-preserving
+// compaction of the rows it keeps (dfb_compact_rows)
+int launch_constraint_status(dfb_handle* h, const dfb_cons_prog& p, const double* rows, int64_t m, int64_t ld,
+                             uint8_t* status, int64_t* counts_host);
+int launch_compact_rows(dfb_handle* h, const double* rows, int64_t m, int d, int64_t ld, const uint8_t* status, int keep,
+                        int64_t idx_base, double* out_rows, int64_t* out_idx, int64_t* count_host);
+
 }  // namespace dfb

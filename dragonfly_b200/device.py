@@ -437,6 +437,36 @@ class DevicePosterior(object):
         C.c_void_p(out.data_ptr())), 'dfb_fill_mixed_candidates')
     return out
 
+  def constraint_status(self, prog, rows, status=None):
+    """ dfb_constraint_status: one DFB_CONS_* byte per row of the m x d CUDA tensor rows under the dfb_cons_prog prog.
+        Returns (status, a uint8 CUDA tensor of m, [rejected, accepted, undecided] counts). """
+    rows = rows.contiguous()
+    m = int(rows.shape[0])
+    if status is None:
+      status = torch.empty((m,), dtype=torch.uint8, device=self.device)
+    counts = (C.c_int64 * 3)()
+    _lib.check(self.lib.dfb_constraint_status(self.h, C.byref(prog), C.c_void_p(rows.data_ptr()), m,
+                                              int(rows.shape[1]) if rows.dim() == 2 else 0,
+                                              C.c_void_p(status.data_ptr()), counts), 'dfb_constraint_status')
+    return status, [int(c) for c in counts]
+
+  def compact_rows(self, rows, status, keep=_lib.DFB_CONS_ACCEPT, idx_base=0, out_rows=None, out_idx=None):
+    """ dfb_compact_rows: the rows of the m x d CUDA tensor rows whose status byte equals keep, in order, with their
+        indices idx_base + i.  Returns (rows, indices) views of the count kept; out_rows / out_idx (m x d / m, or
+        larger) receive them when given. """
+    rows = rows.contiguous()
+    m, d = int(rows.shape[0]), int(rows.shape[1])
+    if out_rows is None:
+      out_rows = torch.empty((m, d), dtype=torch.float64, device=self.device)
+    if out_idx is None:
+      out_idx = torch.empty((m,), dtype=torch.int64, device=self.device)
+    count = C.c_int64(0)
+    _lib.check(self.lib.dfb_compact_rows(self.h, C.c_void_p(rows.data_ptr()), m, d, d, C.c_void_p(status.data_ptr()),
+                                         int(keep), int(idx_base), C.c_void_p(out_rows.data_ptr()),
+                                         C.c_void_p(out_idx.data_ptr()), C.byref(count)), 'dfb_compact_rows')
+    n = int(count.value)
+    return out_rows.view(-1)[:n * d].view(n, d), out_idx[:n]
+
   def ga_maximise(self, acq_desc, mean_const, ga_desc, seed, n_init, n_total):
     """ dfb_ga_maximise: the whole GA search on the device.  Returns (best value, best index, best level row, the
         n_total x d level rows, the n_total values), the last two CUDA tensors. """

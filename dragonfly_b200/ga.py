@@ -80,6 +80,21 @@ def draw_cp_initial_pool(parts, num_samples):
   return [[c[i] for c in cols] for i in range(n)]
 
 
+def draw_constrained_pool(parts, domain, num_samples):
+  """ get_cp_domain_initial_qinfos on a constrained domain (exd_utils.py:129-148): sample_from_cp_domain
+      (cp_domain_utils.py:401-444) with latin_hc, i.e. at most 10 rounds of draw_cp_initial_pool -- max(10, 2n) points,
+      then 2n -- each filtered by the domain's own constraints_are_satisfied, truncated to n once n are kept.  Fewer
+      than n come back when ten rounds do not find them, as in the reference. """
+  n = int(num_samples)
+  ret, n_draw = [], max(10, 2 * n)
+  for _ in range(10):
+    ret.extend(pt for pt in draw_cp_initial_pool(parts, n_draw) if domain.constraints_are_satisfied(pt))
+    if len(ret) >= n:
+      return ret[:n]
+    n_draw = 2 * n
+  return ret
+
+
 # ---------------------------------------------------------------------------------------------
 # Domain membership (domains.py:90-131, 271-318, 418-428) and the mutation operators (cp_ga_optimiser.py:27-121)
 # ---------------------------------------------------------------------------------------------
@@ -101,8 +116,12 @@ def _part_is_member(p, x):
   return all(isinstance(v, Number) and any(abs(v - e) < 1e-8 for e in loi) for v, loi in zip(x, p.levels))
 
 
-def is_a_member(parts, pt):
-  return hasattr(pt, '__iter__') and len(pt) == len(parts) and all(_part_is_member(p, x) for p, x in zip(parts, pt))
+def is_a_member(parts, pt, domain=None):
+  """ CartesianProductDomain.is_a_member (domains.py:418-428): every part's membership, then, for a constrained domain,
+      the domain's own constraints_are_satisfied. """
+  if not (hasattr(pt, '__iter__') and len(pt) == len(parts) and all(_part_is_member(p, x) for p, x in zip(parts, pt))):
+    return False
+  return domain is None or bool(domain.constraints_are_satisfied(pt))
 
 
 def _gauss_perturbation(x, bounds):
@@ -143,9 +162,10 @@ def sample_parents(vals, num):
   return np.random.choice(len(vals), num, p=probs, replace=True)
 
 
-def mutation_epoch(parts, points, vals):
+def mutation_epoch(parts, points, vals, domain=None):
   """ GAOptimiser.generate_new_eval_points with CPGAOptimiser._mutation_op (ga_optimiser.py:97-132,
-      cp_ga_optimiser.py:159-183): the new points to evaluate, in order. """
+      cp_ga_optimiser.py:159-183): the new points to evaluate, in order.  domain: a constrained domain whose constraints
+      filter the mutations too. """
   num_tries, k = 0, NUM_MUTATIONS_PER_EPOCH
   while True:
     num_tries += 1
@@ -155,7 +175,7 @@ def mutation_epoch(parts, points, vals):
       for _ in range(int(counts[idx])):
         ret.append([mutate_part(p, x) for p, x in zip(parts, points[idx])])
     np.random.shuffle(ret)
-    members = [pt for pt in ret if is_a_member(parts, pt)]
+    members = [pt for pt in ret if (is_a_member(parts, pt) if domain is None else is_a_member(parts, pt, domain))]
     if members:
       return members
     if num_tries >= MAX_TRIES:
@@ -179,20 +199,22 @@ def ga_budget(parts, max_evals):
   return cap, n_pool, max(n_pool, int(np.ceil(float(max_evals))) + 1)
 
 
-def ga_maximise(score, parts, max_evals, log=None):
+def ga_maximise(score, parts, max_evals, log=None, domain=None):
   """ The reference's CP GA with score(list of points) -> their values (one call per batch).  Returns (max_val,
-      max_pt); log, when a list, receives (points, values) of every scored batch in order. """
+      max_pt); log, when a list, receives (points, values) of every scored batch in order.  domain: a constrained
+      domain -- the initial pool is its constrained draw and its constraints filter the mutations. """
   cap, n_pool, n_total = ga_budget(parts, max_evals)
   pool = []
   while len(pool) <= n_pool:           # the loop pops one point more than it dispatches, then sees the capital spent
-    pool.extend(draw_cp_initial_pool(parts, int(cap)))
+    pool.extend(draw_cp_initial_pool(parts, int(cap)) if domain is None else
+                draw_constrained_pool(parts, domain, int(cap)))
   pool = pool[:n_pool]
   points, vals = [], np.zeros((0,))
 
   def evaluate(batch):
     nonlocal vals
     for pt in batch:
-      assert is_a_member(parts, pt)
+      assert is_a_member(parts, pt) if domain is None else is_a_member(parts, pt, domain)
     v = np.asarray(score(batch), dtype=np.float64).reshape(-1)
     if log is not None:
       log.append((batch, v))
@@ -201,7 +223,7 @@ def ga_maximise(score, parts, max_evals, log=None):
 
   evaluate(pool)
   while len(points) < n_total:
-    evaluate(mutation_epoch(parts, points, vals)[:n_total - len(points)])
+    evaluate(mutation_epoch(parts, points, vals, domain)[:n_total - len(points)])
   ok = np.flatnonzero(vals == np.nanmax(vals)) if not np.all(np.isnan(vals)) else []
   if len(ok) == 0:
     return -np.inf, None
@@ -245,11 +267,16 @@ def ga_follow_up(score, parts, ga_val, ga_pt, method, max_evals):
   return ga_val, ga_pt
 
 
-def maximise(score, parts, method, max_evals, log=None, search=None):
-  """ maximise_with_method_on_cp_domain for method 'ga' or 'ga-<method>': returns the point.  log: see ga_maximise.
-      search() -> (max_val, max_pt) replaces the parity GA (the device GA of device_search). """
+def maximise(score, parts, method, max_evals, log=None, search=None, domain=None):
+  """ maximise_with_method_on_cp_domain for method 'ga' or 'ga-<method>': returns the point.  log, domain: see
+      ga_maximise.  search() -> (max_val, max_pt) replaces the parity GA (the device GA of device_search).  The
+      follow-up over the Euclidean parts ignores the constraints, as the reference's does. """
   names = str(method).lower().split('-')
-  val, pt = ga_maximise(score, parts, max_evals, log) if search is None else search()
+  if search is not None:
+    val, pt = search()
+  else:
+    val, pt = ga_maximise(score, parts, max_evals, log) if domain is None else \
+        ga_maximise(score, parts, max_evals, log, domain=domain)
   if len(names) == 2 and any(p.type == 'euclidean' for p in parts):
     val, pt = ga_follow_up(score, parts, val, pt, names[1], max_evals)
   return pt

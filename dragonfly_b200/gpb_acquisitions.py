@@ -62,13 +62,14 @@ class _CPPart(object):
 
 
 def _cp_parts(domain, kernel=None):
-  """ The parts of a CP domain in domain order; raises for what the device does not serve (constraints, NN and
-      discrete-Euclidean parts, nested CP domains).  kernel None: the parts without Hamming tables (and without checking
+  """ The parts of a CP domain in domain order; raises for what the device does not serve (constraints it cannot read,
+      NN and discrete-Euclidean parts, nested CP domains).  kernel None: the parts without Hamming tables (and without checking
       the GP's kernel against the domain). """
   from .kernel import category_codes, _kind_of
-  has_constraints = getattr(domain, 'has_constraints', None)
-  if has_constraints is not None and has_constraints():
-    raise NotImplementedError('Constrained Cartesian-product domains are outside the GPU hot-path scope.')
+  from .constraints import readable
+  if _has_constraints(domain) and not readable(domain):
+    raise NotImplementedError('A constrained Cartesian-product domain needs its constraint list, raw name ordering, '
+                              'get_raw_point and constraints_are_satisfied to be served on the GPU.')
   kernel_list = getattr(kernel, 'kernel_list', None) if kernel is not None else [None] * len(domain.list_of_domains)
   if kernel_list is None or len(kernel_list) != len(domain.list_of_domains):
     raise NotImplementedError('A Cartesian-product domain needs a CPGP whose kernel has one factor per part.')
@@ -93,6 +94,11 @@ def _cp_parts(domain, kernel=None):
       raise NotImplementedError("Domain parts of type '%s' are outside the GPU hot-path scope." % (p.type))
     parts.append(p)
   return parts
+
+
+def _has_constraints(domain):
+  has_constraints = getattr(domain, 'has_constraints', None)
+  return has_constraints is not None and bool(has_constraints())
 
 
 def _level_columns(p, level_values):
@@ -201,12 +207,15 @@ def _cp_point_from_device_row(parts, row):
   return pt
 
 
-def _cp_candidate_source(post, slab_rows, parts, M, mode, levels=False):
+def _cp_candidate_source(post, slab_rows, parts, M, mode, levels=False, domain=None):
   """ The M candidates of the `rand` maximiser on a CP domain as an _IndexedRows, and the seed of the device's candidates
       (None in 'numpy' mode).  'numpy' draws the reference's points (draw_cp_candidates) in host slabs of
       slab_rows(STREAM_SLAB_ROWS) rows; 'device' generates them with dfb_fill_mixed_candidates on `post`, keyed by (seed,
       global row, column), in slabs of slab_rows(2 STREAM_SLAB_ROWS).  levels: category columns hold level indices
-      instead of the parts' column values (_encode_levels maps them). """
+      instead of the parts' column values (_encode_levels maps them).  A constrained domain's candidates are the rows
+      its constraints keep (_constrained_source); their number, source.hi, may then differ from M. """
+  if domain is not None and _has_constraints(domain):
+    return _constrained_source(post, slab_rows, parts, M, mode, levels, domain)
   if mode == 'device':
     seed = _device_seed()
     kinds, bounds, n_levels, luts = _cp_device_layout(parts)
@@ -217,8 +226,129 @@ def _cp_candidate_source(post, slab_rows, parts, M, mode, levels=False):
             parts, post.fill_mixed_candidates(seed, i, 1, kinds, bounds, n_levels).cpu().numpy()[0])), seed
   rows, draws = draw_cp_candidates(parts, M)
   if levels:
-    rows = np.ascontiguousarray(np.concatenate([np.asarray(d, dtype=np.float64) for d in draws], axis=1))
+    rows = _level_rows(draws)
   return _IndexedRows(slab_rows(STREAM_SLAB_ROWS), 0, M, lambda r0, m, out: rows[r0:r0 + m],
+                      lambda i: point_from_draws(parts, draws, i)), None
+
+
+def _level_rows(draws):
+  return np.ascontiguousarray(np.concatenate([np.asarray(d, dtype=np.float64) for d in draws], axis=1))
+
+
+# ---------------------------------------------------------------------------------------------
+# Constrained CP domains: the reference's constrained draw (cp_domain_utils.py:401-444) filtered on the device by the
+# compiled constraints (constraints.py), undecided and residue rows settled on the host by the domain's own evaluator
+# ---------------------------------------------------------------------------------------------
+MAX_CONSTRAINED_TRIES = 10
+
+
+def constrained_rand_draw(parts, M, keep_round):
+  """ The candidates of _rand_maximise_vectorised_objective_in_cp_domain (exd_utils.py:247-274) on a constrained domain:
+      calls of sample_from_cp_domain(domain, M) (cp_domain_utils.py:401-444) until M points are kept, or some are and
+      five calls are spent -- so more than M may be kept.  A call draws at most 10 rounds, max(10, 2M) rows first and 2M
+      after (draw_cp_candidates, the reference's MT19937 consumption), keeps each round's accepted rows in order and
+      stops, truncated to M, once M are kept.  keep_round(rows, draws, need) -> (chunk, k) keeps the first k <= need
+      accepted rows of a round.  Where the reference would draw forever because nothing is ever accepted, this warns
+      as it does at the 10th empty call and raises ValueError.  Returns (chunks, number kept). """
+  from warnings import warn
+  chunks, total, tries = [], 0, 0
+  while not (total >= M or (total > 0 and tries >= 5)):
+    got = constrained_sample(parts, M, keep_round, chunks)
+    total += got
+    tries += 1
+    if total == 0 and tries % MAX_CONSTRAINED_TRIES == 0:
+      warn(('Sampling from domain failed despite %d attempts -- will continue trying but consider reparametrising '
+            'your domain if this problem persists.') % (tries))
+      raise ValueError('No point of the constrained domain was accepted in %d calls of %d draws.' % (tries, 20 * M))
+  return chunks, total
+
+
+def constrained_sample(parts, M, keep_round, chunks):
+  """ One sample_from_cp_domain(domain, M) call of constrained_rand_draw: appends its kept chunks, returns their count. """
+  got, n_draw = 0, max(10, 2 * M)
+  for _ in range(10):
+    rows, draws = draw_cp_candidates(parts, n_draw)
+    chunk, k = keep_round(rows, draws, M - got)
+    if k > 0:
+      chunks.append(chunk)
+    got += k
+    if got >= M:
+      break
+    n_draw = 2 * M
+  return got
+
+
+def _constrained_source(post, slab_rows, parts, M, mode, levels, domain):
+  """ _cp_candidate_source on a constrained domain.  'numpy': constrained_rand_draw, each round uploaded once, given a
+      status per row by dfb_constraint_status, its undecided (and, with residue constraints, accepted) rows settled on
+      the host through point_from_draws, and compacted on the device (dfb_compact_rows).  'device': the first M accepted
+      rows of the device's candidate stream in row order, scanned block by block until M are found or the rows the
+      reference's five calls could draw at most are spent; ValueError when none is accepted. """
+  import torch
+  from .constraints import compile_filter
+  filt = compile_filter(domain, parts, levels=levels)
+  prog = filt.desc()
+  dev = post.device
+
+  def status_of(rows_dev, point_of, need):
+    """ The rows' statuses, the host's share settled in row order up to the first `need` accepted rows. """
+    status, counts = post.constraint_status(prog, rows_dev)
+    if counts[2] > 0 or (filt.residue and counts[1] > 0):
+      status.copy_(torch.from_numpy(filt.settle(status.cpu().numpy(), point_of, need)))
+    return status
+
+  if mode == 'device':
+    seed = _device_seed()
+    kinds, bounds, n_levels, luts = _cp_device_layout(parts)
+    block = slab_rows(2 * STREAM_SLAB_ROWS)
+    cap = 5 * (max(10, 2 * M) + 9 * 2 * M)
+    kept = torch.empty((M, len(kinds)), dtype=torch.float64, device=dev)
+    kept_idx = torch.empty((M,), dtype=torch.int64, device=dev)
+    got, r0, lv, coded = 0, 0, None, None
+    while got < M and r0 < cap:
+      m = min(block, cap - r0)
+      lv = post.fill_mixed_candidates(seed, r0, m, kinds, bounds, n_levels, out=None if lv is None else lv[:m])
+      rows = lv if levels else _encode_levels(torch.clone(lv) if coded is None else coded[:m].copy_(lv), luts)
+      coded = None if levels else rows
+      host_rows = {}
+
+      def point_of(i, lv=lv):
+        if not host_rows:              # the level rows the host may need, copied once per block
+          st = status_now[0]
+          idx = filt.host_rows(st)
+          host_rows['idx'] = idx
+          host_rows['rows'] = lv[torch.from_numpy(idx).to(dev)].cpu().numpy()
+        k = int(np.searchsorted(host_rows['idx'], i))
+        return _cp_point_from_device_row(parts, host_rows['rows'][k])
+      status_now = [None]
+      status, counts = post.constraint_status(prog, rows)
+      if counts[2] > 0 or (filt.residue and counts[1] > 0):
+        status_now[0] = status.cpu().numpy()
+        status.copy_(torch.from_numpy(filt.settle(status_now[0], point_of, M - got)))
+      rows_k, idx_k = post.compact_rows(rows, status, idx_base=r0)
+      take = min(int(rows_k.shape[0]), M - got)
+      kept[got:got + take] = rows_k[:take]
+      kept_idx[got:got + take] = idx_k[:take]
+      got += take
+      r0 += m
+    if got == 0:
+      raise ValueError('No point of the constrained domain was accepted in %d device draws.' % (r0))
+    return _IndexedRows(block, 0, got, lambda a, m, out: kept[a:a + m], lambda i: _cp_point_from_device_row(
+        parts, post.fill_mixed_candidates(seed, int(kept_idx[i]), 1, kinds, bounds, n_levels).cpu().numpy()[0])), seed
+
+  def keep_round(rows, draws, need):
+    X = _level_rows(draws) if levels else rows
+    rows_dev = torch.from_numpy(np.ascontiguousarray(X)).to(dev)
+    status = status_of(rows_dev, lambda i: point_from_draws(parts, draws, i), need)
+    rows_k, idx_k = post.compact_rows(rows_dev, status)
+    k = min(int(rows_k.shape[0]), need)
+    sel = idx_k[:k].cpu().numpy()
+    return (rows_k[:k].clone(), [d[sel] for d in draws]), k
+
+  chunks, total = constrained_rand_draw(parts, M, keep_round)
+  kept = torch.cat([c[0] for c in chunks]) if len(chunks) > 1 else chunks[0][0]
+  draws = [np.concatenate([c[1][j] for c in chunks]) for j in range(len(parts))]
+  return _IndexedRows(slab_rows(STREAM_SLAB_ROWS), 0, total, lambda a, m, out: kept[a:a + m],
                       lambda i: point_from_draws(parts, draws, i)), None
 
 
@@ -235,10 +365,10 @@ def _cp_fused_maximise(gp, anc_data, acq):
   mode = _candidate_rng(anc_data)
   M = int(anc_data.max_evals)
   with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
-    source, seed = _cp_candidate_source(sess.post, sess.slab_rows, parts, M, mode)
+    source, seed = _cp_candidate_source(sess.post, sess.slab_rows, parts, M, mode, domain=anc_data.domain)
     if acq is not None:
       return source.point(*_slab_argmax(source, lambda pts, r0: sess.score(pts)))
-    z = np.random.normal(size=M) if mode == 'numpy' else None
+    z = np.random.normal(size=source.hi) if mode == 'numpy' else None
     nonpos = 0
 
     def score_ts(pts, r0):
@@ -280,15 +410,20 @@ def _cp_other_maximiser(acq_fn, anc_data, gp=None, acq=None):
   if method.startswith('ga'):
     from . import ga
     parts = _cp_parts(anc_data.domain, None if gp is None else gp.kernel)
+    constrained = anc_data.domain if _has_constraints(anc_data.domain) else None
+    cons_kw = {} if constrained is None else {'domain': constrained}
     if _shard_info()[1] > 1:
       raise NotImplementedError('The GA maximiser of Cartesian-product domains is not sharded across ranks.')
     if gp is None or acq is None:
-      return ga.maximise(acq_fn, parts, method, anc_data.max_evals)
+      return ga.maximise(acq_fn, parts, method, anc_data.max_evals, **cons_kw)
+    if constrained is not None and _candidate_rng(anc_data) == 'device':
+      raise NotImplementedError("The device GA (candidate_rng='device') does not serve constrained Cartesian-product "
+                                "domains; use candidate_rng='numpy' or acq_opt_method 'rand'.")
     seed = _device_seed() if _candidate_rng(anc_data) == 'device' else None
     with gp._fused_session(acq, _halluc_points(anc_data)) as sess:
       search = None if seed is None else (lambda: ga.device_search(sess, parts, anc_data.max_evals, seed))
       return ga.maximise(lambda pts: sess.score(pts, want_scores=True)[2], parts, method, anc_data.max_evals,
-                         search=search)
+                         search=search, **cons_kw)
   raise NotImplementedError("acq_opt_method '%s' is not served on Cartesian-product domains; use 'rand'."
                             % (anc_data.acq_opt_method))
 

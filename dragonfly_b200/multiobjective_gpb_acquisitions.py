@@ -144,8 +144,9 @@ def _mo_cp(kind, gps, anc_data, weights, refs, beta_th=0.0):
   with ExitStack() as stack:
     sessions = [stack.enter_context(gp._fused_session(None, halluc)) for gp in gps]
     posts = [sess.post for sess in sessions]
-    source, seed = _cp_candidate_source(posts[0], sessions[0].slab_rows, parts[0], M, mode, levels=True)
-    z = np.random.normal(size=(M, K)) if ts and mode == 'numpy' else None
+    source, seed = _cp_candidate_source(posts[0], sessions[0].slab_rows, parts[0], M, mode, levels=True,
+                                        domain=anc_data.domain)
+    z = np.random.normal(size=(source.hi, K)) if ts and mode == 'numpy' else None
     nonpos = 0
 
     def score(pts, r0):

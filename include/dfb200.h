@@ -390,6 +390,70 @@ int dfb_fill_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, i
 int dfb_fill_mixed_candidates(dfb_handle* h, uint64_t seed, int64_t row0, int64_t m, int32_t d, const int32_t* kinds_host,
                               const double* lo_host, const double* hi_host, const int64_t* n_levels_host, double* out_dev);
 
+/* Domain constraints of a Cartesian-product domain as a certified stack program (dragonfly_b200/constraints.py
+ * compiles it; tests/constraint_ref.py is its NumPy oracle).  Each stack entry is a value and a radius bounding the
+ * distance to NumPy's value of the same expression (radius +inf: unknown); boolean entries hold 0 (false), 1 (true) or
+ * 2 (undecided).  Ops, with arg / arg2 / val:
+ *   COL c; CONST val; LOOKUP column arg, entries [arg2, arg2 + val) of tab_key / tab_val (first equal key; none: unknown)
+ *   ADD SUB MUL DIV (arg 1: integer operands, unknown unless |result| < 2^53), NEG, ABS, SQRT, EXP, LOG,
+ *   POW exponent arg in 0..8 (arg2 1: integer), MIN MAX (Python's builtin, first operand kept on ties),
+ *   NPSUM n / NORM n (pop n entries: np.sum / np.linalg.norm of them), LT LE GT GE EQ NE, AND OR NOT (three-valued),
+ *   ACCEPT (pop a boolean and fold it into the row's status: any 0 rejects, else any 2 leaves it undecided).
+ * Every arithmetic step is round-to-nearest without contraction, radii are formed in the same order by the oracle. */
+#define DFB_CONS_MAX_OPS   128
+#define DFB_CONS_MAX_STACK 16
+#define DFB_CONS_MAX_TAB   64
+#define DFB_CONS_MAX_VEC   16
+#define DFB_CONS_OP_COL     0
+#define DFB_CONS_OP_CONST   1
+#define DFB_CONS_OP_LOOKUP  2
+#define DFB_CONS_OP_ADD     3
+#define DFB_CONS_OP_SUB     4
+#define DFB_CONS_OP_MUL     5
+#define DFB_CONS_OP_DIV     6
+#define DFB_CONS_OP_NEG     7
+#define DFB_CONS_OP_ABS     8
+#define DFB_CONS_OP_SQRT    9
+#define DFB_CONS_OP_EXP     10
+#define DFB_CONS_OP_LOG     11
+#define DFB_CONS_OP_POW     12
+#define DFB_CONS_OP_MIN     13
+#define DFB_CONS_OP_MAX     14
+#define DFB_CONS_OP_NPSUM   15
+#define DFB_CONS_OP_NORM    16
+#define DFB_CONS_OP_LT      17
+#define DFB_CONS_OP_LE      18
+#define DFB_CONS_OP_GT      19
+#define DFB_CONS_OP_GE      20
+#define DFB_CONS_OP_EQ      21
+#define DFB_CONS_OP_NE      22
+#define DFB_CONS_OP_AND     23
+#define DFB_CONS_OP_OR      24
+#define DFB_CONS_OP_NOT     25
+#define DFB_CONS_OP_ACCEPT  26
+#define DFB_CONS_N_OPS    27
+#define DFB_CONS_REJECT    0
+#define DFB_CONS_ACCEPT    1
+#define DFB_CONS_UNDECIDED 2
+typedef struct {
+  int32_t n_ops, n_tab, n_cols, reserved;
+  int32_t op[DFB_CONS_MAX_OPS];
+  int32_t arg[DFB_CONS_MAX_OPS];
+  int32_t arg2[DFB_CONS_MAX_OPS];
+  double  val[DFB_CONS_MAX_OPS];
+  double  tab_key[DFB_CONS_MAX_TAB];
+  double  tab_val[DFB_CONS_MAX_TAB];
+} dfb_cons_prog;
+/* One status byte per row of rows_dev (m x n_cols, row stride ld) in status_dev (DFB_CONS_*), and in counts_host the
+ * number of rows of each status.  The program is validated here: op codes, columns < n_cols <= ld, stack depth within
+ * DFB_CONS_MAX_STACK with one entry left per ACCEPT, table ranges, exponents and vector lengths. */
+int dfb_constraint_status(dfb_handle* h, const dfb_cons_prog* prog, const double* rows_dev, int64_t m, int64_t ld,
+                          uint8_t* status_dev, int64_t* counts_host);
+/* Order-preserving compaction: the rows i of rows_dev (m x d, stride ld) with status_dev[i] == keep are written to
+ * out_rows_dev (count x d, contiguous) in row order, idx_base + i to out_idx_dev, and their number to *count_host.  */
+int dfb_compact_rows(dfb_handle* h, const double* rows_dev, int64_t m, int32_t d, int64_t ld, const uint8_t* status_dev,
+                     int32_t keep, int64_t idx_base, double* out_rows_dev, int64_t* out_idx_dev, int64_t* count_host);
+
 /* The GA acquisition maximiser of a Cartesian-product domain, resident on the device (the reference's CPGAOptimiser,
  * cp_ga_optimiser.py / ga_optimiser.py, driven by Philox instead of MT19937).  Rows are in the level form of
  * dfb_fill_mixed_candidates (categorical columns hold level indices); lut maps them to the column values the kernel
